@@ -1,8 +1,8 @@
-"""ao_b200 — B200-native quantized-linear engine with torchao's operator surface.
+"""ao_b200 — H100-native quantized-linear engine with torchao's operator surface.
 
 Drop-in for the quantized ``nn.Linear`` forward of pytorch/ao (torchao 0.19): the same
 ``quantize_`` / config / tensor-subclass API, with the kernels underneath replaced by
-hand-written sm_100a CUDA (``libao_b200.so``, C ABI in ``include/ao_b200.h``) registered as
+hand-written sm_90a CUDA (``libao_b200.so``, C ABI in ``include/ao_b200.h``) registered as
 ``torch.ops.ao_b200.*``.  There is no CPU or eager fallback for the hot path: importing this
 package without the native library raises.
 """

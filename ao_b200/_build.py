@@ -1,5 +1,5 @@
 """Build the native pieces in-tree (no JIT cache): the C-ABI CUDA library
-``ao_b200/lib/libao_b200.so`` (nvcc, sm_100a only) and the torch.library binding
+``ao_b200/lib/libao_b200.so`` (nvcc, sm_90a only) and the torch.library binding
 ``ao_b200/lib/ao_b200_torch.so`` (g++ against the installed torch headers).
 
 Run ``python -m ao_b200._build`` or call :func:`build_all`.  Nothing here needs a GPU.
@@ -16,7 +16,7 @@ CSRC = ROOT / "csrc"
 LIB = ROOT / "lib"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -64,7 +64,7 @@ def build_cuda_lib(force: bool = False, verbose: bool = False) -> Path:
             raise RuntimeError(f"nvcc failed for {src}:\n{log}")
         if verbose:
             print(log)
-    cmd = [nvcc_path(), "-shared", "-o", str(out), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc_path(), "-shared", "-o", str(out), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"nvcc link failed:\n{r.stdout}")

@@ -1,6 +1,6 @@
 """Loads the in-tree native libraries and fails loudly when they are missing.
 
-``ao_b200/lib/libao_b200.so``  — C-ABI CUDA kernels (nvcc, sm_100a)
+``ao_b200/lib/libao_b200.so``  — C-ABI CUDA kernels (nvcc, sm_90a)
 ``ao_b200/lib/ao_b200_torch.so`` — TORCH_LIBRARY(ao_b200) registration (links the above)
 Built by ``python -m ao_b200._build`` / ``__graft_entry__.build()``; never JIT-compiled.
 """
@@ -37,10 +37,10 @@ def load_native() -> None:
     _LOADED = True
 
 
-def require_sm100(device=None) -> None:
-    """Raise unless the CUDA device can run the sm_100a kernels."""
+def require_sm90(device=None) -> None:
+    """Raise unless the CUDA device can run the sm_90a kernels."""
     if not torch.cuda.is_available():
-        raise RuntimeError("ao_b200: a CUDA device (B200, sm_100) is required; none is visible")
+        raise RuntimeError("ao_b200: a CUDA device (H100, sm_90) is required; none is visible")
     major, minor = torch.cuda.get_device_capability(device)
-    if major != 10:
-        raise RuntimeError(f"ao_b200: kernels are built for sm_100a only, device is sm_{major}{minor}")
+    if (major, minor) != (9, 0):
+        raise RuntimeError(f"ao_b200: kernels are built for sm_90a only, device is sm_{major}{minor}")

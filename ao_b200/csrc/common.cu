@@ -86,43 +86,6 @@ bool pdl_enabled() {
   return v == 1;
 }
 
-bool timeline_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("AO_B200_TIMELINE");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
-
-bool prefill_disabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("AO_B200_NO_PREFILL");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
-
-int ts_flags() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("AO_B200_TS_FLAGS");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-
-int ts_ctas_per_sm() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("AO_B200_TS_CTAS_PER_SM");
-    v = e ? atoi(e) : 0;   // 0 = choose per problem size
-    if (v < 0 || v > 2) v = 0;
-  }
-  return v;
-}
-
 int ts_min_units() {
   static int v = -1;
   if (v < 0) {
@@ -133,33 +96,13 @@ int ts_min_units() {
   return v;
 }
 
-int ts_prefetch() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("AO_B200_TS_PREFETCH");
-    v = e ? atoi(e) : 0;
-    if (v < 0 || v > 4096) v = 0;
-  }
-  return v;
-}
-
-int ts_producers() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("AO_B200_TS_PRODUCERS");
-    v = e ? atoi(e) : 2;
-    if (v != 1) v = 2;
-  }
-  return v;
-}
-
 int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     cudaDeviceProp p;
-    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 148;
+    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 132;
     n = p.multiProcessorCount;
   }
   return n;
@@ -178,7 +121,7 @@ int ao_b200_device_ok(void) {
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   cudaDeviceProp p;
   if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 0;
-  return p.major == 10 ? 1 : 0;
+  return (p.major == 9 && p.minor == 0) ? 1 : 0;
 }
 
 size_t ao_b200_workspace_bytes(int M, int N) {

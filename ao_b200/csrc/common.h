@@ -68,15 +68,7 @@ cudaError_t ensure_dynamic_smem(const void* kernel, size_t bytes);
 
 // PDL can be disabled globally (AO_B200_NO_PDL=1) for debugging.
 bool pdl_enabled();
-// AO_B200_TIMELINE=1: kernels record per-CTA phase timestamps at workspace + 48 KiB (bring-up only).
-bool timeline_enabled();
-// AO_B200_NO_PREFILL=1: M > 128 goes through the decode kernel's 128-token blocks instead of ts_prefill.cuh (A/B runs).
-bool prefill_disabled();
-int ts_flags();  // AO_B200_TS_FLAGS bring-up switches for ts_gemm.cuh
-int ts_ctas_per_sm();  // AO_B200_TS_CTAS_PER_SM (1 or 2; default 0 = by problem size): grid of ts_gemm.cuh in CTAs per SM
-int ts_min_units();    // AO_B200_TS_MIN_UNITS (bring-up): minimum chunks per CTA of ts_gemm.cuh grids, 0 = by problem size
-int ts_prefetch();     // AO_B200_TS_PREFETCH (bring-up): L2 prefetch distance in chunks ahead of the ring's loads (default 0)
-int ts_producers();    // AO_B200_TS_PRODUCERS: weight TMA producer warps of ts_gemm.cuh (1 or 2; default 2)
+int ts_min_units();    // AO_B200_TS_MIN_UNITS: minimum chunks per CTA of ts_gemm.cuh grids, 0 = by problem size
 int sm_count();
 
 }  // namespace ao

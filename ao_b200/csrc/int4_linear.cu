@@ -1,33 +1,32 @@
-// int4 weight-only linear on the tinygemm "tile_packed_to_4d" format, sm_100a.
+// int4 weight-only linear on the tinygemm "tile_packed_to_4d" format, sm_90a.
 //
 //   Y[M,N] = X[M,K] * W^[N,K]^T (+bias),  W^ = bf16((q-8)*s + z)   (group-wise s,z)
 //
 // Replaces aten._weight_int4pack_mm as called from the reference handler
 // (torchao/quantization/quantize_/workflows/int4/int4_tile_packed_to_4d_tensor.py:243-299).
-// The GEMM itself is the persistent tcgen05 TS-mode kernel of ts_gemm.cuh; this file supplies the
-// int4 format policy (how a 128-row x 128-k chunk is fetched and turned into bf16) and the launcher.
+// The GEMM itself is the persistent wgmma kernel of ts_gemm.cuh; this file supplies the int4 format policy (how a
+// 128-row x 128-k chunk is fetched and turned into bf16 wgmma A fragments) and the launcher.
 //
 // qdata layout (int32 [N/8][K/128][32][4], inner_k_tiles = 8), word `wd` of lane `t`:
 //   row n = 8*n8 + t/4;  k0 = 128*ko + 32*wd + 2*(t%4);
 //   bits [4e,4e+4)   = q[n, k0 + 8e]      e = 0..3
 //   bits [16+4e, ..) = q[n, k0 + 8e + 1]
-// so one row's 128 k of a k-tile are the 64 contiguous bytes of lanes 4*(n%8)..+3, a 128-row chunk is
-// 16 runs of 512 B, fetched by ONE 3-D TMA box {32 words, 4 row-pairs, 16 n8-tiles} with 128-byte
-// swizzle -- which makes the per-thread 16-byte ld.shared.v4 of "its" row bank-conflict free (Int4Fmt::load_row).
+// which is the m16n8k16 fragment layout: lane t of n8 tile j holds, for its row, exactly the k pairs that lane t of
+// the wgmma A fragment needs (k 2(t%4) + {0,1} and + 8 of every k16 step).  A 128-row chunk is 16 runs of 512 B,
+// fetched by ONE 3-D TMA box {32 words, 4 row-pairs, 16 n8-tiles} with 128-byte swizzle; a consumer thread reads
+// the 16 bytes of its lane in the n8 tiles of its two fragment rows (conflict-free ld.shared.v4).
 #include <cuda_bf16.h>
 #include <stdlib.h>
 
 #include "common.h"
 #include "ptx.cuh"
 #include "ts_gemm.cuh"
-#include "ts_prefill.cuh"
 
 namespace ao {
 namespace int4k {
 
 using tsg::KCHUNK;
 using tsg::ROWS;
-using tsg::W_BYTES;
 
 // (128+q) bf16x2 bits -> bf16x2 of fma(q-8, s, z), single rounding, = oracle W^.
 __device__ __forceinline__ uint32_t deq_pair(uint32_t magic_bits, __nv_bfloat162 s2, __nv_bfloat162 z2) {
@@ -39,6 +38,11 @@ __device__ __forceinline__ uint32_t deq_pair(uint32_t magic_bits, __nv_bfloat162
 }
 
 struct Int4Fmt {
+  static constexpr bool SS = false;
+  static constexpr bool PROMOTE = false;
+  static constexpr int X_ELEM_BYTES = 2;
+  static constexpr int W_BYTES = ROWS * KCHUNK / 2;   // 8 KiB of 4-bit weights per chunk
+  static constexpr int AUX_BYTES = 2048;              // (s, z) pairs: up to 4 groups x 128 rows x 4 B
   __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params& p) {
     const int gpc = p.group_size <= KCHUNK ? KCHUNK / p.group_size : 1;
     return W_BYTES + gpc * 512;
@@ -49,58 +53,43 @@ struct Int4Fmt {
     tma_load_3d(w_dst, tm_w, bar, 0, 4 * kc, n_tile * (ROWS / 8), policy);
     tma_load_2d(aux_dst, tm_sz, bar, n_tile * ROWS, (kc * KCHUNK) / p.group_size, policy);
   }
-  // One weight row of the chunk in registers: the row's 64 bytes are the four 16-byte lane words of its n8 group
-  // (tinygemm word wd of lane word i holds k = 32wd + 2i + 8e + {0,1}), plus the (s, z) pair of each 32-k word.
+  // the thread's two fragment rows: 16 bytes (4 tinygemm words = 128 k) each, and the (s, z) pair of every 32-k word
   struct Raw {
-    uint4 v[4];
-    uint32_t sz[4];
+    uint4 v[2];
+    uint32_t sz[2][4];
   };
-  __device__ static __forceinline__ void prefetch_w(const CUtensorMap* tm_w, const CUtensorMap* tm_sz, const tsg::Params& p, int n_tile, int kc) {
-    tma_prefetch_l2_3d(tm_w, 0, 4 * kc, n_tile * (ROWS / 8));
-    tma_prefetch_l2_2d(tm_sz, n_tile * ROWS, (kc * KCHUNK) / p.group_size);
-  }
-  // thread r (= TMEM lane = weight row of the tile): 4 x ld.shared.v4 through the TMA 128-byte swizzle -- per
-  // quarter-warp the eight rows hit eight different 16-byte bank groups: conflict-free (the half-row ld.shared.v2
-  // of round 1 was 2-way conflicted: profiles/r01_int4_final_ncu_full.csv) -- and 4 x ld.shared.b32 of (s, z)
-  __device__ static __forceinline__ void load_row(const tsg::Params& p, uint32_t w_smem, uint32_t aux_smem, int r, Raw& raw) {
+  __device__ static __forceinline__ void load(const tsg::Params& p, uint32_t w_smem, uint32_t aux_smem, int row_lo,
+                                              int lane, Raw& raw) {
     const int gshift = p.group_size == 32 ? 0 : (p.group_size == 64 ? 1 : 2);  // 32-k word -> group of the chunk
 #pragma unroll
-    for (int w = 0; w < 4; ++w) raw.sz[w] = tsg::lds32(aux_smem + r * 4 + (w >> gshift) * 512);
-    const uint32_t row_off = (uint32_t)(r >> 3) * 512u + (uint32_t)(r & 7) * 64u;
+    for (int h = 0; h < 2; ++h) {
+      const int r = row_lo + 8 * h;
+      const uint32_t off = (uint32_t)(r >> 3) * 512u + (uint32_t)lane * 16u;
+      raw.v[h] = tsg::lds128(w_smem + (off ^ (((off >> 7) & 7) << 4)));  // undo the TMA 128B swizzle
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint32_t off = row_off + i * 16;
-      raw.v[i] = tsg::lds128(w_smem + (off ^ (((off >> 7) & 7) << 4)));  // undo the TMA 128B swizzle
+      for (int w = 0; w < 4; ++w) raw.sz[h][w] = tsg::lds32(aux_smem + r * 4 + (w >> gshift) * 512);
     }
   }
-  // A value that depends on one destination register of EVERY ld.shared of load_row.  The kernels fold it into the
-  // address of the mbarrier arrive that hands the stage back to the TMA producers (through a comparison that is never
-  // true at run time but that ptxas cannot decide), so the arrive cannot issue before the loads have returned.  Without a
-  // data dependence it does: an empty asm with "r" inputs emits nothing, an unused xor chain is removed by ptxas, the
-  // arrive overtakes the loads in flight and the refill races with them (round 2: 2 of 6 runs of the nvfp4-weight prefill
-  // test off by a few values, profiles/r02_call_s.log).
-  __device__ static __forceinline__ uint32_t touch(const Raw& raw) {
-    return raw.v[0].x ^ raw.v[1].x ^ raw.v[2].x ^ raw.v[3].x ^ raw.sz[0] ^ raw.sz[1] ^ raw.sz[2] ^ raw.sz[3];
-  }
-  // quarter q = the 32 k of tinygemm word q: out[c] = bf16x2 of k pair (32q + 2c, 32q + 2c + 1), c = i + 4e
-  __device__ static __forceinline__ void dequant_quarter(const tsg::Params&, const Raw& raw, int q, uint32_t (&out)[16]) {
+  // k16 step kk = half (kk & 1) of tinygemm word kk / 2: a[0] / a[1] = rows lo / hi at k 2t + {0,1} (nibble e),
+  // a[2] / a[3] = the same rows at k + 8 (nibble e + 1)
+  __device__ static __forceinline__ void frag(const tsg::Params&, const Raw& raw, int kk, uint32_t (&a)[4]) {
     uint32_t magic = 0x43004300u;
     asm volatile("" : "+r"(magic));  // keep it in a register
-    const uint32_t sz = raw.sz[q];
-    const uint32_t s_bits = __byte_perm(sz, sz, 0x1010);
-    const uint32_t z_bits = __byte_perm(sz, sz, 0x3232);
-    const __nv_bfloat162 s2 = *reinterpret_cast<const __nv_bfloat162*>(&s_bits);
-    const __nv_bfloat162 z2 = *reinterpret_cast<const __nv_bfloat162*>(&z_bits);
+    const int wd = kk >> 1, e0 = 2 * (kk & 1);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint32_t word = q == 0 ? raw.v[i].x : q == 1 ? raw.v[i].y : q == 2 ? raw.v[i].z : raw.v[i].w;
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t sz = raw.sz[h][wd];
+      const uint32_t s_bits = __byte_perm(sz, sz, 0x1010);
+      const uint32_t z_bits = __byte_perm(sz, sz, 0x3232);
+      const __nv_bfloat162 s2 = *reinterpret_cast<const __nv_bfloat162*>(&s_bits);
+      const __nv_bfloat162 z2 = *reinterpret_cast<const __nv_bfloat162*>(&z_bits);
+      const uint32_t word = wd == 0 ? raw.v[h].x : wd == 1 ? raw.v[h].y : wd == 2 ? raw.v[h].z : raw.v[h].w;
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        // bf16x2 of 128+q = ((word >> 4e) & 0x000F000F) | 0x43004300 as ONE lop3 (C source compiles to two LOP3
-        // because both constants want the immediate slot)
+      for (int e = 0; e < 2; ++e) {
+        // bf16x2 of 128+q = ((word >> 4e) & 0x000F000F) | 0x43004300 as ONE lop3
         uint32_t m;
-        asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(m) : "r"(word >> (4 * e)), "r"(0x000F000Fu), "r"(magic));
-        out[i + 4 * e] = deq_pair(m, s2, z2);   // k pair (32q + 2i + 8e, +1)
+        asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(m) : "r"(word >> (4 * (e0 + e))), "r"(0x000F000Fu), "r"(magic));
+        a[h + 2 * e] = deq_pair(m, s2, z2);
       }
     }
   }
@@ -188,55 +177,21 @@ static int make_maps(const uint16_t* x, int ldx, int M, int K, const int32_t* qd
   return AO_OK;
 }
 
-template <int N_MMA, int DBUF = 2>
+template <int N_MMA>
 static int launch_tc(const uint16_t* x, int ldx, int M, int K, const int32_t* qdata, const uint16_t* sz, int g, int N,
                      const uint16_t* bias, uint16_t* y, int N_out, void* ws, size_t ws_bytes,
                      cudaStream_t stream) {
-  using C = tsg::Cfg<N_MMA, DBUF>;
-  const int KT = K / 128;
   CUtensorMap tm_w, tm_sz, tm_x;
   if (int rc = make_maps(x, ldx, M, K, qdata, sz, g, N, N_MMA, &tm_w, &tm_sz, &tm_x)) return rc;
   tsg::Params p{};
   p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.epi = tsg::EPI_FLOAT;
   p.M = M; p.N = N; p.N_out = N_out; p.K = K; p.group_size = g;
   p.n_tiles = ceil_div(N_out, ROWS);
   p.m_blocks = ceil_div(M, N_MMA);
-  p.KT = KT;
-  int grid = 0;
-  if (int rc = tsg::plan<N_MMA>(p, ws, ws_bytes, "int4 linear", &grid)) return rc;
-  // bring-up timeline: two slots (consecutive launches alternate) of 100 CTAs x 16 stamps + 8 chunks x 8 fine stamps at workspace + 20 MiB
-  static unsigned tl_launch = 0;
-  p.timeline = timeline_enabled() ? reinterpret_cast<unsigned long long*>(reinterpret_cast<uint8_t*>(ws) + ((size_t)20 << 20) +
-                                                                         (size_t)(tl_launch++ & 1) * (100 * 16 + 64) * 8)
-                                  : nullptr;
-  auto kern = (p.timeline && N_MMA <= 32) ? tsg::ts_gemm_kernel<Int4Fmt, (N_MMA <= 32 ? N_MMA : 16), true, DBUF>
-                                           : tsg::ts_gemm_kernel<Int4Fmt, N_MMA, false, DBUF>;
-  AO_CUDA_CHECK(ensure_dynamic_smem(reinterpret_cast<const void*>(kern), C::SMEM_BYTES));
-  AO_CUDA_CHECK(launch(kern, dim3(grid), dim3(tsg::NUM_THREADS), C::SMEM_BYTES, stream, pdl_enabled(), tm_w, tm_sz,
-                       tm_x, p));
-  return AO_OK;
-}
-
-// M > 128 tokens: the prefill-shaped kernel (ts_prefill.cuh), weights dequantised once per 256 tokens
-static int launch_prefill(const uint16_t* x, int ldx, int M, int K, const int32_t* qdata, const uint16_t* sz, int g, int N,
-                          const uint16_t* bias, uint16_t* y, int N_out, void* ws, size_t ws_bytes, cudaStream_t stream) {
-  CUtensorMap tm_w, tm_sz, tm_x;
-  if (int rc = make_maps(x, ldx, M, K, qdata, sz, g, N, tsp::N_TOK, &tm_w, &tm_sz, &tm_x)) return rc;
-  tsg::Params p{};
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.M = M; p.N = N; p.N_out = N_out; p.K = K; p.group_size = g;
-  p.n_tiles = ceil_div(N_out, ROWS);
-  p.m_blocks = ceil_div(M, tsp::N_TOK);
   p.KT = K / 128;
-  int grid = 0;
-  if (int rc = tsp::plan(p, ws, ws_bytes, "int4 linear (prefill)", &grid)) return rc;
-  auto kern = tsp::ts_prefill_kernel<Int4Fmt>;
-  AO_CUDA_CHECK(ensure_dynamic_smem(reinterpret_cast<const void*>(kern), tsp::SMEM_BYTES));
-  AO_CUDA_CHECK(launch(kern, dim3(grid), dim3(tsp::NUM_THREADS), tsp::SMEM_BYTES, stream, pdl_enabled(), tm_w, tm_sz,
-                       tm_x, p));
-  return AO_OK;
+  return tsg::launch_gemm<Int4Fmt, N_MMA>(p, tm_w, tm_sz, tm_x, ws, ws_bytes, "int4 linear", stream);
 }
 
 }  // namespace int4k
@@ -278,10 +233,7 @@ extern "C" int ao_int4_tilepacked_linear_strided(const uint16_t* x, int ldx, int
   if (M <= 64)
     return int4k::launch_tc<64>(x, ldx, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
                                 workspace_bytes, st);
-  if (!tsp::worth_it(M, N_out, K))
-    return int4k::launch_tc<128>(x, ldx, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
-                                 workspace_bytes, st);
-  return int4k::launch_prefill(x, ldx, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
+  return int4k::launch_tc<128>(x, ldx, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
                                workspace_bytes, st);
 }
 

@@ -1,449 +1,271 @@
-// Swap-AB streaming GEMMs for 8-bit / 4-bit operands on tcgen05 (sm_100a):
-//   int8 x int8 -> int32  (kind::i8)         replaces aten._int_mm + the scale epilogue
-//   e4m3 x e4m3 -> f32    (kind::f8f6f4)     replaces torch._scaled_mm rowwise
-//   mxfp8 block-32 e8m0   (kind::mxf8f6f4)   replaces torch._scaled_mm block-scaled
-//   nvfp4 block-16 e4m3   (kind::mxf4nvf4)   replaces torch._scaled_mm fp4 + pts/bias kernels
+// Swap-AB streaming GEMMs for 8-bit / 4-bit operands on Hopper wgmma (sm_90a), all on the kernel of ts_gemm.cuh:
+//   int8 x int8 -> int32  (wgmma s8, both operands TMA tiles)      replaces aten._int_mm + the scale epilogue
+//   e4m3 x e4m3 -> f32    (wgmma e4m3, both operands TMA tiles)    replaces torch._scaled_mm rowwise
+//   mxfp8 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm block-scaled
+//   nvfp4 block-16 e4m3   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm fp4 + pts/bias kernels
 // Reference call sites: int8/kernels.py:18-76,114-144 + int8_tensor.py:305-359;
 // float8/inference.py:86-123; mx_formats/mx_tensor.py:759-843; nvfp4_tensor.py:487-578.
 //
-// Decode-shaped (M <= 128 tokens per block).  The weight matrix W[N,K] (K-major, exactly the
-// stored qdata) is the UMMA A operand: 128 output features per CTA; the activations are the B
-// operand (N_MMA tokens).  TMA (SWIZZLE_128B) streams 128-byte-wide K blocks of W through a
-// deep smem ring straight into tcgen05.mma (SS mode) -- no register staging at all; block
-// scales go smem -> TMEM with tcgen05.cp.  Epilogue: TMEM -> registers -> scale/bias -> bf16.
-// Persistent stream-K (streamk.cuh): (tile, K-chunk) units split evenly over the CTAs; tiles shared by several
-// CTAs are finished by their owner CTA from the contributors' published 32-bit partials in CTA order
-// (deterministic; int32 for int8: stays exact).
+// The weight matrix W[N,K] (K-major, exactly the stored qdata) is the wgmma A operand: 128 output features per tile;
+// the activations are the B operand (N_MMA tokens).  Hopper's tensor cores have no block-scaled kinds, so for mxfp8 and
+// nvfp4 every element is multiplied by its block scale BEFORE the MMA, in bf16, where the product is exact (e4m3 x
+// 2^k: 4 significant bits; e2m1 x e4m3: at most 6): the weights inside the kernel (register-A fragments), the
+// activations by a pre-pass into a bf16 slab of the workspace.  The fp32 sums then see the same products a
+// block-scaled MMA sees.
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <stdlib.h>
 
 #include "common.h"
+#include "nvfp4_fmt.cuh"
 #include "ptx.cuh"
 #include "streamk.cuh"
+#include "ts_gemm.cuh"
 
 namespace ao {
 namespace lowp {
 
 enum Kind { KIND_I8 = 0, KIND_F8 = 1, KIND_MXF8 = 2, KIND_NVF4 = 3 };
 
-using streamk::ROWS;
-constexpr int KB = 128;             // bytes of K per stage per row (128 elems for 8-bit, 256 for fp4)
-constexpr int A_BYTES = ROWS * KB;  // 16 KiB
-constexpr int EPI_WARP0 = 0, TMA_WARP = 4, MMA_WARP = 5;
-constexpr int NUM_THREADS = 192;
+using tsg::KCHUNK;
+using tsg::ROWS;
 
-template <int KIND, int N_MMA>
-struct Cfg {
-  static constexpr bool BLOCK_SCALED = (KIND == KIND_MXF8 || KIND == KIND_NVF4);
-  static constexpr int B_BYTES = N_MMA * KB;
-  // scale tiles per stage: mxfp8 1 blocked tile (128 rows x 4 sf), nvfp4 4 tiles (16 sf / row)
-  static constexpr int SF_TILES = KIND == KIND_MXF8 ? 1 : (KIND == KIND_NVF4 ? 4 : 0);
-  static constexpr int SF_BYTES = SF_TILES * 512;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES + 2 * SF_BYTES + (BLOCK_SCALED ? (1024 - (2 * SF_BYTES) % 1024) % 1024 : 0);
-  static constexpr int BUDGET = N_MMA <= 64 ? 104 * 1024 : 168 * 1024;
-  static constexpr int STAGES = BUDGET / STAGE_BYTES;
-  static constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 + 1024;
-  // TMEM: two accumulators, then the scale factors (double-buffered by chunk parity)
-  static constexpr int D_COL0 = 0, D_COL1 = N_MMA;
-  static constexpr int SF_COLS = SF_TILES * 4;  // columns per operand per chunk
-  static constexpr int SFA_COL = N_MMA <= 64 ? 128 : 256;
-  static constexpr int SFB_COL = SFA_COL + 32;
-  static constexpr int TMEM_COLS = N_MMA <= 64 ? (BLOCK_SCALED ? 256 : (N_MMA <= 16 ? 32 : (N_MMA <= 32 ? 64 : 128))) : (BLOCK_SCALED ? 512 : 256);
-  static constexpr int MMA_PER_STAGE = 4;  // K bytes per MMA = 32 (8-bit: 32 elems, fp4: 64)
+// int8 / e4m3: both operands straight from the TMA tiles (128-byte swizzle, 128 k per chunk = four k32 wgmmas)
+template <int KIND>
+struct SsFmt {
+  static constexpr bool SS = true;
+  static constexpr bool PROMOTE = KIND == KIND_F8;   // int8 sums are exact in s32
+  static constexpr int X_ELEM_BYTES = 1;
+  static constexpr int W_BYTES = ROWS * KCHUNK;   // 16 KiB
+  static constexpr int AUX_BYTES = 0;
+  __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES; }
+  __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap*, const tsg::Params&,
+                                                 uint8_t* w_dst, uint8_t*, uint64_t* bar, int n_tile, int kc,
+                                                 uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
+  }
+  template <int N_MMA>
+  __device__ static __forceinline__ void mma(uint32_t (&acc)[N_MMA / 2], uint32_t w_s, uint32_t x_s, int wg,
+                                             uint32_t scale_d) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint64_t ad = wgmma_desc_k_sw128(w_s + wg * (64 * 128) + kk * 32);
+      const uint64_t bd = wgmma_desc_k_sw128(x_s + kk * 32);
+      if (KIND == KIND_I8) Wgmma<N_MMA>::ss_s8(acc, ad, bd, kk == 0 ? scale_d : 1u);
+      else Wgmma<N_MMA>::ss_e4m3(acc, ad, bd, kk == 0 ? scale_d : 1u);
+    }
+  }
 };
 
-struct Params {
-  const float* x_scale;   // [M]     (rowwise kinds) or a_pts scalar (nvfp4) or null
-  const float* w_scale;   // [N]     (rowwise kinds) or b_pts scalar (nvfp4) or null
-  const __nv_bfloat16* bias;
-  __nv_bfloat16* y;       // bf16 out [M, N]  (null when i32_out is set)
-  int32_t* i32_out;       // raw int32 accumulators [M, N] (ao_int8_mm_i32)
-  float* ws_partial;      // [grid][N_MMA*128] 32-bit partials (int32 bits for int8): CTA b's CONTRIB partial
-  unsigned int* ws_flag;  // [grid] CTA b's partial is published (streamk.cuh)
-  int M, N, K;            // K in ELEMENTS
-  int n_tiles, m_blocks, KT;  // KT = chunks of 128 K-bytes
-  int sf_col_blocks_w;    // number of 4-wide scale column blocks per row block (blocked layout)
-  int sf_col_blocks_x;
-};
-
-using streamk::cta_of_unit;
-using streamk::unit_begin;
-
-// Persistent stream-K kernel (same work split / fix-up protocol as ts_gemm.cuh, SS-mode MMAs):
-// warps 0-3 epilogue, warp 4 TMA producer, warp 5 MMA issuer.
-template <int KIND, int N_MMA>
-__global__ void __launch_bounds__(NUM_THREADS, (N_MMA <= 64 ? 2 : 1))
-lowp_linear_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
-                   const uint8_t* __restrict__ w_sf, const uint8_t* __restrict__ x_sf,
-                   const Params p) {
-  using C = Cfg<KIND, N_MMA>;
-  constexpr int S = C::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * C::STAGE_BYTES);
-  uint64_t* wfull = bars;            // [S] weights (+ weight scales)
-  uint64_t* xfull = wfull + S;       // [S] activations (+ activation scales)
-  uint64_t* sempty = xfull + S;      // [S] MMA commit
-  uint64_t* dfull = sempty + S;      // [2]
-  uint64_t* dempty = dfull + 2;      // [2] 4 epilogue warps
-  uint64_t* fok = dempty + 2;        // [1] the contributors' flags of an OWNER last segment have been seen (TMA warp polls)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(fok + 1);
-
-  // warp index through a shuffle => known warp-uniform: the single-thread roles are warp-uniform loops with only
-  // the TMA / tcgen05 instructions under elect.sync, so their operands live in uniform registers (with the whole
-  // loop under `lane == 0` ptxas wraps every UTCHMMA / UTMALDG in an elect-broadcast loop, ~2.5x slower issue)
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  const int G = gridDim.x, b = blockIdx.x;
-  const long long U = (long long)p.n_tiles * p.m_blocks * p.KT;
-  const int u0 = unit_begin(b, U, G), u1 = unit_begin(b + 1, U, G);
-  const int nunits = u1 - u0;
-  const streamk::Walk walk(u0, nunits, p.KT);
-  auto tile_of = [&](int i) { return (u0 + i) / p.KT; };
-  auto kc_of = [&](int i) { return (u0 + i) % p.KT; };
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < S; ++i) {
-      mbar_init(&wfull[i], 1);
-      mbar_init(&xfull[i], 1);
-      mbar_init(&sempty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&dfull[i], 1);
-      mbar_init(&dempty[i], 4);
-    }
-    mbar_init(fok, 1);
-    fence_barrier_init();
-  }
-  if (warp == TMA_WARP && lane == 0) {
-    tma_prefetch_desc(&tm_w);
-    tma_prefetch_desc(&tm_x);
-  }
-  if (warp == MMA_WARP) tmem_alloc<C::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-  pdl_launch_dependents();
-
-  if (warp == TMA_WARP) {
-    {
-      const uint64_t pol_w = policy_evict_first();
-      const uint64_t pol_x = policy_evict_last();
-      auto issue_w = [&](int i) {
-        const int s = i % S, n_tile = tile_of(i) % p.n_tiles, kc = kc_of(i);
-        uint8_t* st = smem + (size_t)s * C::STAGE_BYTES;
-        mbar_expect_tx(&wfull[s], A_BYTES + C::SF_BYTES);
-        tma_load_2d(st, &tm_w, &wfull[s], kc * KB, n_tile * ROWS, pol_w);
-        if (C::BLOCK_SCALED) {
-          // blocked scale tiles of this (row block, k chunk): SF_TILES consecutive 512-byte tiles
-          const uint8_t* src = w_sf + ((size_t)n_tile * p.sf_col_blocks_w + (size_t)kc * C::SF_TILES) * 512;
-          asm volatile(
-              "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                  smem_u32(st + A_BYTES + C::B_BYTES)),
-              "l"(src), "r"(C::SF_BYTES), "r"(smem_u32(&wfull[s]))
-              : "memory");
-        }
-      };
-      auto issue_x = [&](int i) {
-        const int s = i % S, m0 = (tile_of(i) / p.n_tiles) * N_MMA, kc = kc_of(i);
-        uint8_t* st = smem + (size_t)s * C::STAGE_BYTES;
-        mbar_expect_tx(&xfull[s], C::B_BYTES + C::SF_BYTES);
-        tma_load_2d(st + A_BYTES, &tm_x, &xfull[s], kc * KB, m0, pol_x);
-        if (C::BLOCK_SCALED) {
-          const uint8_t* src = x_sf + ((size_t)(m0 / 128) * p.sf_col_blocks_x + (size_t)kc * C::SF_TILES) * 512;
-          asm volatile(
-              "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                  smem_u32(st + A_BYTES + C::B_BYTES + C::SF_BYTES)),
-              "l"(src), "r"(C::SF_BYTES), "r"(smem_u32(&xfull[s]))
-              : "memory");
-        }
-      };
-      const int pre = nunits < S ? nunits : S;
-      for (int i = 0; i < pre; ++i) {
-        if (elect_one()) issue_w(i);   // weights never depend on the previous kernel
-        __syncwarp();
-      }
-      pdl_wait();
-      for (int i = 0; i < pre; ++i) {
-        if (elect_one()) issue_x(i);
-        __syncwarp();
-      }
-      for (int i = S; i < nunits; ++i) {
-        mbar_wait(&sempty[i % S], ((i / S) & 1) ^ 1);
-        if (elect_one()) {
-          issue_w(i);
-          issue_x(i);
-        }
-        __syncwarp();
-      }
-      if (walk.seg_kind(walk.nseg - 1) == streamk::SEG_OWNER) {
-        // this warp is done a ring depth before the CTA is: it polls the contributors' flags (ld.acquire.gpu) and passes
-        // the result on through a cta-scope barrier, so that L2 round trip runs under the last MMAs instead of between
-        // them and the owner's gather (same scheme as ts_gemm.cuh)
-        const int tile_l = walk.seg_tile(walk.nseg - 1);
-        const int n_oth = cta_of_unit((long long)tile_l * p.KT + p.KT - 1, U, G) - b;
-        for (int base = 0; base < n_oth; base += 32)
-          if (base + lane < n_oth)
-            while (streamk::ld_acquire_u32(p.ws_flag + b + 1 + base + lane) == 0u) __nanosleep(64);
-        __syncwarp();
-        if (elect_one()) mbar_arrive(fok);
-        __syncwarp();
-      }
-    }
-  } else if (warp == MMA_WARP) {
-    constexpr uint32_t idesc =
-        KIND == KIND_I8   ? make_idesc(2 /*s32*/, 1 /*int8*/, 1 /*int8*/, ROWS, N_MMA)
-        : KIND == KIND_F8 ? make_idesc(1 /*f32*/, 0 /*e4m3*/, 0 /*e4m3*/, ROWS, N_MMA)
-        : KIND == KIND_MXF8 ? make_idesc_bs(0 /*e4m3*/, 0 /*e4m3*/, 1 /*ue8m0*/, ROWS, N_MMA)
-                            : make_idesc_bs(1 /*e2m1*/, 1 /*e2m1*/, 0 /*ue4m3*/, ROWS, N_MMA);
-    int seg = 0;
-    for (int i = 0; i < nunits; ++i) {
-      const int s = i % S;
-      const bool first = (i == 0) || (kc_of(i) == 0);
-      const bool last = (i == nunits - 1) || (kc_of(i) == p.KT - 1);
-      const int buf = seg & 1;
-      if (first) {
-        mbar_wait(&dempty[buf], ((seg >> 1) & 1) ^ 1);
-        tc_fence_after();
-      }
-      mbar_wait(&wfull[s], (i / S) & 1);
-      mbar_wait(&xfull[s], (i / S) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t ab = smem_u32(smem + (size_t)s * C::STAGE_BYTES);
-        const uint32_t bb = ab + A_BYTES;
-        const uint32_t d_t = tmem_base + (buf ? C::D_COL1 : C::D_COL0);
-        uint32_t sfa_t = 0, sfb_t = 0;
-        if (C::BLOCK_SCALED) {
-          const int sb = i & 1;
-          sfa_t = tmem_base + C::SFA_COL + sb * C::SF_COLS;
-          sfb_t = tmem_base + C::SFB_COL + sb * C::SF_COLS;
-#pragma unroll
-          for (int tI = 0; tI < C::SF_TILES; ++tI) {
-            // 512-byte tile = 32 rows x 16 bytes, contiguous: one 8x16B core matrix per 128 B
-            const uint64_t da = umma_desc_k_noswz(bb + C::B_BYTES + tI * 512, 16, 128);
-            const uint64_t db = umma_desc_k_noswz(bb + C::B_BYTES + C::SF_BYTES + tI * 512, 16, 128);
-            tc_cp_32x128b_warpx4(sfa_t + tI * 4, da);
-            tc_cp_32x128b_warpx4(sfb_t + tI * 4, db);
-          }
-        }
-#pragma unroll
-        for (int kk = 0; kk < C::MMA_PER_STAGE; ++kk) {
-          const uint64_t adesc = umma_desc_k_sw128(ab + kk * 32);
-          const uint64_t bdesc = umma_desc_k_sw128(bb + kk * 32);
-          const uint32_t acc = (!first || kk > 0) ? 1u : 0u;
-          if (KIND == KIND_I8) mma_ss_i8(d_t, adesc, bdesc, idesc, acc);
-          else if (KIND == KIND_F8) mma_ss_f8f6f4(d_t, adesc, bdesc, idesc, acc);
-          else if (KIND == KIND_MXF8)
-            // one scale byte per row per MMA: byte kk of the tile's column (sf_id fields)
-            mma_ss_mxf8f6f4(d_t, adesc, bdesc, idesc | ((uint32_t)kk << 29) | ((uint32_t)kk << 4), acc, sfa_t, sfb_t);
-          else
-            // four scale bytes per row per MMA: tile kk
-            mma_ss_mxf4nvf4_b16(d_t, adesc, bdesc, idesc, acc, sfa_t + kk * 4, sfb_t + kk * 4);
-        }
-        tc_commit(&sempty[s]);
-        if (last) tc_commit(&dfull[buf]);
-      }
-      __syncwarp();
-      if (last) ++seg;
-    }
-  } else {
-    // ------------------------------------------------------------ epilogue (warps 0..3)
-    const int q4 = warp & 3;
-    const int r = q4 * 32 + lane;
-    const uint32_t lane_taddr = tmem_base + ((uint32_t)(q4 * 32) << 16);
-    pdl_wait();
-    for (int seg = 0; seg < walk.nseg; ++seg) {
-      const int tile = walk.seg_tile(seg);
-      const int kind = walk.seg_kind(seg);
-      const int buf = seg & 1;
-      mbar_wait(&dfull[buf], (seg >> 1) & 1);
-      tc_fence_after();
-      const int n_tile = tile % p.n_tiles, m_blk = tile / p.n_tiles;
-      const int n = n_tile * ROWS + r, m0 = m_blk * N_MMA;
-      const uint32_t d_t = lane_taddr + (buf ? C::D_COL1 : C::D_COL0);
-      float sw = 1.f, bias = 0.f;
-      if (n < p.N) {
-        if (KIND == KIND_I8 || KIND == KIND_F8) sw = p.w_scale ? p.w_scale[n] : 1.f;
-        if (KIND == KIND_NVF4) sw = (p.x_scale ? *p.x_scale : 1.f) * (p.w_scale ? *p.w_scale : 1.f);
-        if (p.bias) bias = __bfloat162float(p.bias[n]);
-      }
-      // finalise one accumulator value (raw 32 bits: s32 for int8, f32 otherwise) into the output
-      auto emit = [&](int m, uint32_t raw_i, float raw_f) {
-        if (KIND == KIND_I8) {
-          if (p.i32_out) {
-            p.i32_out[(size_t)m * p.N + n] = (int32_t)raw_i;
-            return;
-          }
-          // int8/kernels.py:143-144 + int8_tensor.py:315-359: bf16 round between the scales
-          const float t = __bfloat162float(__float2bfloat16_rn((float)(int32_t)raw_i * p.x_scale[m]));
-          p.y[(size_t)m * p.N + n] = __float2bfloat16_rn(t * sw + bias);
-        } else if (KIND == KIND_F8) {
-          p.y[(size_t)m * p.N + n] = __float2bfloat16_rn(raw_f * (p.x_scale[m] * sw) + bias);
-        } else if (KIND == KIND_MXF8) {
-          p.y[(size_t)m * p.N + n] = __float2bfloat16_rn(raw_f + bias);
-        } else {
-          p.y[(size_t)m * p.N + n] = __float2bfloat16_rn(raw_f * sw + bias);
-        }
-      };
-      if (kind == streamk::SEG_FULL) {
-#pragma unroll
-        for (int j = 0; j < N_MMA; j += 16) {
-          uint32_t rr[16];
-          tmem_ld_x16(d_t + j, rr);
-          tc_wait_ld();
-          if (n < p.N) {
-#pragma unroll
-            for (int q = 0; q < 16; ++q)
-              if (m0 + j + q < p.M) emit(m0 + j + q, rr[q], __uint_as_float(rr[q]));
-          }
-        }
-      } else if (kind == streamk::SEG_CONTRIB) {
-        // publish the partial (column-major slot: coalesced across the 128 rows), then raise this CTA's flag
-        uint32_t* slot = reinterpret_cast<uint32_t*>(p.ws_partial) + (size_t)b * (N_MMA * ROWS) + r;
-#pragma unroll
-        for (int j = 0; j < N_MMA; j += 16) {
-          uint32_t rr[16];
-          tmem_ld_x16(d_t + j, rr);
-          tc_wait_ld();
-#pragma unroll
-          for (int q = 0; q < 16; ++q)
-            if (m0 + j + q < p.M) __stcg(&slot[(j + q) * ROWS], rr[q]);
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");   // all 128 rows stored (cta-scope order) ...
-        if (threadIdx.x == EPI_WARP0 * 32) streamk::st_release_u32(p.ws_flag + b, 1u);   // ... one gpu-scope release
-      } else {
-        // OWNER: own partial (TMEM) + the partials of CTAs b+1 .. b_last in that order (fixed: deterministic)
-        const int b_last = cta_of_unit((long long)tile * p.KT + p.KT - 1, U, G);
-        const int n_oth = b_last - b;
-        const uint32_t* slot0 = reinterpret_cast<const uint32_t*>(p.ws_partial) + (size_t)(b + 1) * (N_MMA * ROWS) + r;
-        mbar_wait(fok, 0);   // flags seen by the TMA warp (above)
-#pragma unroll 1
-        for (int j0 = 0; j0 < N_MMA; j0 += 16) {
-          if (m0 + j0 >= p.M) break;
-          uint32_t own[16];
-          tmem_ld_x16(d_t + j0, own);
-          tc_wait_ld();
-          float vf[16];
-          int32_t vi[16];
-#pragma unroll
-          for (int q = 0; q < 16; ++q) {
-            vf[q] = __uint_as_float(own[q]);
-            vi[q] = (int32_t)own[q];
-          }
-#pragma unroll 1
-          for (int c0 = 0; c0 < n_oth; c0 += 2) {
-            // two contributors x 16 columns of loads in flight (the gather is a chain of L2 round trips)
-            uint32_t t0[16], t1[16];
-            const uint32_t* s0 = slot0 + (size_t)c0 * (N_MMA * ROWS) + (size_t)j0 * ROWS;
-            const uint32_t* s1 = s0 + (size_t)(N_MMA * ROWS);
-            const bool has1 = c0 + 1 < n_oth;
-#pragma unroll
-            for (int q = 0; q < 16; ++q) t0[q] = (n < p.N && m0 + j0 + q < p.M) ? __ldcg(s0 + q * ROWS) : 0u;
-#pragma unroll
-            for (int q = 0; q < 16; ++q) t1[q] = (has1 && n < p.N && m0 + j0 + q < p.M) ? __ldcg(s1 + q * ROWS) : 0u;
-#pragma unroll
-            for (int q = 0; q < 16; ++q) {
-              vi[q] += (int32_t)t0[q] + (int32_t)t1[q];
-              vf[q] = (vf[q] + __uint_as_float(t0[q])) + __uint_as_float(t1[q]);
-            }
-          }
-          if (n < p.N) {
-#pragma unroll
-            for (int q = 0; q < 16; ++q)
-              if (m0 + j0 + q < p.M) emit(m0 + j0 + q, (uint32_t)vi[q], vf[q]);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&dempty[buf]);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == EPI_WARP0 && walk.seg_kind(walk.nseg - 1) == streamk::SEG_OWNER) {
-    // the owner has consumed its contributors' partials: re-arm their flags for the next launch
-    const int b_last = cta_of_unit((long long)walk.seg_tile(walk.nseg - 1) * p.KT + p.KT - 1, U, G);
-    for (int c = b + 1 + lane; c <= b_last; c += 32) p.ws_flag[c] = 0u;
-  }
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc<C::TMEM_COLS>(tmem_base);
-  }
+// 2^(e - 127) for an e8m0 byte (0xFF = NaN)
+__device__ __forceinline__ float e8m0_to_f32(uint32_t e) {
+  return __uint_as_float(e == 0xFFu ? 0x7FC00000u : (e ? e << 23 : 0x00400000u));
 }
 
-template <int KIND, int N_MMA>
-static int launch(const uint8_t* xq, const uint8_t* x_sf, const float* x_scale, int M, int K,
-                  const uint8_t* wq, const uint8_t* w_sf, const float* w_scale, int N,
-                  const uint16_t* bias, uint16_t* y, int32_t* i32_out, void* ws, size_t ws_bytes,
-                  cudaStream_t stream) {
-  using C = Cfg<KIND, N_MMA>;
-  const int epb = KIND == KIND_NVF4 ? 2 : 1;
-  const int k_bytes = K / epb;
-  CUtensorMap tm_w, tm_x;
+// mxfp8 weights as the register-A operand: e4m3 pairs x their block-32 e8m0 scale -> bf16 (exact)
+struct Mxfp8Fmt {
+  static constexpr bool SS = false;
+  static constexpr bool PROMOTE = false;
+  static constexpr int X_ELEM_BYTES = 2;
+  static constexpr int W_BYTES = ROWS * KCHUNK;   // 128 rows x 128 bytes, 128-byte swizzle
+  static constexpr int AUX_BYTES = 512;           // one blocked scale tile (4 scales = 128 k per row)
+  static constexpr int ACC_EXP2 = 0;
+  __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES + AUX_BYTES; }
+  __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap* tm_sf, const tsg::Params& p,
+                                                 uint8_t* w_dst, uint8_t* aux_dst, uint64_t* bar, int n_tile, int kc,
+                                                 uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
+    tma_load_2d(aux_dst, tm_sf, bar, 0, n_tile * p.aux_col_blocks + kc, policy);
+  }
+  // the thread's two fragment rows: for k16 step kk the e4m3 pair at k 16kk + 2t (low half) and + 8 (high half)
+  struct Raw {
+    uint32_t v[2][8];
+    uint32_t sc[2];
+  };
+  __device__ static __forceinline__ void load(const tsg::Params&, uint32_t w_smem, uint32_t aux_smem, int row_lo, int lane,
+                                              Raw& raw) {
+    const int t = lane & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row_lo + 8 * h;
+      raw.sc[h] = tsg::lds32(aux_smem + (uint32_t)(r & 31) * 16u + (uint32_t)(r >> 5) * 4u);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint32_t a = w_smem + (uint32_t)r * 128u + ((uint32_t)(kk ^ (r & 7)) << 4) + 2 * t;   // TMA 128B swizzle
+        raw.v[h][kk] = tsg::lds16(a) | (tsg::lds16(a + 8) << 16);
+      }
+    }
+  }
+  __device__ static __forceinline__ uint32_t deq(uint32_t pair, float s) {
+    const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)pair, __NV_E4M3);
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+    __nv_bfloat162 b = __floats2bfloat162_rn(f.x * s, f.y * s);
+    return *reinterpret_cast<uint32_t*>(&b);
+  }
+  __device__ static __forceinline__ void frag(const tsg::Params&, const Raw& raw, int kk, uint32_t (&a)[4]) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float s = e8m0_to_f32((raw.sc[h] >> (8 * (kk >> 1))) & 0xFFu);   // the 32-k block of step kk
+      a[h] = deq(raw.v[h][kk] & 0xFFFFu, s);
+      a[h + 2] = deq(raw.v[h][kk] >> 16, s);
+    }
+  }
+};
+
+// Activation pre-pass of the block-scaled kinds: rows [m0, m0 + rows) of the quantised activations -> bf16 [rows][K],
+// every element times its block scale (exact in bf16).  One thread per 16 elements.
+template <int KIND>
+__global__ void __launch_bounds__(256) dequant_act_kernel(const uint8_t* __restrict__ xq, const uint8_t* __restrict__ x_sf,
+                                                          int m0, int rows, int K, int sf_col_blocks,
+                                                          __nv_bfloat16* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();   // the slab may still be read by the previous GEMM; the activations may be the previous kernel's output
+  const int per_row = K / 16;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)rows * per_row) return;
+  const int mr = (int)(idx / per_row), k0 = (int)(idx % per_row) * 16, m = m0 + mr;
+  const int kb = KIND == KIND_NVF4 ? k0 / 16 : k0 / 32;
+  const size_t tile = (size_t)(m / 128) * sf_col_blocks + kb / 4;
+  const uint32_t sbyte = x_sf[tile * 512 + (m % 32) * 16 + ((m % 128) / 32) * 4 + kb % 4];
+  __nv_bfloat16 o[16];
+  if (KIND == KIND_NVF4) {
+    const __half_raw sh = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)sbyte, __NV_E4M3);
+    const float s = __half2float(*reinterpret_cast<const __half*>(&sh));
+    const uint2 v = *reinterpret_cast<const uint2*>(xq + (size_t)m * (K / 2) + k0 / 2);
+    const float lut[8] = {0.f, 0.5f, 1.f, 1.5f, 2.f, 3.f, 4.f, 6.f};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const uint32_t nib = ((j < 8 ? v.x : v.y) >> (4 * (j & 7))) & 0xFu;
+      const float x = lut[nib & 7] * s;
+      o[j] = __float2bfloat16_rn(nib & 8 ? -x : x);
+    }
+  } else {
+    const float s = e8m0_to_f32(sbyte);
+    const uint4 v = *reinterpret_cast<const uint4*>(xq + (size_t)m * K + k0);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[j >> 1] >> (16 * (j & 1))), __NV_E4M3);
+      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+      o[2 * j] = __float2bfloat16_rn(f.x * s);
+      o[2 * j + 1] = __float2bfloat16_rn(f.y * s);
+    }
+  }
+  uint4* dst = reinterpret_cast<uint4*>(out + (size_t)mr * K + k0);
+  dst[0] = reinterpret_cast<const uint4*>(o)[0];
+  dst[1] = reinterpret_cast<const uint4*>(o)[1];
+}
+
+template <class Fmt, int N_MMA>
+static int launch_gemm(tsg::Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const void* x, int x_elem,
+                       int ld_bytes, void* ws, size_t ws_bytes, cudaStream_t st) {
+  CUtensorMap tm_x;
   {
-    const uint64_t dims[2] = {(uint64_t)k_bytes, (uint64_t)N};
-    const uint64_t str[1] = {(uint64_t)k_bytes};
-    const uint32_t box[2] = {KB, ROWS};
+    const uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.M};
+    const uint64_t str[1] = {(uint64_t)ld_bytes};
+    const uint32_t box[2] = {(uint32_t)(128 / x_elem), (uint32_t)N_MMA};
+    int rc = make_tmap(&tm_x, x_elem == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, x, dims,
+                       str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+  }
+  p.m_blocks = ceil_div(p.M, N_MMA);
+  return tsg::launch_gemm<Fmt, N_MMA>(p, tm_w, tm_aux, tm_x, ws, ws_bytes, "lowp linear", st);
+}
+
+// MAX_N: widest token tile (fp8 keeps a second accumulator per chunk: 64 tokens)
+template <class Fmt, int MAX_N = 128>
+static int dispatch_m(tsg::Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const void* x, int x_elem,
+                      int ld_bytes, void* ws, size_t ws_bytes, cudaStream_t st) {
+  if (p.M <= 16) return launch_gemm<Fmt, 16>(p, tm_w, tm_aux, x, x_elem, ld_bytes, ws, ws_bytes, st);
+  if (p.M <= 32) return launch_gemm<Fmt, 32>(p, tm_w, tm_aux, x, x_elem, ld_bytes, ws, ws_bytes, st);
+  if (p.M <= 64 || MAX_N == 64) return launch_gemm<Fmt, 64>(p, tm_w, tm_aux, x, x_elem, ld_bytes, ws, ws_bytes, st);
+  return launch_gemm<Fmt, (MAX_N == 64 ? 64 : 128)>(p, tm_w, tm_aux, x, x_elem, ld_bytes, ws, ws_bytes, st);
+}
+
+// int8 / fp8 rowwise
+template <int KIND>
+static int rowwise(const uint8_t* xq, const float* x_scale, int M, int K, const uint8_t* wq, const float* w_scale, int N,
+                   const uint16_t* bias, uint16_t* y, int32_t* i32_out, void* ws, size_t ws_bytes, void* stream) {
+  CUtensorMap tm_w;
+  {
+    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
+    const uint64_t str[1] = {(uint64_t)K};
+    const uint32_t box[2] = {KCHUNK, ROWS};
     int rc = make_tmap(&tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  {
-    const uint64_t dims[2] = {(uint64_t)k_bytes, (uint64_t)M};
-    const uint64_t str[1] = {(uint64_t)k_bytes};
-    const uint32_t box[2] = {KB, (uint32_t)N_MMA};
-    int rc = make_tmap(&tm_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, xq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
-  Params p{};
-  p.x_scale = x_scale; p.w_scale = w_scale;
+  tsg::Params p{};
+  p.row_scale = x_scale;
+  p.w_scale = w_scale;
   p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   p.y = reinterpret_cast<__nv_bfloat16*>(y);
   p.i32_out = i32_out;
-  p.ws_flag = reinterpret_cast<unsigned int*>(ws);
-  p.ws_partial = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws) + streamk::WS_PARTIAL_OFF);
-  p.M = M; p.N = N; p.K = K;
+  p.epi = KIND == KIND_I8 ? tsg::EPI_I8 : tsg::EPI_F8;
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
   p.n_tiles = ceil_div(N, ROWS);
-  p.m_blocks = ceil_div(M, N_MMA);
-  p.KT = ceil_div(k_bytes, KB);   // a K tail is zero-filled by TMA (out-of-bounds box elements) on both operands
-  const int sf_per_row = KIND == KIND_MXF8 ? K / 32 : (KIND == KIND_NVF4 ? K / 16 : 0);
-  p.sf_col_blocks_w = ceil_div(sf_per_row, 4);
-  p.sf_col_blocks_x = ceil_div(sf_per_row, 4);
-  const long long units = (long long)p.n_tiles * p.m_blocks * p.KT;
-  // never fewer than 8 chunks per CTA: finer splits lengthen the split-tile reduction more than they shorten the
-  // streaming phase (fp8, q|k|v projection: 12.6 -> 10.5 us at 1 token, 15.2 -> 13.5 us at 32 with 8 instead of 4; 16 is
-  // worse again: profiles/r02_call_p.log)
-  // two CTAs per SM where they fit (N_MMA <= 64): this kernel has no dequant phase, it is bounded by the bytes in
-  // flight per SM (stages x 16-20 KB against the DRAM round trip), which a second resident CTA doubles
-  const int per_sm = (N_MMA <= 64) ? (ts_ctas_per_sm() ? ts_ctas_per_sm() : 2) : 1;
-  int grid = sm_count() * per_sm;
-  const int min_units = ts_min_units() ? ts_min_units() : 8;
-  if (units / min_units < grid) grid = units / min_units > 0 ? (int)(units / min_units) : 1;
-  const size_t need = streamk::WS_PARTIAL_OFF + (size_t)grid * N_MMA * ROWS * 4;
-  if (!ws || ws_bytes < need || (size_t)grid * 4 > streamk::WS_FLAGS_BYTES)
-    return fail(AO_ERR_WORKSPACE, "lowp linear: workspace too small (%zu < %zu)", ws_bytes, need);
-  auto kern = lowp_linear_kernel<KIND, N_MMA>;
-  AO_CUDA_CHECK(ensure_dynamic_smem(reinterpret_cast<const void*>(kern), C::SMEM_BYTES));
-  AO_CUDA_CHECK(ao::launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, pdl_enabled(), tm_w, tm_x,
-                           w_sf, x_sf, p));
-  return AO_OK;
+  p.KT = ceil_div(K, KCHUNK);   // a K tail is zero-filled by TMA (out-of-bounds box elements) on both operands
+  return dispatch_m<SsFmt<KIND>, (KIND == KIND_F8 ? 64 : 128)>(p, tm_w, tm_w, xq, 1, K, ws, ws_bytes,
+                                                                 reinterpret_cast<cudaStream_t>(stream));
 }
 
+// mxfp8 / nvfp4: activation slabs dequantised into the workspace behind the partial slots, one GEMM per slab
 template <int KIND>
-static int dispatch(const uint8_t* xq, const uint8_t* x_sf, const float* x_scale, int M, int K,
-                    const uint8_t* wq, const uint8_t* w_sf, const float* w_scale, int N,
-                    const uint16_t* bias, uint16_t* y, int32_t* i32_out, void* ws, size_t ws_bytes,
-                    void* stream) {
+static int block_scaled(const uint8_t* xq, const uint8_t* x_sf, const float* a_pts, int M, int K, const uint8_t* wq,
+                        const uint8_t* w_sf, const float* b_pts, int N, const uint16_t* bias, uint16_t* y, void* ws,
+                        size_t ws_bytes, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (M <= 16 && KIND != KIND_MXF8 && KIND != KIND_NVF4)
-    return launch<KIND, 16>(xq, x_sf, x_scale, M, K, wq, w_sf, w_scale, N, bias, y, i32_out, ws, ws_bytes, st);
-  if (M <= 32)
-    return launch<KIND, 32>(xq, x_sf, x_scale, M, K, wq, w_sf, w_scale, N, bias, y, i32_out, ws, ws_bytes, st);
-  if (M <= 64)
-    return launch<KIND, 64>(xq, x_sf, x_scale, M, K, wq, w_sf, w_scale, N, bias, y, i32_out, ws, ws_bytes, st);
-  return launch<KIND, 128>(xq, x_sf, x_scale, M, K, wq, w_sf, w_scale, N, bias, y, i32_out, ws, ws_bytes, st);
+  CUtensorMap tm_w, tm_sf;
+  const int sf_per_row = KIND == KIND_MXF8 ? K / 32 : K / 16;
+  const int sf_col_blocks = ceil_div(sf_per_row, 4);
+  if (KIND == KIND_NVF4) {
+    if (int rc = nvf4w::make_weight_maps(wq, w_sf, N, K, &tm_w, &tm_sf)) return rc;
+  } else {
+    {
+      const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
+      const uint64_t str[1] = {(uint64_t)K};
+      const uint32_t box[2] = {KCHUNK, ROWS};
+      int rc = make_tmap(&tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+      if (rc) return rc;
+    }
+    const uint64_t dims[2] = {128, (uint64_t)ceil_div(N, ROWS) * (uint64_t)sf_col_blocks};
+    const uint64_t str[1] = {512};
+    const uint32_t box[2] = {128, 1};
+    int rc = make_tmap(&tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (rc) return rc;
+  }
+  // the partial slots take at most (SMs x 128 x 128) words; the slab starts on the next MiB
+  const size_t act_off = (streamk::WS_PARTIAL_OFF + (size_t)sm_count() * ROWS * 128 * 4 + (1u << 20) - 1) & ~(size_t)((1u << 20) - 1);
+  const size_t row_bytes = (size_t)K * 2;
+  long long slab = ws && ws_bytes > act_off ? (long long)((ws_bytes - act_off) / row_bytes) : 0;
+  if (slab >= 128) slab &= ~127LL;
+  if (slab < 1)
+    return fail(AO_ERR_WORKSPACE, "block-scaled linear: workspace too small for one bf16 activation row (K=%d)", K);
+  __nv_bfloat16* xb = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<uint8_t*>(ws) + act_off);
+  for (int m0 = 0; m0 < M; m0 += (int)slab) {
+    const int rows = (int)(M - m0 < slab ? M - m0 : slab);
+    const long long threads = (long long)rows * (K / 16);
+    AO_CUDA_CHECK(ao::launch(dequant_act_kernel<KIND>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st,
+                             pdl_enabled(), xq, x_sf, m0, rows, K, sf_col_blocks, xb));
+    tsg::Params p{};
+    p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+    p.y = reinterpret_cast<__nv_bfloat16*>(y) + (size_t)m0 * N;
+    p.epi = tsg::EPI_FLOAT;
+    p.out_scale = KIND == KIND_NVF4 ? b_pts : nullptr;
+    p.out_scale2 = KIND == KIND_NVF4 ? a_pts : nullptr;
+    p.aux_col_blocks = sf_col_blocks;
+    p.M = rows; p.N = N; p.N_out = N; p.K = K;
+    p.n_tiles = ceil_div(N, ROWS);
+    p.KT = ceil_div(K, KCHUNK);   // mxfp8: a K tail is zero-filled by TMA on both operands
+    int rc;
+    if (KIND == KIND_NVF4) {
+      p.acc_exp2 = nvf4w::Nvfp4Fmt::ACC_EXP2;
+      rc = dispatch_m<nvf4w::Nvfp4Fmt>(p, tm_w, tm_sf, xb, 2, K * 2, ws, act_off, st);
+    } else {
+      rc = dispatch_m<Mxfp8Fmt>(p, tm_w, tm_sf, xb, 2, K * 2, ws, act_off, st);
+    }
+    if (rc) return rc;
+  }
+  return AO_OK;
 }
 
 }  // namespace lowp
@@ -460,9 +282,9 @@ extern "C" int ao_int8_dyn_linear(const int8_t* xq, const float* x_scale, int M,
   AO_REQUIRE(N % 8 == 0, "int8 linear: N=%d must be a multiple of 8 (reference: int8/kernels.py:48-58)", N);
   if (M == 0) return AO_OK;
   AO_REQUIRE(xq && x_scale && wq && w_scale && y, "int8 linear: null pointer");
-  return lowp::dispatch<lowp::KIND_I8>(reinterpret_cast<const uint8_t*>(xq), nullptr, x_scale, M, K,
-                                       reinterpret_cast<const uint8_t*>(wq), nullptr, w_scale, N, bias,
-                                       y, nullptr, workspace, workspace_bytes, stream);
+  return lowp::rowwise<lowp::KIND_I8>(reinterpret_cast<const uint8_t*>(xq), x_scale, M, K,
+                                      reinterpret_cast<const uint8_t*>(wq), w_scale, N, bias, y, nullptr, workspace,
+                                      workspace_bytes, stream);
 }
 
 extern "C" int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, int N, int32_t* acc,
@@ -470,9 +292,9 @@ extern "C" int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, 
   AO_REQUIRE(M >= 0 && K > 0 && N > 0 && K % 16 == 0, "int8 mm: bad sizes M=%d K=%d N=%d (K%%16==0)", M, K, N);
   if (M == 0) return AO_OK;
   AO_REQUIRE(xq && wq && acc, "int8 mm: null pointer");
-  return lowp::dispatch<lowp::KIND_I8>(reinterpret_cast<const uint8_t*>(xq), nullptr, nullptr, M, K,
-                                       reinterpret_cast<const uint8_t*>(wq), nullptr, nullptr, N, nullptr,
-                                       nullptr, acc, workspace, workspace_bytes, stream);
+  return lowp::rowwise<lowp::KIND_I8>(reinterpret_cast<const uint8_t*>(xq), nullptr, M, K,
+                                      reinterpret_cast<const uint8_t*>(wq), nullptr, N, nullptr, nullptr, acc, workspace,
+                                      workspace_bytes, stream);
 }
 
 extern "C" int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, int M, int K,
@@ -484,8 +306,8 @@ extern "C" int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, in
   AO_REQUIRE(N % 16 == 0, "fp8 linear: N=%d must be a multiple of 16 (reference: quantization/utils.py:663-687)", N);
   if (M == 0) return AO_OK;
   AO_REQUIRE(xq && x_scale && wq && w_scale && y, "fp8 linear: null pointer");
-  return lowp::dispatch<lowp::KIND_F8>(xq, nullptr, x_scale, M, K, wq, nullptr, w_scale, N, bias, y, nullptr,
-                                       workspace, workspace_bytes, stream);
+  return lowp::rowwise<lowp::KIND_F8>(xq, x_scale, M, K, wq, w_scale, N, bias, y, nullptr, workspace, workspace_bytes,
+                                      stream);
 }
 
 extern "C" int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,
@@ -496,8 +318,8 @@ extern "C" int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked
   AO_REQUIRE(K % 32 == 0, "mxfp8 linear: K=%d must be a multiple of 32 (mx_tensor.py:244-246)", K);
   if (M == 0) return AO_OK;
   AO_REQUIRE(xq && x_scale_blocked && wq && w_scale_blocked && y, "mxfp8 linear: null pointer");
-  return lowp::dispatch<lowp::KIND_MXF8>(xq, x_scale_blocked, nullptr, M, K, wq, w_scale_blocked, nullptr, N,
-                                         bias, y, nullptr, workspace, workspace_bytes, stream);
+  return lowp::block_scaled<lowp::KIND_MXF8>(xq, x_scale_blocked, nullptr, M, K, wq, w_scale_blocked, nullptr, N, bias,
+                                             y, workspace, workspace_bytes, stream);
 }
 
 extern "C" int ao_nvfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, const float* a_pts,
@@ -509,6 +331,6 @@ extern "C" int ao_nvfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked
   AO_REQUIRE(N % 16 == 0, "nvfp4 linear: N=%d must be a multiple of 16 (inference_workflow.py:248-251)", N);
   if (M == 0) return AO_OK;
   AO_REQUIRE(xq && x_scale_blocked && wq && w_scale_blocked && y, "nvfp4 linear: null pointer");
-  return lowp::dispatch<lowp::KIND_NVF4>(xq, x_scale_blocked, a_pts, M, K, wq, w_scale_blocked, b_pts, N, bias,
-                                         y, nullptr, workspace, workspace_bytes, stream);
+  return lowp::block_scaled<lowp::KIND_NVF4>(xq, x_scale_blocked, a_pts, M, K, wq, w_scale_blocked, b_pts, N, bias, y,
+                                             workspace, workspace_bytes, stream);
 }

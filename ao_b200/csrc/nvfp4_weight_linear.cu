@@ -4,121 +4,32 @@
 // weight-only handler inference_workflow.py:356-400), with an optional per-token activation scale applied in
 // the epilogue so that e4m3-rowwise-quantised activations (BASELINE config 5; SURVEY section 0-5) run on the
 // same kernel: their values are exact in bf16, the scale is a row factor.
-// tcgen05 has no nvfp4 x bf16/fp8 MMA kind, so the weights are dequantised in-kernel to bf16 (exact: 2
-// significant bits x 4 significant bits) and fed from TMEM exactly like the int4 path (ts_gemm.cuh); the
-// per-tensor scale is applied in fp32 in the epilogue.
-//
-// e2m1 -> bf16 without a table: nibble x = (s e1 e0 m) placed at bf16 bits 15|8:6 is the bf16 number
-// value(x) * 2^-126 (denormal for e = 0, which bf16 multiplies handle exactly); ONE exact multiply by
-// (block_scale * 2^66) gives value(x) * block_scale * 2^-60, and the 2^60 is taken back out of the fp32 accumulator in the
-// epilogue (Params::acc_exp2; power-of-two factors commute with every rounding on the way).  bf16(block_scale * 2^66) =
-// (byte << 4) + 0x5D00 for the (always normal, >= 2^-6) e4m3 scale bytes.
+// Hopper has no fp4 tensor-core kind, so the weights are dequantised in-kernel to the bf16 wgmma A fragment (exact,
+// nvfp4_fmt.cuh) and run through the int4 path's kernel (ts_gemm.cuh); the per-tensor scale is applied in fp32 in
+// the epilogue.
 #include <cuda_bf16.h>
 #include <cuda_fp8.h>
 
 #include "common.h"
+#include "nvfp4_fmt.cuh"
 #include "ptx.cuh"
 #include "ts_gemm.cuh"
-#include "ts_prefill.cuh"
 
 namespace ao {
 namespace nvf4w {
 
-using tsg::KCHUNK;
 using tsg::ROWS;
-using tsg::W_BYTES;
 
-struct Nvfp4Fmt {
-  __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES + 1024; }
-  __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap* tm_sf, const tsg::Params& p,
-                                                 uint8_t* w_dst, uint8_t* aux_dst, uint64_t* bar, int n_tile, int kc,
-                                                 uint64_t policy) {
-    tma_load_2d(w_dst, tm_w, bar, kc * 64, n_tile * ROWS, policy);  // 128 rows x 64 bytes, 64B swizzle
-    // two consecutive blocked scale tiles (128 rows x 4 scales each = 64 k per tile): the blocked scale tensor is a
-    // [row block][column block] array of contiguous 512-byte tiles = a 2-D tensor of 128 words x tiles
-    tma_load_2d(aux_dst, tm_sf, bar, 0, n_tile * p.aux_col_blocks + kc * 2, policy);
-  }
-  __device__ static __forceinline__ void prefetch_w(const CUtensorMap* tm_w, const CUtensorMap* tm_sf, const tsg::Params& p, int n_tile, int kc) {
-    tma_prefetch_l2_2d(tm_w, kc * 64, n_tile * ROWS);
-    tma_prefetch_l2_2d(tm_sf, 0, n_tile * p.aux_col_blocks + kc * 2);
-  }
-  // one weight row of the chunk: its 64 bytes (k 0..127, even k in the low nibble) and the 8 block scales
-  struct Raw {
-    uint4 v[4];
-    uint32_t sc[2];   // blocked tile h (k 64h..64h+63): four e4m3 scale bytes
-  };
-  __device__ static __forceinline__ void load_row(const tsg::Params&, uint32_t w_smem, uint32_t aux_smem, int r, Raw& raw) {
-    const uint32_t sc_off = (uint32_t)(r & 31) * 16u + (uint32_t)(r >> 5) * 4u;
-    raw.sc[0] = tsg::lds32(aux_smem + sc_off);
-    raw.sc[1] = tsg::lds32(aux_smem + 512 + sc_off);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint32_t off = (uint32_t)r * 64u + i * 16;
-      raw.v[i] = tsg::lds128(w_smem + (off ^ (((off >> 7) & 3) << 4)));  // undo the TMA 64B swizzle
-    }
-  }
-  // depends on one destination register of every ld.shared of load_row (see Int4Fmt::touch)
-  __device__ static __forceinline__ uint32_t touch(const Raw& raw) {
-    return raw.v[0].x ^ raw.v[1].x ^ raw.v[2].x ^ raw.v[3].x ^ raw.sc[0] ^ raw.sc[1];
-  }
-  // quarter q = bytes 16q..16q+15 of the row = k 32q..32q+31: out[c] = bf16x2 of k pair (32q + 2c, +1)
-  __device__ static __forceinline__ void dequant_quarter(const tsg::Params&, const Raw& raw, int q, uint32_t (&out)[16]) {
-    const uint4 v = raw.v[q];
-    const uint32_t sc = raw.sc[q >> 1] >> (16 * (q & 1));   // two scale bytes: blocks 2q, 2q + 1
-#pragma unroll
-    for (int w = 0; w < 4; ++w) {  // word w = k 8w..8w+7 of the quarter; scale block = w/2
-      const uint32_t word = w == 0 ? v.x : w == 1 ? v.y : w == 2 ? v.z : v.w;
-      const uint32_t sb = (sc >> (8 * (w >> 1))) & 0xFFu;
-      // bf16x2 of scale * 2^66: the e4m3 byte re-biased (<< 4, + (127 - 7 + 66) << 7).  2^66 = 2^126 (undoes the
-      // denormal placement below) * 2^-60 (ACC_EXP2: taken back out in the epilogue, in fp32) -- one exact multiply per
-      // pair instead of two; the product value * scale * 2^-60 has at most 6 significant bits and is far inside the
-      // normal bf16 range
-      const uint32_t s_bits = ((sb << 4) + 0x5D00u) * 0x00010001u;
-      const __nv_bfloat162 s2 = *reinterpret_cast<const __nv_bfloat162*>(&s_bits);
-      const uint32_t lo = word & 0x0F0F0F0Fu, hi = (word >> 4) & 0x0F0F0F0Fu;   // even / odd k, one nibble per byte
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        // hh = nibble of k = 8w + 2j in bits 3:0, of k + 1 in bits 19:16: one prmt (selector nibble 8|j replicates the
-        // sign bit of a byte < 16: zero)
-        uint32_t hh;
-        asm("prmt.b32 %0, %1, %2, %3;" : "=r"(hh) : "r"(lo), "r"(hi), "r"((uint32_t)(((8 | j) << 12) | ((4 + j) << 8) | ((8 | j) << 4) | j)));
-        const uint32_t bits = (hh * 0x1040u) & 0x81C081C0u;           // sign | e1 e0 m at bf16 bits 15 | 8:6 = value * 2^-126
-        __nv_bfloat162 x = *reinterpret_cast<const __nv_bfloat162*>(&bits);
-        x = __hmul2(x, s2);
-        out[4 * w + j] = *reinterpret_cast<uint32_t*>(&x);
-      }
-    }
-  }
-  static constexpr int ACC_EXP2 = 60;   // the accumulators hold the result * 2^-60 (Params::acc_exp2)
-};
-
-// N_MMA = tokens per tile of the decode kernel (16 .. 128), or 0 = the prefill-shaped kernel (ts_prefill.cuh, 256 tokens)
 template <int N_MMA>
 static int launch_tc(const uint16_t* x, int ldx, const float* x_scale, int M, int K, const uint8_t* wq, const uint8_t* w_sf,
                      const float* b_pts, int b_pts_per_row, int N, const uint16_t* bias, uint16_t* y, void* ws,
                      size_t ws_bytes, cudaStream_t stream) {
-  constexpr bool PREFILL = N_MMA == 0;
-  constexpr int TOK = PREFILL ? tsp::N_TOK : N_MMA;
-  CUtensorMap tm_w, tm_x;
-  {
-    const uint64_t dims[2] = {(uint64_t)K / 2, (uint64_t)N};
-    const uint64_t str[1] = {(uint64_t)K / 2};
-    const uint32_t box[2] = {64, 128};
-    int rc = make_tmap(&tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B);
-    if (rc) return rc;
-  }
-  CUtensorMap tm_sf;
-  {
-    const uint64_t dims[2] = {128, (uint64_t)ceil_div(N, ROWS) * (uint64_t)ceil_div(K / 16, 4)};
-    const uint64_t str[1] = {512};
-    const uint32_t box[2] = {128, 2};
-    int rc = make_tmap(&tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-    if (rc) return rc;
-  }
+  CUtensorMap tm_w, tm_sf, tm_x;
+  if (int rc = make_weight_maps(wq, w_sf, N, K, &tm_w, &tm_sf)) return rc;
   {
     const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
     const uint64_t str[1] = {(uint64_t)ldx * 2};
-    const uint32_t box[2] = {64, (uint32_t)TOK};
+    const uint32_t box[2] = {64, (uint32_t)N_MMA};
     int rc = make_tmap(&tm_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
@@ -128,28 +39,14 @@ static int launch_tc(const uint16_t* x, int ldx, const float* x_scale, int M, in
   p.out_scale = b_pts;
   p.out_scale_per_row = b_pts_per_row;
   p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.aux_base = w_sf;
+  p.epi = tsg::EPI_FLOAT;
   p.acc_exp2 = Nvfp4Fmt::ACC_EXP2;
   p.aux_col_blocks = ceil_div(K / 16, 4);
   p.M = M; p.N = N; p.N_out = N; p.K = K; p.group_size = 16;
   p.n_tiles = ceil_div(N, ROWS);
-  p.m_blocks = ceil_div(M, TOK);
+  p.m_blocks = ceil_div(M, N_MMA);
   p.KT = K / 128;
-  int grid = 0;
-  if constexpr (PREFILL) {
-    if (int rc = tsp::plan(p, ws, ws_bytes, "nvfp4 weight linear (prefill)", &grid)) return rc;
-    auto kern = tsp::ts_prefill_kernel<Nvfp4Fmt>;
-    AO_CUDA_CHECK(ensure_dynamic_smem(reinterpret_cast<const void*>(kern), tsp::SMEM_BYTES));
-    AO_CUDA_CHECK(launch(kern, dim3(grid), dim3(tsp::NUM_THREADS), tsp::SMEM_BYTES, stream, pdl_enabled(), tm_w, tm_sf, tm_x, p));
-  } else {
-    using C = tsg::Cfg<(PREFILL ? 128 : N_MMA)>;
-    if (int rc = tsg::plan<(PREFILL ? 128 : N_MMA)>(p, ws, ws_bytes, "nvfp4 weight linear", &grid)) return rc;
-    p.timeline = nullptr;
-    auto kern = tsg::ts_gemm_kernel<Nvfp4Fmt, (PREFILL ? 128 : N_MMA)>;
-    AO_CUDA_CHECK(ensure_dynamic_smem(reinterpret_cast<const void*>(kern), C::SMEM_BYTES));
-    AO_CUDA_CHECK(launch(kern, dim3(grid), dim3(tsg::NUM_THREADS), C::SMEM_BYTES, stream, pdl_enabled(), tm_w, tm_sf, tm_x, p));
-  }
-  return AO_OK;
+  return tsg::launch_gemm<Nvfp4Fmt, N_MMA>(p, tm_w, tm_sf, tm_x, ws, ws_bytes, "nvfp4 weight linear", stream);
 }
 
 // per-token e4m3 "fake quantisation": x -> bf16(e4m3(x / s)) and s = f32(bf16(amax/448)); the bf16 values
@@ -237,9 +134,7 @@ extern "C" int ao_nvfp4_weight_linear_ex(const uint16_t* x, int ldx, const float
   if (M <= 16) return nvf4w::launch_tc<16>(x, ldx, x_scale, M, K, wq, w_scale_blocked, b_pts, b_pts_per_row, N, bias, y, workspace, workspace_bytes, st);
   if (M <= 32) return nvf4w::launch_tc<32>(x, ldx, x_scale, M, K, wq, w_scale_blocked, b_pts, b_pts_per_row, N, bias, y, workspace, workspace_bytes, st);
   if (M <= 64) return nvf4w::launch_tc<64>(x, ldx, x_scale, M, K, wq, w_scale_blocked, b_pts, b_pts_per_row, N, bias, y, workspace, workspace_bytes, st);
-  if (!tsp::worth_it(M, N, K))
-    return nvf4w::launch_tc<128>(x, ldx, x_scale, M, K, wq, w_scale_blocked, b_pts, b_pts_per_row, N, bias, y, workspace, workspace_bytes, st);
-  return nvf4w::launch_tc<0>(x, ldx, x_scale, M, K, wq, w_scale_blocked, b_pts, b_pts_per_row, N, bias, y, workspace, workspace_bytes, st);
+  return nvf4w::launch_tc<128>(x, ldx, x_scale, M, K, wq, w_scale_blocked, b_pts, b_pts_per_row, N, bias, y, workspace, workspace_bytes, st);
 }
 
 extern "C" int ao_nvfp4_weight_linear(const uint16_t* x, const float* x_scale, int M, int K, const uint8_t* wq,

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (TMEM alloc / ld / st / cp / mma / commit), PDL.  No CUTLASS/CuTe.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), PDL, wgmma shared-memory
+// descriptors (the wgmma instructions themselves are in wgmma.cuh).  No CUTLASS/CuTe.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -85,187 +85,23 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const void* tmap, uint64_
       : "memory");
 }
 
-// HBM -> L2 only (no shared memory, no barrier): run ahead of the ring
-__device__ __forceinline__ void tma_prefetch_l2_2d(const void* tmap, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(tmap), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_l2_3d(const void* tmap, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(tmap), "r"(c0), "r"(c1),
-               "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_prefetch_l2(const void* gptr, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gptr), "r"(bytes) : "memory");
-}
-
 // ---------------------------------------------------------------- PDL
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-#define AO_DEF_MMA_SS(NAME, KIND)                                                              \
-  __device__ __forceinline__ void NAME(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,     \
-                                       uint32_t idesc, uint32_t accumulate) {                 \
-    asm volatile(                                                                              \
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"                                      \
-        "tcgen05.mma.cta_group::1.kind::" KIND " [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),  \
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)                                  \
-        : "memory");                                                                           \
-  }
-AO_DEF_MMA_SS(mma_ss_f16, "f16")
-AO_DEF_MMA_SS(mma_ss_i8, "i8")
-AO_DEF_MMA_SS(mma_ss_f8f6f4, "f8f6f4")
-#undef AO_DEF_MMA_SS
-
-// D[tmem] (+)= A[tmem] * B[smem desc]   (A: lane = row, 32-bit column = 2 bf16 along K)
-__device__ __forceinline__ void mma_ts_f16(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                           uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ts_f8f6f4(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// block-scaled: scale factors in TMEM
-__device__ __forceinline__ void mma_ss_mxf8f6f4(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                                uint32_t idesc, uint32_t accumulate,
-                                                uint32_t sfa_tmem, uint32_t sfb_tmem) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}\n" ::
-          "r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(sfa_tmem), "r"(sfb_tmem)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ss_mxf4nvf4_b16(uint32_t d_tmem, uint64_t a_desc,
-                                                    uint64_t b_desc, uint32_t idesc,
-                                                    uint32_t accumulate, uint32_t sfa_tmem,
-                                                    uint32_t sfb_tmem) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf4nvf4.block_scale.block16 [%0], %1, %2, %3, [%5], [%6], "
-      "p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(sfa_tmem), "r"(sfb_tmem)
-      : "memory");
-}
-// smem (descriptor) -> TMEM copy of 32 rows x 128 bit, replicated to the 4 lane quarters
-__device__ __forceinline__ void tc_cp_32x128b_warpx4(uint32_t dst_tmem, uint64_t src_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(dst_tmem), "l"(src_desc)
-               : "memory");
-}
-
-// ---- descriptors -----------------------------------------------------------------
-// K-major operand tile in shared memory, 128-byte swizzle (what TMA SWIZZLE_128B writes):
-// row r at byte r*128, 16-byte chunks XOR-ed with (r%8); 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// ---------------------------------------------------------------- wgmma descriptors
+// K-major operand tile in shared memory, 128-byte swizzle (what TMA SWIZZLE_128B writes): row r at byte r*128,
+// 16-byte chunks XOR-ed with (r%8); 8-row groups 1024 B apart (stride byte offset).  The tile base is 1024-byte
+// aligned; a K step inside the 128-byte row advances the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);  // start address  [0,14)
-  d |= (uint64_t)1 << 16;                       // leading byte offset (unused for SW128 K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset: 8 rows * 128 B
-  d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                       // layout type: SWIZZLE_128B
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);  // start address      [0,14)
+  d |= (uint64_t)1 << 16;                       // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset  [32,46)
+  d |= (uint64_t)1 << 62;                       // layout type [62,64): 1 = SWIZZLE_128B
   return d;
-}
-// K-major, no swizzle ("interleave"): 8x16B core matrices; LBO = byte distance between
-// core matrices adjacent in K, SBO = between core matrices adjacent in M/N.
-__device__ __forceinline__ uint64_t umma_desc_k_noswz(uint32_t smem_addr, uint32_t lbo,
-                                                      uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(lbo >> 4) << 16;
-  d |= (uint64_t)(sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-
-// instruction descriptor (dense kinds): c_format [4,6) a_format [7,10) b_format [10,13)
-// a_major bit15 b_major bit16 (0 = K-major)  n>>3 [17,23)  m>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t c_fmt, uint32_t a_fmt, uint32_t b_fmt,
-                                                  uint32_t M, uint32_t N) {
-  return (c_fmt << 4) | (a_fmt << 7) | (b_fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// block-scaled kinds: b_sf_id [4,6) a_format [7,10) b_format [10,13) n>>3 [17,23)
-// scale_format bit23 (0 = ue4m3, 1 = ue8m0) m>>4 [24,29) a_sf_id [29,31)
-__host__ __device__ constexpr uint32_t make_idesc_bs(uint32_t a_fmt, uint32_t b_fmt,
-                                                     uint32_t scale_fmt, uint32_t M, uint32_t N) {
-  return (a_fmt << 7) | (b_fmt << 10) | ((N >> 3) << 17) | (scale_fmt << 23) | ((M >> 4) << 24);
-}
-
-// ---- TMEM <-> registers (32 lanes x 32 bit; thread i of the warp owns lane base+i) ----
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]),
-      "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]),
-      "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-      "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]),
-      "r"(r[15])
-      : "memory");
 }
 
 }  // namespace ao

@@ -1,16 +1,16 @@
 // Persistent stream-K work split and the split-tile ("fix-up") protocol shared by the decode GEMM kernels
-// (ts_gemm.cuh: int4 / nvfp4-weight TS-mode kernel, lowp_linear.cu: int8 / fp8 / mxfp8 / nvfp4 SS-mode kernel).
+// (ts_gemm.cuh, for every weight format).
 //
 // Work split.  The GEMM is n_tiles x m_blocks output tiles (128 weight rows x N_MMA tokens) times KT chunks of
 // 128 k: U = tiles * KT units, unit u = (tile u / KT, chunk u % KT).  CTA b of G owns the contiguous range
 // [U*b/G, U*(b+1)/G): every SM streams the same number of bytes whatever N and K are.  A CTA's range is a
-// sequence of SEGMENTS (maximal runs of units of one tile), each accumulated in its own TMEM buffer:
+// sequence of SEGMENTS (maximal runs of units of one tile), each accumulated in registers in turn:
 //   FULL     all KT chunks of the tile: the epilogue writes the outputs directly
 //   CONTRIB  starts at chunk > 0 (only ever the CTA's FIRST segment): the CTA is not the tile's first
 //            contributor; it publishes its partial sums to its workspace slot and raises its flag
 //   OWNER    starts at chunk 0 but the CTA's range ends before the tile does (only ever the CTA's LAST
 //            segment): the remaining chunks belong to CTAs b+1 .. b_last, each of which holds them as its
-//            CONTRIB segment.  The owner keeps its partial in TMEM, waits for the contributors' flags, adds
+//            CONTRIB segment.  The owner keeps its partial in registers, waits for the contributors' flags, adds
 //            their partials in CTA order (= k order: fixed, so results are bit-reproducible run to run) and
 //            writes the outputs.
 // Compared with a symmetric "last arriver reduces" protocol this takes the owner's own partial, every atomic
@@ -20,8 +20,7 @@
 // have no other work do publish and gather run back to back.
 //
 // Workspace (caller-owned, zero-initialised once): flags uint32[grid] at +0 (0 = empty, 1 = published; the owner
-// resets the flags it consumed, so the buffer is all-zero again when the kernel ends), bring-up timeline at
-// +48 KiB, partial slots [grid][N_MMA * 128] 32-bit words at +64 KiB (slot b = CTA b's CONTRIB partial,
+// resets the flags it consumed, so the flags are all-zero again when the kernel ends), partial slots [grid][N_MMA * 128] 32-bit words at +64 KiB (slot b = CTA b's CONTRIB partial,
 // column-major: word (j, r) at j * 128 + r).
 //
 // Forward progress: an owner spins on flags of CTAs with HIGHER block indices.  The launchers keep the grid at or
@@ -35,7 +34,6 @@ namespace streamk {
 
 constexpr int ROWS = 128;
 constexpr size_t WS_FLAGS_BYTES = 16 * 1024;      // up to 4096 CTAs
-constexpr size_t WS_TIMELINE_OFF = 48 * 1024;     // bring-up only
 constexpr size_t WS_PARTIAL_OFF = 64 * 1024;
 
 __device__ __forceinline__ int unit_begin(int b, long long U, int G) { return (int)((U * b) / G); }

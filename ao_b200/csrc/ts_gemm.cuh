@@ -1,111 +1,74 @@
-// Persistent "dequantise-into-TMEM" decode GEMM for sub-byte weights with bf16 activations (sm_100a).
+// Persistent stream-K GEMM on Hopper wgmma (sm_90a) for every quantized linear of the library.
 //
-//   Y[M,N] = X[M,K] * W^[N,K]^T (+bias),   W^ produced in-kernel from 4-bit weights + group scales
+//   Y[M,N] = X[M,K] * W^[N,K]^T (+bias),   W^ = the weights, dequantised in-kernel where the format needs it
 //
-// Used by int4_linear.cu (tinygemm tile-packed int4, W^ = bf16((q-8)s+z)) and
-// nvfp4_weight_linear.cu (e2m1 * e4m3 block scale).  Structure:
-//   * swap-AB: 128 weight rows = UMMA M, tokens = UMMA N (16..128), fp32 accumulator in TMEM
-//   * persistent stream-K (streamk.cuh): the (tile, 128-k chunk) units of the whole GEMM are split EVENLY over
-//     the CTAs; split tiles are finished by their OWNER CTA from the contributors' published partials
-//   * 16 warps in four warpgroups, 64 registers per thread, 256 TMEM columns, ~105 KB smem (two CTAs fit per SM,
-//     so the next linear's CTA is resident -- PDL -- and has its weights in flight while this one finishes):
-//       WG0..WG2 (warps 0-11): dequant, chunk i belongs to warpgroup i % 3: the thread's weight row into registers
-//                  (conflict-free ld.shared.v4; the weight stage is handed back right away), unpack/scale in bf16x2
-//                  a quarter row (16 registers) at a time -> tcgen05.st.x16 of the bf16 A operand into one of the
-//                  TMEM A stages.  A chunk is a serial chain of waits (weights landed, A stage free, TMEM store
-//                  done) around ~400 instructions, so what counts is how many chunks are in flight per SM: three.
-//                  The same warpgroups run the epilogues (tcgen05.ld of a finished accumulator -- double-buffered
-//                  in TMEM, so it overlaps the next segment's MMAs -- bias / scales, store or publish): the
-//                  warpgroup that dequantised a segment's last chunk finishes the segment after its NEXT chunk,
-//                  when the accumulator is long complete, so nothing ever blocks on the tensor pipe mid-stream
-//       WG3: warps 12 and 15 weight TMA producers (alternate chunks; never wait for the previous kernel), warp 14
-//                  activation TMA producer (after griddepcontrol.wait), warp 13 MMA issuer
-//   * the weight stream is what the kernel is made of, and it depends on nothing: a CTA that is resident under the
-//     previous kernel (PDL) fills its ring while it waits for its activations.  (An L2 prefetch ahead of the ring --
-//     cp.async.bulk.prefetch.tensor -- was measured neutral to slightly negative and removed: profiles/r02_call_b.log.
-//     So was prefetching the NEXT linear's packed weights into L2 from this kernel's tail, by cp.async.bulk.prefetch.L2
-//     or per-line prefetch.global.L2, whole or capped, early or late: never faster, the bulk form up to 4x slower because
-//     it queues in front of the SM's TMA loads; profiles/r02_call_l.log, r02_call_m.log, scripts/attic)
-//   * single-thread roles are WARP-UNIFORM loops with only the tcgen05 / TMA / mbarrier instruction under elect.sync
-//     (warp index through __shfl_sync so the compiler knows it is uniform): with a loop under `lane == 0` ptxas wraps
-//     every UTCHMMA / UTMALDG in an elect-broadcast loop and one thread issues an MMA only every ~52 cycles instead
-//     of ~20, the tensor pipe's own floor for M128 N16 K16 (scripts/mma_microbench7.cu)
-//   * the issuer does ONE wait and ONE commit per chunk: chunk i owns "chunk slot" i % X_SLOTS = its activation
-//     tile in shared memory plus a barrier pair (cfull = 4 dequant-warp arrivals + the activation tile's TMA
-//     transaction bytes; one tcgen05.commit on cempty says "the MMAs of chunk i are done": the activation slot is
-//     free for chunk i + X_SLOTS and the TMEM A stage i % A_STAGES for chunk i + A_STAGES).  The activation ring is
-//     DEEPER than the TMEM A ring on purpose: an activation tile can only be requested when its slot frees, its TMA
-//     load queues behind the weight boxes already in the SM's TMA unit, and the MMA of its chunk cannot issue before
-//     it lands -- with the rings tied together (round 1: 3 + 3) that latency, not dequant or HBM, set the chunk rate
-//   * the CTA's last segment is on the kernel's critical path: when it is an OWNER segment with more than 8 token
-//     columns, all four warpgroups share the gather (each takes every fourth group of 8 columns)
-//   * PDL: griddepcontrol.launch_dependents at start; only activations / outputs / workspace wait
-//     (griddepcontrol.wait) for the previous kernel.
+// Swap-AB: 128 weight rows of a tile are the wgmma M dimension (two consumer warpgroups of 64 rows each), the tokens
+// are the wgmma N dimension (N_MMA = 16..128).  A format policy (Fmt) decides how the weights reach the tensor core:
+//   * register-A (Fmt::SS == false): int4 tinygemm, nvfp4, mxfp8 weights.  Each consumer thread loads the packed
+//     weights of its two fragment rows straight from the TMA-filled stage and dequantises them into the bf16 A
+//     fragment of wgmma.m64nNk16 (4 x bf16x2 per k16 step); the activations (bf16) are the shared-memory B operand
+//   * shared-memory A (Fmt::SS == true): int8 x int8 -> s32 and e4m3 x e4m3 -> f32 (wgmma k32), both operands are
+//     the TMA tiles themselves
+// Roles (384 threads): warpgroup 0 = one TMA producer warp (weights first: they never depend on the previous kernel;
+// activations after griddepcontrol.wait), warpgroups 1 and 2 = consumers (dequant, wgmma, epilogue).  A stage holds
+// one 128-k chunk: weights + scales (wfull) and the activation tile (xfull); the 8 consumer warps hand it back
+// (sempty) once the wgmmas that read it have completed.  The wgmmas of chunk i run while chunk i+1 is dequantised.
+//
+// Work split (streamk.cuh): the (tile, chunk) units are split evenly over the CTAs; the accumulator of a segment lives
+// in registers and is finished by the consumers right after the segment's last chunk (FULL: outputs, CONTRIB: publish
+// the partial + flag, OWNER: add the contributors' partials in CTA order, then outputs).
 #pragma once
 #include <cuda_bf16.h>
 
 #include "common.h"
 #include "ptx.cuh"
 #include "streamk.cuh"
+#include "wgmma.cuh"
 
 namespace ao {
 namespace tsg {
 
 using streamk::ROWS;
 constexpr int KCHUNK = 128;
-constexpr int W_BYTES = ROWS * KCHUNK / 2;  // 8 KiB of 4-bit weights per chunk
-constexpr int AUX_BYTES = 2048;             // scales per chunk (<= 2 KiB), 1 KiB aligned slot
-constexpr int A_COLS = 64;                  // TMEM columns of one bf16 A stage (128 k / 2)
-constexpr int DEQ_WGS = 3, DEQ_WARPS = 4 * DEQ_WGS, TMA_WARP = 12, MMA_WARP = 13, XTMA_WARP = 14, TMA_WARP1 = 15;
-constexpr int WSTAGE_BYTES = W_BYTES + AUX_BYTES;  // one weight stage: packed nibbles + scales
-constexpr int NUM_THREADS = 16 * 32;
+constexpr int NUM_THREADS = 384;
+constexpr int CONSUMER_WARPS = 8;
+constexpr int SMEM_BUDGET = 200 * 1024;   // of the 227 KB a block may use on H100: one CTA per SM
+constexpr int MAX_STAGES = 12;
 
-// DBUF = accumulator buffers (2: the epilogue of a segment overlaps the next segment's MMAs)
-template <int N_MMA, int DBUF = 2, int XS = 0>
-struct Cfg {
-  static constexpr int X_BYTES = 2 * N_MMA * 128;   // activation tile of one chunk (two 64-k swizzle atoms)
-  static constexpr int TMEM_COLS = N_MMA <= 64 ? 256 : 512;
-  static constexpr int D_COLS = DBUF * N_MMA;
-  static constexpr int A_COL0 = D_COLS <= 64 ? 64 : (D_COLS <= 128 ? 128 : 256);
-  static constexpr int A_STAGES = (TMEM_COLS - A_COL0) / A_COLS;  // 3, 2 or 4 TMEM A stages
-  // chunk slots = depth of the activation ring (see the header): 6 x 4 / 8 KB for the decode sizes
-  static constexpr int X_SLOTS = N_MMA <= 32 ? (XS ? XS : 3) : (N_MMA <= 64 ? 3 : 4);
-  static constexpr int BUDGET = N_MMA <= 64 ? 110 * 1024 : 190 * 1024;
-  // weight stages (8, 8, 6, 6).  A stage is consumed by whichever warpgroup its chunk belongs to, and a parity wait
-  // must never be TWO phases ahead of its barrier (waiting for chunk i + STAGES to land while chunk i has not landed
-  // yet returns at once: the stale phase has the same parity).  Two ways to rule that out:
-  //   * STAGES % 3 == 0: a stage always belongs to the same warpgroup, which takes its chunks in order;
-  //   * STAGES >= A_STAGES + 3: the warpgroup that wants chunk i + STAGES has stored chunk i + STAGES - 3 before,
-  //     which needed the MMAs of chunk i + STAGES - 3 - A_STAGES >= i, which needed chunk i dequantised.
-  // (Round 2 found the 128-token variant with 4 stages / 4 A stages violating both: sporadic wrong results and
-  // launch failures at 65..128 tokens; profiles/r02_call_k.log.)
-  static constexpr int STAGES_RAW = (BUDGET - X_SLOTS * X_BYTES) / WSTAGE_BYTES;
-  static constexpr int STAGES = STAGES_RAW >= 6 ? (STAGES_RAW & ~1) : STAGES_RAW;   // even when there is room: two producers
-  static_assert(STAGES % 3 == 0 || STAGES >= A_STAGES + 3, "weight-stage parity waits could alias (see above)");
-  static constexpr int X_OFF = STAGES * WSTAGE_BYTES;
-  static constexpr int BAR_OFF = X_OFF + X_SLOTS * X_BYTES;
-  static constexpr size_t SMEM_BYTES = (size_t)BAR_OFF + 1024 + 1024;
-  __host__ __device__ static constexpr int d_col(int buf) { return buf * N_MMA; }
-};
+// Epilogue arithmetic, per kind (must stay what each format's reference computes, see Params)
+enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2 };
 
 struct Params {
   const __nv_bfloat16* bias;
-  const float* row_scale;   // optional per-token scale [M] applied in the epilogue (fp8 activations)
-  const float* out_scale;   // optional scale applied in the epilogue: a device scalar (nvfp4 per-tensor scale) or,
-  int out_scale_per_row;    // when set, one value per output feature [N] (fused group of nvfp4 weights)
+  const float* row_scale;   // EPI_FLOAT: optional per-token scale [M]; EPI_I8 / EPI_F8: the activation scale [M]
+  const float* out_scale;   // EPI_FLOAT: optional device scalar, or (out_scale_per_row) one value per output feature
+  const float* out_scale2;  // EPI_FLOAT: optional second device scalar multiplied into out_scale (nvfp4 a_pts * b_pts)
+  int out_scale_per_row;
   int acc_exp2;             // the accumulators hold the result * 2^-acc_exp2 (format policy folds a power of two into
                             // its dequant multiply); undone in the epilogue together with out_scale
+  const float* w_scale;     // EPI_I8 / EPI_F8: per-output-feature weight scale [N]
+  int epi;
   __nv_bfloat16* y;         // [M, N_out]
+  int32_t* i32_out;         // EPI_I8: raw int32 accumulators [M, N] instead of y
   float* ws_partial;        // [grid][N_MMA*128]   CTA b's CONTRIB partial (streamk.cuh)
   unsigned int* ws_flag;    // [grid]              CTA b's partial is published
-  const uint8_t* aux_base;  // format-specific scale base pointer (nvfp4: blocked scales)
   int M, N, N_out, K, group_size;
-  int n_tiles, m_blocks, KT;   // KT = K/128
-  int aux_col_blocks;
-  int producers; // weight TMA producer warps (1 or 2)
-  int prefetch;  // bring-up: L2 prefetch distance in chunks (0 = off)
-  int flags;  // bring-up switches (AO_B200_TS_FLAGS, results are garbage): 1 = skip dequant arithmetic + TMEM stores, 2 = skip MMAs, 4 = no activation loads after the first ring-full
-  unsigned long long* timeline;  // debug: per-CTA [16] timestamps (AO_B200_TIMELINE=1), else null
+  int n_tiles, m_blocks, KT;   // KT = chunks of 128 k
+  int aux_col_blocks;          // blocked block-scale layouts: 4-scale column blocks per 128-row block
+};
+
+template <class Fmt, int N_MMA>
+struct Cfg {
+  static constexpr int X_BYTES = N_MMA * KCHUNK * Fmt::X_ELEM_BYTES;   // activation tile of one chunk
+  static constexpr int X_ATOMS = Fmt::X_ELEM_BYTES;                    // 128-byte-wide swizzle atoms per chunk
+  static constexpr int AUX_SLOT = (Fmt::AUX_BYTES + 1023) & ~1023;
+  static constexpr int STAGE_BYTES = Fmt::W_BYTES + AUX_SLOT + X_BYTES;
+  static constexpr int STAGES_FIT = SMEM_BUDGET / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT > MAX_STAGES ? MAX_STAGES : STAGES_FIT;
+  static_assert(STAGES >= 2, "stage does not fit");
+  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+  static constexpr int BAR_BYTES = 3 * STAGES * 8;   // wfull, xfull, sempty per stage
+  static constexpr size_t SMEM_BYTES = (size_t)BAR_OFF + BAR_BYTES + 1024;   // + the 1024-byte alignment of the base
 };
 
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
@@ -113,534 +76,306 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
 __device__ __forceinline__ uint2 lds64(uint32_t addr) {
   uint2 v;
   asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ void tmem_ld_x8(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-  tc_wait_ld();
-#pragma unroll
-  for (int q = 0; q < 8; ++q) v[q] = __uint_as_float(r[q]);
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint32_t lds16(uint32_t addr) {
+  unsigned short v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
+  return v;
 }
 
 // Fmt policy:
+//   SS, PROMOTE (SS only: sum each chunk's wgmmas into the fp32 registers), X_ELEM_BYTES (2: bf16 activations,
+//   1: 8-bit), W_BYTES, AUX_BYTES (per stage)
 //   static void issue_w(tm_w, tm_aux, p, w smem dst, aux smem dst, full barrier, n_tile, kc, policy)  (one thread)
 //   static uint32_t w_tx_bytes(p)
-//   struct Raw; static void load_row(p, w smem, aux smem, row r, Raw&)      (128 threads: one weight row each)
-//   static uint32_t touch(const Raw&)                                      (a value depending on every load of load_row)
-//   static void dequant_quarter(p, raw, q, out[16])                        (out[c] = bf16x2 of k = 32q + 2c, + 1)
-// TL = true compiles the per-CTA phase-timestamp instrumentation in (bring-up builds only).
-template <class Fmt, int N_MMA, bool TL = false, int DBUF = 2>
-__global__ void __launch_bounds__(NUM_THREADS, (N_MMA <= 64 ? 2 : 1))
+//   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
+//   RA:  struct Raw; static void load(p, w smem, aux smem, row_lo, lane, Raw&)   rows row_lo and row_lo + 8
+//        static void frag(p, raw, kk, a[4])                        bf16 A fragment of k16 step kk (0..7)
+template <class Fmt, int N_MMA>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_aux,
                const __grid_constant__ CUtensorMap tm_x, const Params p) {
-  using C = Cfg<N_MMA, DBUF>;
+  using C = Cfg<Fmt, N_MMA>;
+  using MMA = Wgmma<N_MMA>;
   constexpr int S = C::STAGES;
-  constexpr int T = C::A_STAGES;
-  constexpr int SX = C::X_SLOTS;
-  static_assert(SX >= T, "a chunk slot must outlive its TMEM A stage");
+  constexpr int NACC = N_MMA / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
-  uint64_t* wfull = bars;             // [S]   weight TMA transaction
-  uint64_t* sempty = wfull + S;       // [S]   4 dequant warps (the chunk's warpgroup) have the weights in registers
-  // chunk-slot barriers (slot c = chunk % SX, use u = chunk / SX = phase u).  Waiters: the issuer and the activation
-  // producer visit every chunk in order; a dequant warpgroup looks at cempty of chunk i - T, which is either the
-  // barrier's current phase or the one just completed (later uses of the slot need chunks > i): no parity aliasing.
-  uint64_t* cfull = sempty + S;       // [SX] 4 dequant warps (A stage stored) + activation TMA (arrive.expect_tx)
-  uint64_t* cempty = cfull + SX;      // [SX] MMA commit: the chunk's MMAs are done
-  uint64_t* dfull = cempty + SX;      // [2]   accumulator of a segment complete
-  uint64_t* dempty = dfull + 2;       // [2]   the 4 warps of the warpgroup that ran the segment's epilogue
-  uint64_t* dlast = dempty + 2;       // [1]   accumulator of the CTA's LAST segment complete (single phase: any warp
-                                      //       may wait on it without having followed the dfull phases)
-  uint64_t* fok = dlast + 1;          // [1]   the contributors' flags of an OWNER last segment have been seen (one poller)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(fok + 1);
+  uint64_t* wfull = bars;        // [S] weights + scales landed
+  uint64_t* xfull = wfull + S;   // [S] activation tile landed
+  uint64_t* sempty = xfull + S;  // [S] the 8 consumer warps are done with the stage
 
-  // The warp index goes through a shuffle so that the compiler knows it is warp-uniform: the single-thread
-  // roles below run as warp-uniform loops with only the tcgen05 / TMA / mbarrier instruction itself under
-  // elect.sync.  With the whole loop under `lane == 0` instead, ptxas treats every operand as divergent and
-  // wraps each UTCHMMA / UTMALDG in an elect-broadcast "waterfall" loop (52 instead of 20 cycles per MMA,
-  // scripts/mma_microbench7.cu).
+  // warp and warpgroup indices through a shuffle: the compiler then knows that the role branches below are
+  // warp-uniform and warpgroup-uniform (wgmma in code it must treat as divergent is serialised)
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const int wgi = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int G = gridDim.x, b = blockIdx.x;
-  auto stamp = [&](int e) {
-    if (TL && p.timeline && b < 100) {   // absolute globaltimer ns: comparable across back-to-back kernels
-      unsigned long long gt;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(gt));
-      p.timeline[(size_t)b * 16 + e] = gt;
-    }
-  };
-  // fine-grained per-chunk stamps of CTA 0 (clock64: one SM, comparable across its warps), chunks FS0 .. FS0+7:
-  // 0 weights requested, 1 weights seen landed, 2 weight stage handed back, 3 A stage stored (cfull), 4 issuer saw the
-  // chunk complete, 5 MMAs issued + committed, 6 dequant saw the A stage free again
-  constexpr int FS0 = 16;
-  auto fstamp = [&](int i, int e) {
-    if (TL && p.timeline && b == 0 && i >= FS0 && i < FS0 + 8) p.timeline[100 * 16 + (i - FS0) * 8 + e] = (unsigned long long)clock64();
-  };
-  if (threadIdx.x == 0) stamp(0);
   const long long U = (long long)p.n_tiles * p.m_blocks * p.KT;
   const int u0 = streamk::unit_begin(b, U, G), u1 = streamk::unit_begin(b + 1, U, G);
   const int nunits = u1 - u0;
   const streamk::Walk walk(u0, nunits, p.KT);
+  auto tile_of = [&](int i) { return (u0 + i) / p.KT; };
+  auto kc_of = [&](int i) { return (u0 + i) % p.KT; };
+  auto stage = [&](int s) { return smem + (size_t)s * C::STAGE_BYTES; };
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < S; ++i) {
       mbar_init(&wfull[i], 1);
-      mbar_init(&sempty[i], 4);
+      mbar_init(&xfull[i], 1);
+      mbar_init(&sempty[i], CONSUMER_WARPS);
     }
-    for (int i = 0; i < SX; ++i) {
-      mbar_init(&cfull[i], 5);
-      mbar_init(&cempty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&dfull[i], 1);
-      mbar_init(&dempty[i], 4);
-    }
-    mbar_init(dlast, 1);
-    mbar_init(fok, 1);
     fence_barrier_init();
   }
-  if (warp == TMA_WARP && lane == 0) {
+  if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tm_w);
     tma_prefetch_desc(&tm_aux);
+    tma_prefetch_desc(&tm_x);
   }
-  if (warp == XTMA_WARP && lane == 0) tma_prefetch_desc(&tm_x);
-  if (warp == MMA_WARP) tmem_alloc<C::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
   pdl_launch_dependents();
-  if (threadIdx.x == 0) stamp(1);
 
-  // unit i of this CTA -> (tile, kc); tiles are (m_blk, n_tile) pairs, n_tile fastest
-  auto tile_of = [&](int i) { return (u0 + i) / p.KT; };
-  auto kc_of = [&](int i) { return (u0 + i) % p.KT; };
-
-  // the CTA's last segment
   const int seg_last = walk.nseg - 1;
-  const int last_kind = walk.seg_kind(seg_last);
-  const int last_tile = walk.seg_tile(seg_last);
-  const int last_buf = seg_last % DBUF;
-  // all four warpgroups share an OWNER gather that has several groups of 8 token columns (otherwise the hand-over
-  // costs more than it saves)
-  const bool coop = (last_kind == streamk::SEG_OWNER) && (p.M - (last_tile / p.n_tiles) * N_MMA > 8);
+  const bool last_is_owner = walk.seg_kind(seg_last) == streamk::SEG_OWNER;
 
-  // one accumulator value -> output
-  auto emit8 = [&](const float (&v)[8], int n, int m_first, float bias, float osc) {
+  if (wgi == 0) {
+    if (warp != 0) goto done;
+    // ------------------------------------------------------------ TMA producer
+    const uint64_t pol_w = policy_evict_first();
+    const uint64_t pol_x = policy_evict_last();
+    auto issue_w = [&](int i) {
+      const int s = i % S;
+      uint8_t* st = stage(s);
+      mbar_expect_tx(&wfull[s], Fmt::w_tx_bytes(p));
+      Fmt::issue_w(&tm_w, &tm_aux, p, st, st + Fmt::W_BYTES, &wfull[s], tile_of(i) % p.n_tiles, kc_of(i), pol_w);
+    };
+    auto issue_x = [&](int i) {
+      const int s = i % S;
+      uint8_t* xs = stage(s) + Fmt::W_BYTES + C::AUX_SLOT;
+      const int m0 = (tile_of(i) / p.n_tiles) * N_MMA;
+      mbar_expect_tx(&xfull[s], C::X_BYTES);
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const int m = m_first + q;
-      if (m < p.M) {
-        float t = v[q];
-        if (p.row_scale) t *= p.row_scale[m];
-        p.y[(size_t)m * p.N_out + n] = __float2bfloat16_rn(t * osc + bias);
-      }
+      for (int a = 0; a < C::X_ATOMS; ++a)
+        tma_load_2d(xs + a * (N_MMA * 128), &tm_x, &xfull[s], kc_of(i) * KCHUNK + a * (KCHUNK / C::X_ATOMS), m0, pol_x);
+    };
+    const int pre = nunits < S ? nunits : S;
+    for (int i = 0; i < pre; ++i) {
+      if (elect_one()) issue_w(i);   // weights never depend on the previous kernel
+      __syncwarp();
     }
-  };
-
-  // OWNER finish of `tile` (accumulator at TMEM columns d_lane + [0, N_MMA) of this warp's lanes): own partial +
-  // the partials of CTAs b+1 .. b_last in that order, for the column groups helper, helper + nhelp, ...
-  // Called by whole warps (tcgen05.ld is warp-collective); r = the thread's weight row of the tile = TMEM lane.
-  auto finish_owner = [&](int tile, uint32_t d_lane, int r, int helper, int nhelp) {
-    const int b_last = streamk::cta_of_unit((long long)tile * p.KT + p.KT - 1, U, G);
-    const int n_oth = b_last - b;
-    const int n_tile = tile % p.n_tiles, m_blk = tile / p.n_tiles;
-    const int n = n_tile * ROWS + r, m0 = m_blk * N_MMA;
-    const bool row_ok = n < p.N_out;
-    const float bias = (p.bias && row_ok) ? __bfloat162float(p.bias[n]) : 0.f;
-    const float osc = (p.out_scale ? (p.out_scale_per_row ? (row_ok ? p.out_scale[n] : 1.f) : *p.out_scale) : 1.f) *
-                      __int_as_float((127 + p.acc_exp2) << 23);
-    const float* slot0 = p.ws_partial + (size_t)(b + 1) * (N_MMA * ROWS) + r;
-    // the contributors' flags were seen by the activation-producer warp (ld.acquire.gpu, then this cta-scope barrier):
-    // its L2 round trip -- ~0.8 us even when the flags were raised long ago -- runs under the last MMAs instead of
-    // between them and the gather
-    mbar_wait(fok, 0);
-    if (helper == 0 && r == 0) stamp(8);
-    if (p.M - m0 == 1) {
-      // decode, one token column: every contributor's value in flight at once
-      if (helper != 0) return;
-      float v[8];
-      tmem_ld_x8(d_lane, v);
-      float acc = v[0];
-#pragma unroll 1
-      for (int c0 = 0; c0 < n_oth; c0 += 8) {
-        float t[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) t[c] = (c0 + c < n_oth && row_ok) ? __ldcg(slot0 + (size_t)(c0 + c) * (N_MMA * ROWS)) : 0.f;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) acc += t[c];
-      }
-      if (row_ok) {
-        if (p.row_scale) acc *= p.row_scale[m0];
-        p.y[(size_t)m0 * p.N_out + n] = __float2bfloat16_rn(acc * osc + bias);
-      }
-      return;
+    pdl_wait();   // activations are the previous kernel's output
+    for (int i = 0; i < pre; ++i) {
+      if (elect_one()) issue_x(i);
+      __syncwarp();
     }
-#pragma unroll 1
-    for (int j0 = helper * 8; j0 < N_MMA; j0 += nhelp * 8) {
-      if (m0 + j0 >= p.M) break;
-      float v[8];
-      tmem_ld_x8(d_lane + j0, v);
-      const float* sj = slot0 + (size_t)j0 * ROWS;
-#pragma unroll 1
-      for (int c0 = 0; c0 < n_oth; c0 += 3) {
-        // three contributors x 8 columns of loads in flight (the gather is a chain of L2 round trips)
-        float t[3][8];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const float* sc = sj + (size_t)(c0 + c) * (N_MMA * ROWS);
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            t[c][q] = (c0 + c < n_oth && row_ok && m0 + j0 + q < p.M) ? __ldcg(sc + q * ROWS) : 0.f;
-        }
-#pragma unroll
-        for (int c = 0; c < 3; ++c)
-#pragma unroll
-          for (int q = 0; q < 8; ++q) v[q] += t[c][q];
+    for (int i = S; i < nunits; ++i) {
+      mbar_wait(&sempty[i % S], ((i / S) & 1) ^ 1);
+      if (elect_one()) {
+        issue_w(i);
+        issue_x(i);
       }
-      if (row_ok) emit8(v, n, m0 + j0, bias, osc);
+      __syncwarp();
     }
-  };
-  // cooperative OWNER finish of the last segment: every warpgroup takes every fourth group of 8 token columns
-  auto coop_help = [&](int helper) {
-    // (every warp has executed griddepcontrol.wait by now -- at a point where it had nothing else to do, see the roles)
-    while (!mbar_try_wait(dlast, 0)) __nanosleep(32);   // the producers get here early: do not steal issue slots
-    tc_fence_after();
-    if (helper == 0 && (warp & 3) == 0 && lane == 0) stamp(6);
-    const int q4 = warp & 3;
-    finish_owner(last_tile, tmem_base + ((uint32_t)(q4 * 32) << 16) + C::d_col(last_buf), q4 * 32 + lane, helper, 4);
-    if (helper == 0 && (warp & 3) == 0 && lane == 0) stamp(7);
-  };
+  } else {
+    // ------------------------------------------------------------ consumers: warpgroup wg owns rows 64wg .. 64wg+63
+    const int wg = wgi - 1, wq = warp & 3;
+    const int g = lane >> 2, t = lane & 3;
+    const int row_lo = wg * 64 + wq * 16 + g;   // fragment rows row_lo and row_lo + 8 (accumulator rows as well)
+    pdl_wait();   // outputs, workspace and scales belong to the previous kernel's stream order
 
-  if (warp < DEQ_WARPS) {
-    // ------------------------------------------------------------ dequant warpgroups: chunk i belongs to WG i % 3
-    const int wg = warp >> 2, q4 = warp & 3;
-    const int r = q4 * 32 + lane;  // weight row of the tile == TMEM lane
-    const uint32_t lane_taddr = tmem_base + ((uint32_t)(q4 * 32) << 16);
-    bool waited_prev = false;   // griddepcontrol.wait executed (outputs / workspace belong to the previous kernel)
+    uint32_t acc[NACC];
+    uint32_t a[8][4];   // register-A formats: the bf16 fragments of one chunk (read by the wgmmas until they complete)
+    int pending = -1;   // stage whose wgmmas may still be in flight
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&sempty[s]);
+    };
 
-    // Epilogue of a segment that is NOT the CTA's last one (FULL or CONTRIB), by this warpgroup.
-    auto epilogue = [&](int seg) {
-      if (!waited_prev) { pdl_wait(); waited_prev = true; }
+    // ---- epilogue of segment `seg` from v = the accumulator, once its wgmmas completed (wait_group 0 + operand fence,
+    // in warpgroup-uniform code: no wgmma is in flight while the epilogue's divergent code touches it).  Value
+    // j = 4q + 2h + c of this thread is (weight row row_lo + 8h, token 8q + 2t + c) of the tile (wgmma m64nN fragment)
+    auto epilogue = [&](int seg, uint32_t (&v)[NACC]) {
       const int tile = walk.seg_tile(seg);
       const int kind = walk.seg_kind(seg);
-      const int buf = seg % DBUF;
-      mbar_wait(&dfull[buf], (seg / DBUF) & 1);
-      tc_fence_after();
       const int n_tile = tile % p.n_tiles, m_blk = tile / p.n_tiles;
-      const int n = n_tile * ROWS + r, m0 = m_blk * N_MMA;
-      const uint32_t d_lane = lane_taddr + C::d_col(buf);
-      if (kind == streamk::SEG_FULL) {
-        // the whole K range of this tile was ours: straight to the output
-        const float bias = (p.bias && n < p.N_out) ? __bfloat162float(p.bias[n]) : 0.f;
-        const float osc = (p.out_scale ? (p.out_scale_per_row ? (n < p.N_out ? p.out_scale[n] : 1.f) : *p.out_scale) : 1.f) *
-                          __int_as_float((127 + p.acc_exp2) << 23);
-#pragma unroll 1
-        for (int j = 0; j < N_MMA; j += 8) {
-          if (m0 + j >= p.M) break;
-          float v[8];
-          tmem_ld_x8(d_lane + j, v);
-          if (n < p.N_out) emit8(v, n, m0 + j, bias, osc);
-        }
-      } else {
-        // CONTRIB: publish the partial (column-major slot: coalesced across the 128 rows), then raise this CTA's flag
-        float* slot = p.ws_partial + (size_t)b * (N_MMA * ROWS) + r;
-#pragma unroll 1
-        for (int j = 0; j < N_MMA; j += 8) {
-          if (m0 + j >= p.M) break;
-          float v[8];
-          tmem_ld_x8(d_lane + j, v);
+      const int m0 = m_blk * N_MMA;
+      if (kind == streamk::SEG_CONTRIB) {
+        // publish the partial (column-major slot: word (token j, row r) at j * 128 + r), then one gpu-scope release
+        uint32_t* slot = reinterpret_cast<uint32_t*>(p.ws_partial) + (size_t)b * (N_MMA * ROWS);
 #pragma unroll
-          for (int q = 0; q < 8; ++q)
-            if (m0 + j + q < p.M) __stcg(&slot[(j + q) * ROWS], v[q]);
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // all 128 rows stored (cta-scope order) ...
-        if (q4 == 0 && lane == 0) streamk::st_release_u32(p.ws_flag + b, 1u);   // ... then one gpu-scope release
+        for (int q = 0; q < NACC / 4; ++q)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+              const int col = 8 * q + 2 * t + c, r = row_lo + 8 * h;
+              if (m0 + col < p.M) __stcg(&slot[col * ROWS + r], v[4 * q + 2 * h + c]);
+            }
+        asm volatile("bar.sync 1, 256;" ::: "memory");   // all 128 rows stored (cta-scope order) ...
+        if (warp == 4 && lane == 0) streamk::st_release_u32(p.ws_flag + b, 1u);   // ... then one gpu-scope release
+        return;
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&dempty[buf]);
-    };
-    // the segment whose last chunk is e belongs to warpgroup e % 3, which runs its epilogue after its next chunk.
-    // ep_at = last chunk of the next segment (before the CTA's last one) that belongs to this warpgroup, kept outside the
-    // chunk loop: the loop itself pays one compare per chunk (the integer pipe is what the dequant warps are short of)
-    int ep_seg = 0, ep_at = 0x7fffffff;
-    const bool eager0 = walk.seg_kind(0) == streamk::SEG_CONTRIB && nunits - walk.seg_count(0) < 12;
-    auto seg_end = [&](int sg) { return walk.seg_begin(sg) + walk.seg_count(sg) - 1; };
-    auto next_owned = [&]() {
-      while (ep_seg < seg_last && seg_end(ep_seg) % DEQ_WGS != wg) ++ep_seg;
-      ep_at = ep_seg < seg_last ? seg_end(ep_seg) : 0x7fffffff;
-    };
-    next_owned();
-    auto run_epilogues = [&](int before_chunk) {
-      while (ep_at < before_chunk) {
-        epilogue(ep_seg);
-        ++ep_seg;
-        next_owned();
+      if (kind == streamk::SEG_OWNER) {
+        // own partial + the partials of CTAs b+1 .. b_last in that order (fixed: bit-reproducible run to run)
+        const int b_last = streamk::cta_of_unit((long long)tile * p.KT + p.KT - 1, U, G);
+        for (int c = b + 1; c <= b_last; ++c)
+          while (streamk::ld_acquire_u32(p.ws_flag + c) == 0u) __nanosleep(64);
+#pragma unroll 1
+        for (int c = b + 1; c <= b_last; ++c) {
+          const uint32_t* slot = reinterpret_cast<const uint32_t*>(p.ws_partial) + (size_t)c * (N_MMA * ROWS);
+#pragma unroll
+          for (int q = 0; q < NACC / 4; ++q)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int cc = 0; cc < 2; ++cc) {
+                const int col = 8 * q + 2 * t + cc, r = row_lo + 8 * h, j = 4 * q + 2 * h + cc;
+                if (m0 + col < p.M) {
+                  const uint32_t o = __ldcg(slot + col * ROWS + r);
+                  if (p.epi == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o);
+                  else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o));
+                }
+              }
+        }
+      }
+      // outputs
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int n = n_tile * ROWS + row_lo + 8 * h;
+        if (n >= p.N_out) continue;
+        const float bias = p.bias ? __bfloat162float(p.bias[n]) : 0.f;
+        float osc = 1.f, sw = 1.f;
+        if (p.epi == EPI_FLOAT) {
+          osc = (p.out_scale ? (p.out_scale_per_row ? p.out_scale[n] : *p.out_scale) : 1.f);
+          if (p.out_scale2) osc *= *p.out_scale2;
+          osc *= __int_as_float((127 + p.acc_exp2) << 23);
+        } else {
+          sw = p.w_scale ? p.w_scale[n] : 1.f;
+        }
+#pragma unroll
+        for (int q = 0; q < NACC / 4; ++q)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int m = m0 + 8 * q + 2 * t + c;
+            if (m >= p.M) continue;
+            const uint32_t raw = v[4 * q + 2 * h + c];
+            __nv_bfloat16* dst = p.y ? p.y + (size_t)m * p.N_out + n : nullptr;
+            if (p.epi == EPI_FLOAT) {
+              float x = __uint_as_float(raw);
+              if (p.row_scale) x *= p.row_scale[m];
+              *dst = __float2bfloat16_rn(x * osc + bias);
+            } else if (p.epi == EPI_I8) {
+              if (p.i32_out) {
+                p.i32_out[(size_t)m * p.N_out + n] = (int32_t)raw;
+              } else {
+                // int8 reference: bf16 round between the activation and the weight scale
+                const float x = __bfloat162float(__float2bfloat16_rn((float)(int32_t)raw * p.row_scale[m]));
+                *dst = __float2bfloat16_rn(x * sw + bias);
+              }
+            } else {
+              *dst = __float2bfloat16_rn(__uint_as_float(raw) * (p.row_scale[m] * sw) + bias);
+            }
+          }
       }
     };
 
-    // ring positions of chunk i = wg, wg + 3, ... kept incrementally (the integer pipe is busy enough here):
-    // weight stage s (phase sph), TMEM A stage t, chunk slot c, and the slot / phase of chunk i - T (ec, eph)
-    int s = wg % S, sph = (wg / S) & 1, t = wg % T, c = wg % SX;
-    // chunk wg - T: when negative it stands for "the lap before the first" (parity 1; never waited on)
-    int ec = wg >= T ? (wg - T) % SX : wg - T + SX, eph = wg >= T ? ((wg - T) / SX) & 1 : 1;
-    for (int i = wg; i < nunits; i += DEQ_WGS) {
-      const uint32_t st = smem_u32(smem + (size_t)s * WSTAGE_BYTES);
-      const uint32_t a_t = lane_taddr + C::A_COL0 + t * A_COLS;
-      mbar_wait(&wfull[s], sph);
-      if (i == 0 && warp == 0 && lane == 0) stamp(3);
-      if (q4 == 0 && lane == 0) fstamp(i, 1);
-      // the whole row into registers (16 + a few), then four quarters of 32 k -> 16 registers -> tcgen05.st.x16 each.
-      // The weight stage goes back to the producers as soon as the row is in registers; quarter 0 is computed before
-      // the A stage is known to be free, so that wait overlaps arithmetic.
-      if (p.flags & 1) {   // bring-up: no dequant arithmetic, no TMEM stores (garbage results)
-        if (i >= T) mbar_wait(&cempty[ec], eph);
-        __syncwarp();
-        if (elect_one()) { mbar_arrive(&sempty[s]); mbar_arrive(&cfull[c]); }
-      } else {
-        typename Fmt::Raw raw;
-        Fmt::load_row(p, st, st + W_BYTES, r, raw);
-        // weights are in registers: the stage goes back to the producers BEFORE any arithmetic -- the ring (8 stages x
-        // 10 KB against a 3000-4500 cycle loaded DRAM round trip) is what paces the streaming phase, and every cycle a
-        // landed stage is held is added to that round trip.  "In registers" has to be enforced: the arrive's address
-        // depends on the loaded values (Fmt::touch; `never` is always 0)
-        const uint32_t never = (Fmt::touch(raw) == 0x9E3779B9u) & (p.flags == 0x7fffffff);
-        __syncwarp();
-        if (elect_one()) mbar_arrive(&sempty[s] + never);
-        if (q4 == 0 && lane == 0) fstamp(i, 2);
-        uint32_t out[16];
-        Fmt::dequant_quarter(p, raw, 0, out);   // (before the A stage is known to be free: that wait overlaps arithmetic)
-        if (i >= T) {
-          // the first T chunks were dequantised under the previous kernel; from here on the warpgroup needs MMAs of
-          // THIS kernel, which need its activations, which need the previous kernel: the dependency wait costs nothing
-          // here, and every later use of outputs / workspace by this warp is covered
-          if (!waited_prev) { pdl_wait(); waited_prev = true; }
-          mbar_wait(&cempty[ec], eph);  // MMAs of chunk i - T are done: A stage t is free
-        }
-        if (q4 == 0 && lane == 0) fstamp(i, 6);
-        tc_fence_after();
-        tmem_st_x16(a_t, out);   // source registers are consumed at issue: no tcgen05.wait::st before reusing them
+    int i = 0;
+    for (int seg = 0; seg < walk.nseg; ++seg) {
+      const int cnt = walk.seg_count(seg);
+      for (int c = 0; c < cnt; ++c, ++i) {
+        const uint32_t scale_d = c > 0;   // the first wgmma of a segment overwrites the accumulator
+        const int s = i % S;
+        const uint32_t ph = (i / S) & 1;
+        uint8_t* st = stage(s);
+        const uint32_t w_s = smem_u32(st), aux_s = w_s + Fmt::W_BYTES, x_s = aux_s + C::AUX_SLOT;
+        mbar_wait(&wfull[s], ph);
+        if constexpr (Fmt::PROMOTE) {
+          // e4m3: a chain of wgmmas accumulates in the tensor core's reduced-precision adder; each chunk's four k32
+          // wgmmas go to a fresh accumulator that is added to the fp32 registers here (fp32 accuracy across K)
+          mbar_wait(&xfull[s], ph);
+          uint32_t part[NACC];
+          wgmma_fence();
+          Fmt::template mma<N_MMA>(part, w_s, x_s, wg, 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_operand(part);
+          release(s);
 #pragma unroll
-        for (int q = 1; q < 4; ++q) {
-          Fmt::dequant_quarter(p, raw, q, out);
-          tmem_st_x16(a_t + 16 * q, out);
-        }
-        tc_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (elect_one()) mbar_arrive(&cfull[c]);
-        if (q4 == 0 && lane == 0) fstamp(i, 3);
-      }
-      s += DEQ_WGS;
-      if (s >= S) { s -= S; sph ^= 1; }
-      t += DEQ_WGS;
-      while (t >= T) t -= T;
-      c += DEQ_WGS;
-      if (c >= SX) c -= SX;
-      ec += DEQ_WGS;
-      if (ec >= SX) { ec -= SX; eph ^= 1; }
-      // segments this warpgroup's EARLIER chunks completed: their accumulators are long done.  Exception: a short
-      // range's CONTRIB segment (always the first) is published as soon as its last chunk is stored -- its owner CTA
-      // is about to finish too and would otherwise wait for this flag (small projections: 6-10 chunks per CTA)
-      run_epilogues((eager0 && ep_seg == 0) ? i + 1 : i);
-    }
-    if (!waited_prev) { pdl_wait(); waited_prev = true; }
-    run_epilogues(nunits);   // whatever is left of the segments before the last one
-    // ---- the CTA's last segment
-    if (coop) {
-      coop_help(wg);
-    } else if (wg == (nunits - 1 + 1) % DEQ_WGS) {
-      // the warpgroup that did NOT dequantise the last chunk has been idle longest: it finishes the segment
-      if (!waited_prev) { pdl_wait(); waited_prev = true; }
-      while (!mbar_try_wait(dlast, 0)) __nanosleep(32);
-      tc_fence_after();
-      if (warp == (wg << 2) && lane == 0) stamp(6);
-      const uint32_t d_lane = lane_taddr + C::d_col(last_buf);
-      if (last_kind == streamk::SEG_OWNER) {
-        finish_owner(last_tile, d_lane, r, 0, 1);
-      } else {
-        // FULL or CONTRIB as the last segment: same code as mid-stream (dfull of the last segment == dlast)
-        epilogue(seg_last);
-      }
-      if (warp == (wg << 2) && lane == 0) stamp(7);
-    }
-  } else if (warp >= TMA_WARP) {
-    if (warp == TMA_WARP || (warp == TMA_WARP1 && p.producers == 2)) {
-      // ---------------------------------------------------------- weight producers.  Weights never depend on the
-      // previous kernel: no griddepcontrol.wait on this path.  One thread gets a TMA box pair out every ~600
-      // cycles (scripts/stream_microbench.cu: one producer warp 4.4-4.8 TB/s, two 5.1-6.0 TB/s), so with
-      // p.producers == 2 warps 12 and 15 take alternate chunks (STAGES is even: a stage always belongs to the same
-      // producer, which therefore sees every phase of its sempty barrier)
-      const uint64_t pol_w = policy_evict_first();
-      const int np = p.producers, pi = (warp == TMA_WARP) ? 0 : 1;
-      int s = pi, sph = 0, kc = kc_of(0) + pi, n_tile = tile_of(0) % p.n_tiles;
-      if (kc >= p.KT) { kc -= p.KT; if (++n_tile == p.n_tiles) n_tile = 0; }
-      for (int i = pi; i < nunits; i += np) {
-        if (i >= S) mbar_wait(&sempty[s], sph ^ 1);
-        if (elect_one()) {
-          uint8_t* st = smem + (size_t)s * WSTAGE_BYTES;
-          mbar_expect_tx(&wfull[s], Fmt::w_tx_bytes(p));
-          Fmt::issue_w(&tm_w, &tm_aux, p, st, st + W_BYTES, &wfull[s], n_tile, kc, pol_w);
-          fstamp(i, 0);
-          if (p.prefetch > 0 && i + p.prefetch < nunits) {   // HBM -> L2 of a chunk further down this CTA's range
-            const int u = u0 + i + p.prefetch;
-            Fmt::prefetch_w(&tm_w, &tm_aux, p, (u / p.KT) % p.n_tiles, u % p.KT);
+          for (int j = 0; j < NACC; ++j)
+            acc[j] = scale_d ? __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(part[j])) : part[j];
+          continue;
+        } else if constexpr (Fmt::SS) {
+          mbar_wait(&xfull[s], ph);
+          wgmma_fence_operand(acc);
+          wgmma_fence();
+          Fmt::template mma<N_MMA>(acc, w_s, x_s, wg, scale_d);
+        } else {
+          typename Fmt::Raw raw;
+          Fmt::load(p, w_s, aux_s, row_lo, lane, raw);
+          // the previous chunk's wgmmas still read a[]: they complete (their stage goes back) before a[] is rewritten,
+          // and the operand fence keeps the old fragment registers alive up to that point.  The wgmmas overlap this
+          // chunk's weight loads and barrier waits, not its dequant arithmetic
+          wgmma_wait<0>();
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk) wgmma_fence_operand(a[kk]);
+          if (pending >= 0) release(pending);
+          pending = -1;
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk) Fmt::frag(p, raw, kk, a[kk]);
+          mbar_wait(&xfull[s], ph);
+          wgmma_fence_operand(acc);
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk) {
+            // k16 step kk of the bf16 B tile: atom kk / 4 (64 k each), 32 bytes per step inside the 128-byte row
+            const uint64_t bd = wgmma_desc_k_sw128(x_s + (kk >> 2) * (N_MMA * 128) + (kk & 3) * 32);
+            MMA::ra_bf16(acc, a[kk], bd, kk == 0 ? scale_d : 1u);
           }
         }
-        __syncwarp();
-        s += np;
-        if (s >= S) { s -= S; sph ^= 1; }
-        kc += np;
-        if (kc >= p.KT) { kc -= p.KT; if (++n_tile == p.n_tiles) n_tile = 0; }
+        wgmma_commit();
+        wgmma_fence_operand(acc);
+        wgmma_wait<1>();   // the wgmmas of the previous chunk are done: its stage goes back to the producer
+        if (pending >= 0) release(pending);
+        pending = s;
       }
-      pdl_wait();   // idle from here on: be ready to help with the last segment's outputs
-    } else if (warp == XTMA_WARP) {
-      // ---------------------------------------------------------- activation producer
-      const uint64_t pol_x = policy_evict_last();
-      pdl_wait();   // activations are the previous kernel's output
-      if (lane == 0) stamp(2);
-      int c = 0, cph = 1, kc = kc_of(0), tile = tile_of(0);   // cph: parity of the slot's PREVIOUS use
-      for (int i = 0; i < nunits; ++i) {
-        uint64_t* full = &cfull[c];
-        if (i >= SX) mbar_wait(&cempty[c], cph);   // MMAs of chunk i - SX are done: the slot is free
-        if (elect_one()) {
-          uint8_t* xs = smem + C::X_OFF + (size_t)c * C::X_BYTES;
-          const int m0 = (tile / p.n_tiles) * N_MMA, k0 = kc * KCHUNK;
-          if ((p.flags & 4) && i >= SX) {
-            mbar_arrive(full);   // bring-up: no activation loads after the first ring-full (garbage results)
-          } else {
-            mbar_expect_tx(full, C::X_BYTES);
-            tma_load_2d(xs, &tm_x, full, k0, m0, pol_x);
-            tma_load_2d(xs + N_MMA * 128, &tm_x, full, k0 + 64, m0, pol_x);
-          }
-        }
-        __syncwarp();
-        if (++c == SX) { c = 0; cph ^= 1; }
-        if (++kc == p.KT) { kc = 0; ++tile; }
-      }
-      if (last_kind == streamk::SEG_OWNER) {
-        // this warp's work is done a few chunks before the CTA's: it becomes the ONE poller of the contributors' flags
-        // (sixteen warps polling global memory from here was measured 15 % slower per layer, profiles/r02_call_s.log)
-        const int b_last = streamk::cta_of_unit((long long)last_tile * p.KT + p.KT - 1, U, G);
-        const int n_oth = b_last - b;
-        for (int base = 0; base < n_oth; base += 32)
-          if (base + lane < n_oth)
-            while (streamk::ld_acquire_u32(p.ws_flag + b + 1 + base + lane) == 0u) __nanosleep(64);
-        __syncwarp();
-        if (elect_one()) mbar_arrive(fok);
-        __syncwarp();
-      }
-    } else if (warp == MMA_WARP) {
-      // ---------------------------------------------------------- MMA issuer
-      constexpr uint32_t idesc = make_idesc(1 /*f32*/, 1 /*bf16*/, 1 /*bf16*/, ROWS, N_MMA);
-      const uint32_t x0 = smem_u32(smem + C::X_OFF);
-      // The issuer shares its scheduler with three dequant warps, so every instruction it needs per chunk costs it
-      // issue slots it has to win: the chunk loop is unrolled over the X_SLOTS chunk slots, which makes the slot,
-      // its barriers, the activation descriptors and (X_SLOTS % A_STAGES == 0) the TMEM A stage compile-time
-      // constants -- one try_wait, eight UTCHMMA with immediate / uniform operands, one commit.
-      pdl_wait();   // its first MMA needs the activations anyway
-      constexpr bool T_STATIC = (SX % T) == 0;
-      int c = 0, seg = 0, seg_end = walk.seg_count(0) - 1, t_dyn = 0;
-      uint32_t cph = 0;          // phase parity of the current lap over the chunk slots
-      uint32_t acc = 0;          // first MMA of a segment overwrites the accumulator
-      uint32_t d_t = tmem_base + C::d_col(0);
-      mbar_wait(&dempty[0], 1);  // (fresh barrier: returns at once)
-      while (c < nunits) {
-#pragma unroll
-        for (int j = 0; j < SX; ++j) {
-          if (c < nunits) {
-            mbar_wait(&cfull[j], cph);
-            if (!(p.flags & 8)) tc_fence_after();   // bring-up: flag 8 drops the per-chunk tcgen05.fence of the issuer
-            const uint32_t a_t = tmem_base + C::A_COL0 + (T_STATIC ? (j % T) : t_dyn) * A_COLS;
-            if (elect_one()) {
-              if (c == 0) stamp(4);
-              fstamp(c, 4);
-              const uint32_t xb = x0 + j * C::X_BYTES;
-              const uint64_t b_lo = umma_desc_k_sw128(xb), b_hi = umma_desc_k_sw128(xb + N_MMA * 128);
-#pragma unroll
-              for (int kk = 0; kk < 8; ++kk)
-                if (!(p.flags & 2))   // bring-up: flag 2 skips the MMAs
-                  mma_ts_f16(d_t, a_t + kk * 8, (kk < 4 ? b_lo : b_hi) + (uint64_t)((kk & 3) * 2), idesc, (kk == 0) ? acc : 1u);
-              tc_commit(&cempty[j]);
-              fstamp(c, 5);
-              if (c == nunits - 1) stamp(5);
-            }
-            __syncwarp();
-            acc = 1u;
-            if (!T_STATIC) { if (++t_dyn == T) t_dyn = 0; }
-            if (c == seg_end) {
-              // segment complete: its accumulator is ready once these MMAs are; move to the next buffer
-              const int buf = seg % DBUF;
-              if (elect_one()) {
-                tc_commit(&dfull[buf]);
-                if (seg == seg_last) tc_commit(dlast);
-              }
-              __syncwarp();
-              ++seg;
-              if (seg < walk.nseg) {
-                seg_end += walk.seg_count(seg);
-                const int nb = seg % DBUF;
-                mbar_wait(&dempty[nb], ((seg / DBUF) & 1) ^ 1);   // epilogue of segment seg - DBUF done
-                d_t = tmem_base + C::d_col(nb);
-                acc = 0;
-              }
-            }
-            ++c;
-          }
-        }
-        cph ^= 1;
-      }
-    }
-    if (coop) {
-      if (warp == TMA_WARP1 && p.producers != 2) pdl_wait();
-      coop_help(3);
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      if (pending >= 0) release(pending);
+      pending = -1;
+      epilogue(seg, acc);
     }
   }
 
-  __syncwarp();
-  tc_fence_before();
+done:
   __syncthreads();
-  if (threadIdx.x == 0) stamp(9);
-  if (last_kind == streamk::SEG_OWNER && warp == 0) {
-    // every warpgroup has read the contributors' partials: re-arm their flags for the next launch
-    const int b_last = streamk::cta_of_unit((long long)last_tile * p.KT + p.KT - 1, U, G);
+  if (last_is_owner && warp == 4) {
+    // every consumer has read the contributors' partials: re-arm their flags for the next launch
+    const int b_last = streamk::cta_of_unit((long long)walk.seg_tile(seg_last) * p.KT + p.KT - 1, U, G);
     for (int c = b + 1 + lane; c <= b_last; c += 32) p.ws_flag[c] = 0u;
-  }
-  if (warp == MMA_WARP) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<C::TMEM_COLS>(tmem_base);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
 // Grid choice + workspace carve-up shared by the launchers of this kernel.
-//   * one CTA per SM: the second slot of every SM belongs to the NEXT linear's CTA, which becomes resident under
-//     this one (PDL) and has its first weights in flight while this kernel finishes.  A grid that fills both slots
-//     makes each kernel's CTAs wait for the previous kernel's CTAs to exit, so one late CTA delays a CTA of every
-//     following kernel (measured: 2 CTAs/SM 92.7 us per Llama-3-8B layer at bs=32, 1 CTA/SM 74.3;
-//     profiles/r02_call_a.log).  Also keeps the grid within the resident capacity, which the owner protocol needs
-//     for forward progress (streamk.cuh)
+//   * at most one CTA per SM (the stage ring takes most of the shared memory): the grid stays within the resident
+//     capacity, which the owner protocol needs for forward progress (streamk.cuh)
 //   * never fewer than `min_units` chunks per CTA: splitting a tile over more CTAs shortens the streaming phase but
 //     lengthens the owner's gather
-template <int N_MMA>
-inline int plan(Params& p, void* ws, size_t ws_bytes, const char* what, int* grid_out) {
+template <class Fmt, int N_MMA>
+inline int launch_gemm(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const CUtensorMap& tm_x,
+                       void* ws, size_t ws_bytes, const char* what, cudaStream_t stream) {
+  using C = Cfg<Fmt, N_MMA>;
   const long long units = (long long)p.n_tiles * p.m_blocks * p.KT;
-  const int per_sm = ts_ctas_per_sm() ? ts_ctas_per_sm() : 1;
-  int grid = sm_count() * (N_MMA <= 64 ? per_sm : 1);
+  int grid = sm_count();
   const int min_units = ts_min_units() ? ts_min_units() : 4;
   if (units / min_units < grid) grid = units / min_units > 0 ? (int)(units / min_units) : 1;
   const size_t need = streamk::WS_PARTIAL_OFF + (size_t)grid * N_MMA * ROWS * 4;
@@ -648,10 +383,9 @@ inline int plan(Params& p, void* ws, size_t ws_bytes, const char* what, int* gri
     return fail(AO_ERR_WORKSPACE, "%s: workspace too small (%zu < %zu)", what, ws_bytes, need);
   p.ws_flag = reinterpret_cast<unsigned int*>(ws);
   p.ws_partial = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws) + streamk::WS_PARTIAL_OFF);
-  p.flags = ts_flags();
-  p.producers = (ts_producers() == 1 || (Cfg<N_MMA>::STAGES & 1)) ? 1 : 2;
-  p.prefetch = ts_prefetch();
-  *grid_out = grid;
+  auto kern = ts_gemm_kernel<Fmt, N_MMA>;
+  AO_CUDA_CHECK(ensure_dynamic_smem(reinterpret_cast<const void*>(kern), C::SMEM_BYTES));
+  AO_CUDA_CHECK(launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, pdl_enabled(), tm_w, tm_aux, tm_x, p));
   return AO_OK;
 }
 

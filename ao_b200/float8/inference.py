@@ -8,7 +8,7 @@ from ao_b200.quantization.granularity import PerBlock, PerRow, PerTensor
 
 class Float8MMConfig(NamedTuple):
     """Matmul options carried by Float8Tensor; ``use_fast_accum`` is accepted for compatibility --
-    the tcgen05 kernel always accumulates in fp32 TMEM."""
+    the wgmma kernel sums every 128-k chunk into fp32 registers."""
 
     emulate: bool = False
     use_fast_accum: bool = False

@@ -12,7 +12,7 @@ import logging
 
 import torch
 
-from ao_b200._native import require_sm100
+from ao_b200._native import require_sm90
 from ao_b200.core.config import AOBaseConfig
 from ao_b200.quantization.quant_api import _set_quantized_param
 from ao_b200.quantization.quantize_.common.kernel_preference import KernelPreference
@@ -62,7 +62,7 @@ def _check_nvfp4_shape(weight):
 
 
 def _nvfp4_kernel_compat(weight, k_multiple: int) -> bool:
-    """The sm_100a kernels stream K in chunks whose block-scale tiles must exist in full: K % 256 for nvfp4 x nvfp4
+    """The sm_90a kernels stream K in chunks whose block-scale tiles must exist in full: K % 256 for nvfp4 x nvfp4
     (lowp_linear.cu), K % 128 for the weight-only / fp8-activation kernel (ts_gemm.cuh).  The reference accepts any
     K % 16 (inference_workflow.py:248-251); such a layer is left unquantized here, with a log line, the way the int4
     and float8 flows skip incompatible shapes (quant_api.py:549-553, quantization/utils.py:663-687) -- never
@@ -92,7 +92,7 @@ def _nvfp4_inference_linear_transform(module, config, *, parameter_name="weight"
     weight = getattr(module, parameter_name)
     _check_nvfp4_shape(weight)
     if torch.cuda.is_available():
-        require_sm100()
+        require_sm90()
     assert weight.dim() == 2, "3D (MoE) weights are out of scope"
     if not _nvfp4_kernel_compat(weight, 256):
         return module

@@ -1,4 +1,4 @@
-"""MXFP8 weight/activation tensor on tcgen05 kind::mxf8f6f4.block_scale.
+"""MXFP8 weight/activation tensor on Hopper wgmma (bf16, exactly dequantised operands).
 
 Attribute names/order match torchao's MXTensor (torchao/prototype/mx_formats/mx_tensor.py:509-517):
 ``qdata, scale | elem_dtype, block_size, orig_dtype, kernel_preference, act_quant_kwargs,
@@ -122,7 +122,7 @@ def _(func, types, args, kwargs):
     k = w.act_quant_kwargs
     if k is None:
         raise NotImplementedError("MX weight-only linear is outside this engine's scope (SURVEY §8)")
-    assert w.is_swizzled_scales and k.is_swizzled_scales, "the tcgen05 kernel consumes pre-swizzled (blocked) scales"
+    assert w.is_swizzled_scales and k.is_swizzled_scales, "the kernel consumes pre-swizzled (blocked) scales"
     N, K = w.shape[-2], w.shape[-1]
     orig_shape = x.shape
     x2 = x.reshape(-1, K)

@@ -1,4 +1,4 @@
-"""NVFP4 (e2m1 data, e4m3 block-16 scales, fp32 per-tensor scale) on tcgen05 kind::mxf4nvf4.
+"""NVFP4 (e2m1 data, e4m3 block-16 scales, fp32 per-tensor scale) on Hopper wgmma (bf16, exactly dequantised operands).
 
 Attribute names/order match torchao's NVFP4Tensor (torchao/prototype/mx_formats/nvfp4_tensor.py:69-79):
 ``qdata, scale | block_size, orig_dtype | per_tensor_scale?, act_per_tensor_scale? |
@@ -117,7 +117,7 @@ def _(func, types, args, kwargs):
     x, w, bias = args[0], args[1], args[2] if len(args) > 2 else None
     if not isinstance(w, NVFP4Tensor):
         raise NotImplementedError("NVFP4Tensor: weight must be NVFP4Tensor")
-    assert w.is_swizzled_scales, "the tcgen05 kernels consume pre-swizzled (blocked) weight scales"
+    assert w.is_swizzled_scales, "the kernels consume pre-swizzled (blocked) weight scales"
     N, K = w.shape[-2], w.shape[-1]
     orig_shape = x.shape
     x2 = x.reshape(-1, K)
@@ -126,7 +126,7 @@ def _(func, types, args, kwargs):
     k = w.act_quant_kwargs
     b_pts = w.per_tensor_scale.reshape(-1) if w.per_tensor_scale is not None else None
     if k is None:
-        # weight-only: y = x_bf16 @ dequant(W)^T, weights dequantised inside the tcgen05 kernel; a column slice of a
+        # weight-only: y = x_bf16 @ dequant(W)^T, weights dequantised inside the wgmma kernel; a column slice of a
         # wider buffer goes in as is (the TMA descriptor carries the row pitch)
         xb = rows_for_kernel(x2.to(torch.bfloat16))
         y = torch.ops.ao_b200.nvfp4_weight_linear(xb, None, w.qdata, w.scale.view(torch.uint8), b_pts, bias)

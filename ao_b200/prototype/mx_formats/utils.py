@@ -7,7 +7,7 @@ def ceil_div(a, b):
 
 
 def to_blocked(input_matrix: torch.Tensor) -> torch.Tensor:
-    """[H, W] -> flat 32*ceil(H/128) x 16*ceil(W/4): the cuBLAS / tcgen05.cp block-scale layout
+    """[H, W] -> flat 32*ceil(H/128) x 16*ceil(W/4): the cuBLAS block-scale layout
     (each 128x4 tile becomes 32 rows of 16 bytes: (r%32)*16 + (r/32)*4 + c)."""
     rows, cols = input_matrix.shape
     rb, cb = ceil_div(rows, 128), ceil_div(cols, 4)

@@ -21,7 +21,7 @@ from typing import Any, Callable, List, Optional, Tuple, Union
 import torch
 import torch.nn as nn
 
-from ao_b200._native import require_sm100
+from ao_b200._native import require_sm90
 from ao_b200.core.config import AOBaseConfig
 from ao_b200.float8.inference import FP8Granularity, Float8MMConfig, _normalize_granularity
 from ao_b200.quantization.granularity import Granularity, PerRow, PerTensor
@@ -148,7 +148,7 @@ def _int4_weight_only_quantize_tensor(weight, config: Int4WeightOnlyConfig):
                                                     config.int4_choose_qparams_algorithm),
                                                 ntile_size=config.int4_tile_packed_ntile)
     raise NotImplementedError(
-        f"int4_packing_format={fmt.value!r}: only 'tile_packed_to_4d' has sm_100a kernels in this engine "
+        f"int4_packing_format={fmt.value!r}: only 'tile_packed_to_4d' has sm_90a kernels in this engine "
         f"(plain/preshuffled need the external mslk library in the reference as well)")
 
 
@@ -197,7 +197,7 @@ def _int8_dynamic_activation_int8_weight_quantize_tensor(weight, config):
         # (int8/kernels.py:48-58); this engine has no fallback and its TMA row pitch needs K % 16 == 0: leave the
         # layer unquantized, with a log line, like the int4 / float8 flows do for incompatible shapes
         logger.info(f"Skipping int8 dynamic quantization: weight shape {tuple(weight.shape)} needs in_features % 16 == 0 "
-                    f"and out_features % 8 == 0 for the sm_100a kernel")
+                    f"and out_features % 8 == 0 for the sm_90a kernel")
         return weight
     return Int8Tensor.from_hp(
         weight, granularity=w, mapping_type=MappingType.SYMMETRIC,
@@ -269,7 +269,7 @@ def _float8_dynamic_activation_float8_weight_quantize_tensor(weight, config):
 @register_quantize_module_handler(Float8DynamicActivationFloat8WeightConfig)
 def _float8_dynamic_activation_float8_weight_transform(module, config, *, parameter_name="weight"):
     if torch.cuda.is_available():
-        require_sm100()
+        require_sm90()
     assert hasattr(module, parameter_name), f"Expected module to have {parameter_name!r}"
     new_weight = _float8_dynamic_activation_float8_weight_quantize_tensor(getattr(module, parameter_name), config)
     return _set_quantized_param(module, parameter_name, new_weight)

@@ -1,7 +1,7 @@
 """Kernel family switch carried by the quantized tensors
 (reference: torchao/quantization/quantize_/common/kernel_preference.py).
 
-On this engine AUTO resolves to the hand-written sm_100a kernels (``B200``).  ``TORCH`` keeps the
+On this engine AUTO resolves to the hand-written sm_90a kernels (``B200``).  ``TORCH`` keeps the
 reference's library route (``torch._scaled_mm`` / ``torch._int_mm``) and ``EMULATED`` the
 dequantize-then-matmul route; both exist for parity runs only and are never chosen implicitly.
 """

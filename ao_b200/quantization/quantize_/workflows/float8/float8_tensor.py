@@ -1,4 +1,4 @@
-"""e4m3 rowwise-scaled weight, dynamic rowwise activation quant, tcgen05 kind::f8f6f4 GEMM.
+"""e4m3 rowwise-scaled weight, dynamic rowwise activation quant, wgmma e4m3 GEMM.
 
 Attribute names / order match torchao's Float8Tensor
 (torchao/quantization/quantize_/workflows/float8/float8_tensor.py:105-113).  The linear replaces

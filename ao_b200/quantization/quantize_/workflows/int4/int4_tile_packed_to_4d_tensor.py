@@ -1,4 +1,4 @@
-"""int4 weight in the tinygemm tile-packed layout, served by the sm_100a tcgen05 kernel.
+"""int4 weight in the tinygemm tile-packed layout, served by the sm_90a wgmma kernel.
 
 Same class / attribute names and on-disk layout as the reference
 (torchao/quantization/quantize_/workflows/int4/int4_tile_packed_to_4d_tensor.py): ``qdata`` int32
@@ -62,7 +62,7 @@ class Int4TilePackedTo4dTensor(TorchAOBaseTensor):
             # same exception type as the reference, where aten::_convert_weight_to_int4pack has no CPU kernel
             # (test_int4_tile_packed_to_4d_tensor.py:194-202)
             raise NotImplementedError("Could not run 'ao_b200::int4_pack_tile4d' with arguments from the 'CPU' backend: "
-                                      "Int4TilePackedTo4dTensor.from_hp needs a CUDA tensor (sm_100a packing kernel)")
+                                      "Int4TilePackedTo4dTensor.from_hp needs a CUDA tensor (sm_90a packing kernel)")
         original_shape = hp_tensor.shape
         N0, K0 = original_shape
         g = block_size[-1]

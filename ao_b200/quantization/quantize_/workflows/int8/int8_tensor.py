@@ -1,4 +1,4 @@
-"""int8 per-row weight with dynamic per-token int8 activations on tcgen05 kind::i8.
+"""int8 per-row weight with dynamic per-token int8 activations on wgmma s8.
 
 Attribute names / order match torchao's Int8Tensor
 (torchao/quantization/quantize_/workflows/int8/int8_tensor.py:74-85).  The linear replaces

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — headline benchmark of the quantized-linear hot path.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--bs 32] [--impl ours|reference] [--quick]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--bs 32] [--impl ours|reference] [--quick] [--dump-outputs DIR]
 
 Metric (BASELINE.json): tok/s of the Llama-3-8B int4 weight-only (tile_packed_to_4d, group_size=32) linear stack.
 One "step" = one pass of all 32 layers of quantized linears over a batch of `bs` tokens per GPU (decode: one token
@@ -18,12 +18,16 @@ tensor-subclass dispatch -> torch.ops.ao_b200).  The same JSON line carries
   * the roofline of the dominant kernel and a CPU baseline.
 
 Weights are synthetic random-init of the real shapes (no checkpoints offline); 4.36 GB of packed weights per step
->> the 126 MB L2, so no L2 flush is needed between iterations.  Multi-GPU (torchrun): batch sharding, one NCCL
+>> the 50 MB L2 of an H100, so no L2 flush is needed between iterations.  Multi-GPU (torchrun): batch sharding, one NCCL
 broadcast of the packed weights at setup, no collective in the forward; value = N*bs / max-over-ranks time.
 
 --impl reference: the reference's own CPU implementation of the path (torchao's CPU int4 route is the PyTorch-core op
 aten._weight_int4pack_mm_for_cpu, int4_opaque_tensor.py:414), whole steps timed on the host cores, this repo's package
 never imported.
+
+--dump-outputs DIR: after the timed steps, the outputs of the headline path's last step (bs and bs=1) as float32
+DIR/<name>.npy.  Weights and inputs come from fixed seeds, so two builds run with the same arguments can be compared
+output for output.
 """
 from __future__ import annotations
 
@@ -65,23 +69,8 @@ def workload_config(bs, world, layers):
 
 
 def _peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return float(d["hbm_gbs"]), float(d.get("bf16_tflops", 1590.0)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
-
-
-def _traffic_from_profiles(bs):
-    """dram bytes per launch of the dominant kernel from the committed ncu capture (profiles/r02_int4_traffic.json,
-    written by scripts/ncu_traffic.py from an `ncu --set full` report); None when no capture is committed."""
-    p = os.path.join(ROOT, "profiles", "r02_int4_traffic.json")
-    try:
-        with open(p) as f:
-            return float(json.load(f)[f"bs{bs}"]["dram_bytes_per_launch"])
-    except Exception:
-        return None
+    """HBM GB/s and dense bf16 TFLOP/s the roofline fractions are taken against: NVIDIA's H100 SXM data sheet (700 W)."""
+    return 3350.0, 989.0, "H100 SXM data sheet (700 W)"
 
 
 class ClockSampler:
@@ -257,7 +246,8 @@ def run_ours(args):
             sampler.start()
         ms = time_replays(graph, args.steps, args.warmup, barrier)
         clk = sampler.stop() if sampler else None
-        res = {"ms": ms, "launches": launches, "clocks": clk, "finite": bool(torch.isfinite(y_static.float()).all())}
+        res = {"ms": ms, "launches": launches, "clocks": clk, "finite": bool(torch.isfinite(y_static.float()).all()),
+               "y": y_static.float().cpu().numpy()}
         if with_e2e:
             # end-to-end: host buffers, H2D + D2H inside the timed region
             x_host = x_static.cpu().pin_memory()
@@ -278,7 +268,7 @@ def run_ours(args):
             res["ms_e2e"] = e2.elapsed_time(e3) / args.steps
             # eager (no graph) end-to-end, for reference
             e4, e5 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            n_eager = max(1, min(args.steps, 5))
+            n_eager = args.steps
             e4.record()
             with torch.no_grad():
                 for _ in range(n_eager):
@@ -295,6 +285,12 @@ def run_ours(args):
 
     main = measure(args.bs, clocks=True)
     bs1 = measure(1) if args.bs != 1 else main
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, f"y_bs{args.bs}.npy"), main["y"])
+        np.save(os.path.join(args.dump_outputs, "y_bs1.npy"), bs1["y"])
 
     # ---- the kernel the reference calls on a GPU, same weights / chain / protocol / box --------------------
     gpu_ref = None
@@ -348,7 +344,7 @@ def run_ours(args):
         "gpu_launches": main["launches"] * args.steps,
         "clocks": main["clocks"],
         "roofline": {"bound": "hbm", "kernel": "ao::tsg::ts_gemm_kernel<ao::int4k::Int4Fmt, 32>", "achieved": achieved, "peak": peak,
-                     "unit": "GB/s", "frac": achieved / peak, "traffic": _traffic_from_profiles(args.bs),
+                     "unit": "GB/s", "frac": achieved / peak,
                      "algorithmic_bytes_per_launch": ab / max(1, main["launches"]), "peak_source": peak_src,
                      "algorithmic_bytes_per_step": ab, "launches_per_step": main["launches"]},
         "finite_outputs": main["finite"],
@@ -415,7 +411,7 @@ def gpu_reference_int4(model, hidden, batch_sizes, args, dev, barrier):
 
     out = {"kernel": "aten._weight_int4pack_mm (torch " + torch.__version__ + ")",
            "protocol": "same packed weights, same dependent chain, CUDA-graph replays, CUDA events"}
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     for bs in batch_sizes:
         x = torch.randn(bs, hidden, device=dev).to(torch.bfloat16)
         rec = {}
@@ -436,11 +432,12 @@ def gpu_reference_int4(model, hidden, batch_sizes, args, dev, barrier):
 def prefill_gemms(args, dev, peak_tf):
     """Per-GEMM tensor-core roofline at prefill token counts (SURVEY section 8d: the only place the north star's
     ">= 70 % of the tensor-core roofline" clause applies): the four fused Llama-3-8B projections at M = 512 and 4096,
-    int4 weight-only (the prefill-shaped TS kernel, csrc/ts_prefill.cuh) with the kernel the reference calls
+    int4 weight-only (csrc/ts_gemm.cuh in 128-token blocks) with the kernel the reference calls
     (aten._weight_int4pack_mm, M = 512 only: it needs tens of milliseconds at 4096) and cuBLAS bf16 (F.linear on
     bf16 weights, what `peak_tf` was measured with) beside it; fp8-rowwise, int8-dynamic, mxfp8 and nvfp4 with their library kernels.
     TFLOP/s = 2 M N K / time, CUDA events over back-to-back launches on weights + activations larger than L2 for
-    the big shapes; `frac` is against the measured bf16 peak (x2 for the 8-bit kinds)."""
+    the big shapes; `frac` is against the data-sheet bf16 peak (x2 for int8 / fp8; mxfp8 and nvfp4 run bf16 wgmmas
+    on exactly dequantised operands, x1)."""
     import torch
 
     ops = torch.ops.ao_b200
@@ -459,8 +456,8 @@ def prefill_gemms(args, dev, peak_tf):
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / iters * 1e3
 
-    out = {"peak_bf16_tflops": peak_tf, "unit": "TFLOP/s", "note": "one GEMM per entry; frac = TFLOP/s over the measured bf16 "
-           "tensor peak (x2 for fp8 / int8 / mxfp8, x4 for nvfp4); int4 runs ao::tsp::ts_prefill_kernel, the others lowp_linear_kernel in 128-token blocks"}
+    out = {"peak_bf16_tflops": peak_tf, "unit": "TFLOP/s", "note": "one GEMM per entry; frac = TFLOP/s over the data-sheet bf16 "
+           "tensor peak (x2 for fp8 / int8); every kind runs ao::tsg::ts_gemm_kernel in 128-token blocks"}
     for M in (512, 4096):
         for name, N, K in shapes:
             flops = 2.0 * M * N * K
@@ -468,14 +465,14 @@ def prefill_gemms(args, dev, peak_tf):
             rec = {}
             qd = torch.randint(-2**31, 2**31 - 1, (N // 8, K // 128, 32, 4), device=dev, dtype=torch.int32)
             sz = ((torch.rand(K // GROUP, N, 2, device=dev) - 0.5) * 0.004).to(torch.bfloat16)
-            us = t_us(lambda: ops.int4_tilepacked_linear(x, qd, GROUP, sz, None, N, 1), 5)
+            us = t_us(lambda: ops.int4_tilepacked_linear(x, qd, GROUP, sz, None, N, 1), args.steps)
             rec["int4"] = {"us": us, "tflops": flops / us / 1e6, "frac": flops / us / 1e6 / peak_tf}
             if M == 512:
-                lus = t_us(lambda: torch.ops.aten._weight_int4pack_mm(x, qd, GROUP, sz), 2)
+                lus = t_us(lambda: torch.ops.aten._weight_int4pack_mm(x, qd, GROUP, sz), args.steps)
                 rec["int4"]["aten_int4pack_mm_us"] = lus
             del qd, sz
             w = torch.randn(N, K, device=dev).to(torch.bfloat16)
-            rec["bf16_cublas_us"] = t_us(lambda: torch.nn.functional.linear(x, w), 5)
+            rec["bf16_cublas_us"] = t_us(lambda: torch.nn.functional.linear(x, w), args.steps)
             for fmt in ("fp8", "int8", "mxfp8", "nvfp4"):
                 if fmt == "mxfp8":
                     wq, ws = ops.mxfp8_quantize(w, True)
@@ -501,11 +498,11 @@ def prefill_gemms(args, dev, peak_tf):
                     xq, xs = ops.int8_quantize_rowwise(x)
                     fn = lambda: ops.int8_dyn_linear(xq, xs.reshape(-1), wq, ws.reshape(-1), None)
                     lib = lambda: torch._int_mm(xq, wq.t())
-                us = t_us(fn, 5)
-                mul = 4 if fmt == "nvfp4" else 2   # dense peak of the kind relative to bf16
+                us = t_us(fn, args.steps)
+                mul = 2 if fmt in ("fp8", "int8") else 1   # dense peak of the tensor-core kind used, relative to bf16
                 rec[fmt] = {"us": us, "tflops": flops / us / 1e6, "frac": flops / us / 1e6 / (mul * peak_tf)}
                 try:
-                    rec[fmt]["library_us"] = t_us(lib, 5)
+                    rec[fmt]["library_us"] = t_us(lib, args.steps)
                 except Exception as ex:  # pragma: no cover
                     rec[fmt]["library_error"] = f"{type(ex).__name__}: {ex}"[:120]
                 del wq, ws, xq, xs
@@ -525,7 +522,7 @@ def other_configs(args, dev, world, rank, barrier, max_over_ranks, peak):
     from ao_b200.prototype.mx_formats.inference_workflow import NVFP4WeightFloat8ActivationConfig
     from ao_b200.quantization import (Float8DynamicActivationFloat8WeightConfig, Int8DynamicActivationInt8WeightConfig, PerRow)
 
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     plans = []
     if world == 1:
         plans = [
@@ -788,13 +785,16 @@ def run_reference(args):
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20,
+                    help="timed steps of every leg: CUDA-graph replays, or launches per GEMM in the prefill block")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--bs", type=int, default=32, help="tokens per GPU per step (decode batch)")
     ap.add_argument("--layers", type=int, default=0, help="override layer count (debug only; default = 32)")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--quick", action="store_true", help="headline only: skip gpu_reference and the other configs")
     ap.add_argument("--no-fuse", action="store_true", help="7 launches per layer (q, k, v, gate, up not fused)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the headline path's last-step outputs as float32 DIR/<name>.npy")
     a = ap.parse_args()
     if a.warmup < 3:
         a.warmup = 3

@@ -1,5 +1,5 @@
 /*
- * ao_b200.h — C ABI of the B200-native quantized-linear engine (libao_b200.so).
+ * ao_b200.h — C ABI of the H100-native quantized-linear engine (libao_b200.so).
  *
  * This is the drop-in boundary for the quantized nn.Linear forward of pytorch/ao
  * (torchao 0.19).  Every entry point replaces one kernel-level call the reference
@@ -40,7 +40,7 @@ extern "C" {
 /* library / device ---------------------------------------------------------- */
 int ao_b200_version(void);
 const char* ao_b200_last_error(void);
-/* 1 when the current device is compute capability 10.x (sm_100a kernels can run). */
+/* 1 when the current device is compute capability 9.0 (sm_90a kernels can run). */
 int ao_b200_device_ok(void);
 /* bytes of workspace any linear below may need for (M, N) outputs. */
 size_t ao_b200_workspace_bytes(int M, int N);
@@ -78,7 +78,7 @@ int ao_int4_dequant_tile4d(const int32_t* qdata, const uint16_t* scale_and_zero,
  * x bf16 [M,K]; qdata int32 [N/8][K/128][32][4]; scale_and_zero bf16 [K/g][N][2];
  * bias bf16 [N_out] or NULL; y bf16 [M, N_out] with N_out <= N (row stride N_out).
  * K%1024==0 (the format pads K to 1024), N%8==0, g in {32,64,128,256}.
- * impl: 0 = auto, 1 = tcgen05 pipeline, 2 = CUDA-core reference-grade kernel.      */
+ * impl: 0 = auto, 1 = wgmma pipeline, 2 = CUDA-core reference-grade kernel.      */
 int ao_int4_tilepacked_linear(const uint16_t* x, int M, int K, const int32_t* qdata,
                               const uint16_t* scale_and_zero, int group_size, int N,
                               const uint16_t* bias, uint16_t* y, int N_out,
@@ -152,7 +152,7 @@ int ao_nvfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, const flo
                     void* workspace, size_t workspace_bytes, void* stream);
 /* nvfp4 weight-only and nvfp4-weight x fp8-rowwise-activation (BASELINE config 5):
  * y = bf16( (sum_k x[m,k] * e2m1(W)[n,k] * blockscale[n,k/16]) * x_scale[m] * b_pts + bias ),
- * weights dequantised to bf16 inside the tcgen05 kernel.  x is bf16 [M,K]; x_scale f32 [M] or NULL.
+ * weights dequantised to bf16 inside the wgmma kernel.  x is bf16 [M,K]; x_scale f32 [M] or NULL.
  * Semantics = F.linear(x_dq, NVFP4Tensor.dequantize()) (nvfp4_tensor.py:199-231,
  * inference_workflow.py:356-400); for e4m3 activations pass the output of ao_fp8_fakequant_rowwise. */
 int ao_nvfp4_weight_linear(const uint16_t* x, const float* x_scale, int M, int K,

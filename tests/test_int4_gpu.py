@@ -112,8 +112,8 @@ def test_linear_full_size_vs_aten_and_linearity(ops, M, N, K):
     (700, 256, 2048, 256, False),
 ])
 def test_prefill_kernel_vs_oracle(ops, M, N, K, g, bias):
-    """M > 128 runs the prefill-shaped kernel (csrc/ts_prefill.cuh: 256-token tiles, weights dequantised once per
-    tile); same oracle, same 45 dB bar as the decode kernel, ragged token / feature tails included."""
+    """M > 128 runs several 128-token blocks of the kernel (tiles of the stream-K walk); same oracle, same 45 dB bar
+    as the decode sizes, ragged token / feature tails included."""
     o = _o()
     q, q_u8, sz = _mk_q(N, K, g, M * 5 + N)
     qd = ops.int4_pack_tile4d(q_u8, 8)
@@ -159,9 +159,8 @@ def test_prefill_full_size_vs_aten_and_properties(ops, M, N, K):
 
 @pytest.mark.parametrize("M", [65, 100, 128, 512])
 def test_many_token_variants_are_stable_over_repeated_launches(ops, M):
-    """Regression (round 2): with 4 weight stages and 3 dequant warpgroups a warpgroup could pass the parity wait for
-    chunk i + 4 before chunk i had landed -- sporadic wrong results / launch failures of the 65..128-token variant (and of
-    the prefill kernel built on the same ring).  Short per-CTA ranges (a small projection) made it likely."""
+    """The 65..128-token variants launched back to back on a small projection (short per-CTA ranges, many split
+    tiles): stage-ring parity waits and the split-tile flags must hold across launches."""
     N, K, g = 6144, 4096, 32
     q, q_u8, sz = _mk_q(N, K, g, 5)
     qd = ops.int4_pack_tile4d(q_u8, 8)
@@ -221,8 +220,8 @@ def test_quantize_api_end_to_end(ops):
 
 
 def test_prefill_token_counts_through_the_public_api(ops):
-    """quantize_ -> nn.Linear.forward with hundreds / thousands of tokens: a gate|up-sized layer takes the prefill-shaped
-    kernel (>= 50 chunks of 128 x 256 per SM), a small one the 128-token-block path; both against the linear on the
+    """quantize_ -> nn.Linear.forward with hundreds / thousands of tokens, a gate|up-sized layer and a small one, both
+    in 128-token blocks; both against the linear on the
     dequantised weight (>= 45 dB: bf16 output rounding only) and the bf16 linear (>= 20 dB, the reference's bar), with a
     3-D batch and a bias."""
     from ao_b200.quantization import Int4WeightOnlyConfig, quantize_
