@@ -77,13 +77,13 @@ __device__ __forceinline__ void st_release_u32(unsigned* p, unsigned v) {
   asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-// All lanes of the calling warp: wait until flags[0 .. n) are raised (lanes poll distinct flags).
+// All lanes of the calling warp: wait until flags[0 .. n) are raised (lanes poll distinct flags, backing off while a
+// flag is down so that the polling does not compete with the contributors still streaming).
 __device__ __forceinline__ void wait_flags(const unsigned* flags, int n, int lane) {
   for (int base = 0; base < n; base += 32) {
     if (base + lane < n) {
       const unsigned* f = flags + base + lane;
-      while (ld_acquire_u32(f) == 0u) {
-      }
+      while (ld_acquire_u32(f) == 0u) __nanosleep(64);
     }
   }
   __syncwarp();

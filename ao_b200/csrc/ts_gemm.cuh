@@ -12,7 +12,7 @@
 // Roles (384 threads): warpgroup 0 = one TMA producer warp (weights first: they never depend on the previous kernel;
 // activations after griddepcontrol.wait), warpgroups 1 and 2 = consumers (dequant, wgmma, epilogue).  A stage holds
 // one 128-k chunk: weights + scales (wfull) and the activation tile (xfull); the 8 consumer warps hand it back
-// (sempty) once the wgmmas that read it have completed.  The wgmmas of chunk i run while chunk i+1 is dequantised.
+// (sempty) once the wgmmas that read it have completed.  The wgmmas of chunk i overlap chunk i+1's weight loads.
 //
 // Work split (streamk.cuh): the (tile, chunk) units are split evenly over the CTAs; the accumulator of a segment lives
 // in registers and is finished by the consumers right after the segment's last chunk (FULL: outputs, CONTRIB: publish
@@ -226,11 +226,15 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       }
       if (kind == streamk::SEG_OWNER) {
         // own partial + the partials of CTAs b+1 .. b_last in that order (fixed: bit-reproducible run to run)
+        // One warp polls the flags, on distinct lanes at once (one L2 round trip when they are up, not one per
+        // contributor), and the consumer barrier passes its acquire on; narrow tiles then load the partials of GB
+        // contributors before adding any of them
         const int b_last = streamk::cta_of_unit((long long)tile * p.KT + p.KT - 1, U, G);
-        for (int c = b + 1; c <= b_last; ++c)
-          while (streamk::ld_acquire_u32(p.ws_flag + c) == 0u) __nanosleep(64);
+        if (warp == 4) streamk::wait_flags(p.ws_flag + b + 1, b_last - b, lane);
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        constexpr int GB = NACC <= 8 ? 4 : (NACC <= 16 ? 2 : 1);   // registers: GB x NACC words of partials
 #pragma unroll 1
-        for (int c = b + 1; c <= b_last; ++c) {
+        for (int c = b + 1; c <= b_last && GB == 1; ++c) {
           const uint32_t* slot = reinterpret_cast<const uint32_t*>(p.ws_partial) + (size_t)c * (N_MMA * ROWS);
 #pragma unroll
           for (int q = 0; q < NACC / 4; ++q)
@@ -245,6 +249,40 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
                   else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o));
                 }
               }
+        }
+#pragma unroll 1
+        for (int c0 = b + 1; c0 <= b_last && GB > 1; c0 += GB) {
+          uint32_t o[GB][NACC];
+#pragma unroll
+          for (int gi = 0; gi < GB; ++gi) {
+            if (c0 + gi > b_last) break;
+            const uint32_t* slot = reinterpret_cast<const uint32_t*>(p.ws_partial) + (size_t)(c0 + gi) * (N_MMA * ROWS);
+#pragma unroll
+            for (int q = 0; q < NACC / 4; ++q)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int cc = 0; cc < 2; ++cc) {
+                  const int col = 8 * q + 2 * t + cc, r = row_lo + 8 * h, j = 4 * q + 2 * h + cc;
+                  o[gi][j] = m0 + col < p.M ? __ldcg(slot + col * ROWS + r) : 0u;
+                }
+          }
+#pragma unroll
+          for (int gi = 0; gi < GB; ++gi) {
+            if (c0 + gi > b_last) break;
+#pragma unroll
+            for (int q = 0; q < NACC / 4; ++q)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int cc = 0; cc < 2; ++cc) {
+                  const int col = 8 * q + 2 * t + cc, j = 4 * q + 2 * h + cc;
+                  if (m0 + col < p.M) {
+                    if (p.epi == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o[gi][j]);
+                    else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o[gi][j]));
+                  }
+                }
+          }
         }
       }
       // outputs
