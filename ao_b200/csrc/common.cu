@@ -96,6 +96,10 @@ int ts_min_units() {
   return v;
 }
 
+// test-only override of the stream-K grid (ao_b200_debug_set_streamk_ctas); 0 = the heuristic of launch_gemm
+static std::atomic<int> g_streamk_ctas{0};
+int streamk_ctas_override() { return g_streamk_ctas.load(std::memory_order_relaxed); }
+
 int sm_count() {
   static int n = 0;
   if (n == 0) {
@@ -133,5 +137,7 @@ size_t ao_b200_workspace_bytes(int M, int N) {
 }
 
 uint64_t ao_b200_launch_count(void) { return ao::g_launch_count.load(); }
+
+int ao_b200_debug_set_streamk_ctas(int n) { return ao::g_streamk_ctas.exchange(n > 0 ? n : 0); }
 
 }  // extern "C"

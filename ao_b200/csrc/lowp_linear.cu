@@ -8,10 +8,14 @@
 //
 // The weight matrix W[N,K] (K-major, exactly the stored qdata) is the wgmma A operand: 128 output features per tile;
 // the activations are the B operand (N_MMA tokens).  Hopper's tensor cores have no block-scaled kinds, so for mxfp8 and
-// nvfp4 every element is multiplied by its block scale BEFORE the MMA, in bf16, where the product is exact (e4m3 x
-// 2^k: 4 significant bits; e2m1 x e4m3: at most 6): the weights inside the kernel (register-A fragments), the
-// activations by a pre-pass into a bf16 slab of the workspace.  The fp32 sums then see the same products a
-// block-scaled MMA sees.
+// nvfp4 every element is multiplied by its block scale BEFORE the MMA, in bf16: the weights inside the kernel
+// (register-A fragments), the activations by a pre-pass into a bf16 slab of the workspace.  The fp32 sums then see the
+// same products a block-scaled MMA sees, as long as the scaled element is exact in bf16:
+//   * e2m1 x e4m3 (at most 6 significant bits, >= 2^-10): exact for every finite non-negative scale byte, the
+//     subnormal and zero bytes included (nvfp4_fmt.cuh);
+//   * e4m3 x 2^(e-127) (4 significant bits, every code a multiple of 2^-9): exact for e8m0 bytes e >= 3.  For
+//     e = 0, 1, 2 the codes whose lowest set bit lies below 2^-(6+e) need bits under 2^-133, the smallest bf16
+//     subnormal, and round.
 #include <cuda_bf16.h>
 #include <cuda_fp8.h>
 #include <stdlib.h>
@@ -233,7 +237,8 @@ static int block_scaled(const uint8_t* xq, const uint8_t* x_sf, const float* a_p
     int rc = make_tmap(&tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
   }
-  // the partial slots take at most (SMs x 128 x 128) words; the slab starts on the next MiB
+  // the partial slots take at most (SMs x 128 x 128) words; the slab starts on the next MiB (restated by
+  // tests/test_exact_gemm_gpu.py::test_block_scaled_activation_slabs, which sizes workspaces to given slab heights)
   const size_t act_off = (streamk::WS_PARTIAL_OFF + (size_t)sm_count() * ROWS * 128 * 4 + (1u << 20) - 1) & ~(size_t)((1u << 20) - 1);
   const size_t row_bytes = (size_t)K * 2;
   long long slab = ws && ws_bytes > act_off ? (long long)((ws_bytes - act_off) / row_bytes) : 0;

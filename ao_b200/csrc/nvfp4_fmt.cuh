@@ -5,9 +5,15 @@
 // e2m1 -> bf16 without a table: nibble x = (s e1 e0 m) placed at bf16 bits 15|8:6 is the bf16 number
 // value(x) * 2^-126 (denormal for e = 0, which bf16 multiplies handle exactly); ONE exact multiply by
 // (block_scale * 2^66) gives value(x) * block_scale * 2^-60, and the 2^60 is taken back out of the fp32 accumulator in the
-// epilogue (Params::acc_exp2; power-of-two factors commute with every rounding on the way).  bf16(block_scale * 2^66) =
-// (byte << 4) + 0x5D00 for the (always normal, >= 2^-6) e4m3 scale bytes.  The product has at most 6 significant
-// bits, so the bf16 A operand is exact.
+// epilogue (Params::acc_exp2; power-of-two factors commute with every rounding on the way).  The scale byte placed at
+// bf16 bits 10:4 is the bf16 number block_scale * 2^-120 for EVERY byte 0x00..0x7E: normal bytes map exponent to
+// exponent, and the subnormal bytes 0x01..0x07 (m * 2^-9) and the zero byte become bf16 subnormals / zero, which bf16
+// multiplies handle exactly.  Two exact multiplies (by 2^127, then 2^59) give bf16(block_scale * 2^66), once per
+// chunk in load() for two scales at a time rather than once per k16 step in frag(); this is
+// (byte << 4) + 0x5D00 only for the normal bytes >= 0x08, and quantizers without a lower clamp on the scale (such as
+// the TransformerEngine NVFP4 recipe) do write 0x00..0x07.  The product with an e2m1 value has at most 6 significant
+// bits and, when not zero, lies between 2^-70 and 2^-48 (normal), so the bf16 A operand is exact.  Bytes with the sign bit and 0x7F (NaN) are not
+// decoded: no quantizer writes them.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -34,10 +40,11 @@ struct Nvfp4Fmt {
     tma_load_2d(aux_dst, tm_sf, bar, 0, n_tile * p.aux_col_blocks + kc * 2, policy);
   }
   // the thread's two fragment rows: bytes 8kk .. 8kk+7 of each (k16 step kk: byte 8kk + t holds k pair 16kk + 2t,
-  // byte 8kk + 4 + t the pair 8 further), and the two scale words (four e4m3 bytes = four 16-k blocks each)
+  // byte 8kk + 4 + t the pair 8 further), and the eight block scales of each row, decoded once per chunk: s2[h][j] =
+  // bf16x2 of (scale of step 2j, scale of step 2j + 1) * 2^66
   struct Raw {
     uint2 v[2][8];
-    uint32_t sc[2][2];
+    uint32_t s2[2][4];
   };
   __device__ static __forceinline__ void load(const tsg::Params&, uint32_t w_smem, uint32_t aux_smem, int row_lo, int,
                                               Raw& raw) {
@@ -45,8 +52,16 @@ struct Nvfp4Fmt {
     for (int h = 0; h < 2; ++h) {
       const int r = row_lo + 8 * h;
       const uint32_t sc_off = (uint32_t)(r & 31) * 16u + (uint32_t)(r >> 5) * 4u;
-      raw.sc[h][0] = tsg::lds32(aux_smem + sc_off);
-      raw.sc[h][1] = tsg::lds32(aux_smem + 512 + sc_off);
+      const uint32_t sc[2] = {tsg::lds32(aux_smem + sc_off), tsg::lds32(aux_smem + 512 + sc_off)};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        // scale bytes 2j, 2j + 1 at bf16 bits 10:4 of each half = scale * 2^-120, then two exact multiplies
+        const uint32_t bits = __byte_perm(sc[j >> 1], 0u, (j & 1) ? 0x4342u : 0x4140u) << 4;
+        __nv_bfloat162 s2 = *reinterpret_cast<const __nv_bfloat162*>(&bits);
+        s2 = __hmul2(__hmul2(s2, __nv_bfloat162(__ushort_as_bfloat16(0x7F00), __ushort_as_bfloat16(0x7F00))),
+                     __nv_bfloat162(__ushort_as_bfloat16(0x5D00), __ushort_as_bfloat16(0x5D00)));   // * 2^127 * 2^59
+        raw.s2[h][j] = *reinterpret_cast<const uint32_t*>(&s2);
+      }
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk) {
         const uint32_t off = (uint32_t)r * 64u + kk * 8;
@@ -65,8 +80,8 @@ struct Nvfp4Fmt {
     const int t = threadIdx.x & 3;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const uint32_t sb = (raw.sc[h][kk >> 2] >> (8 * (kk & 3))) & 0xFFu;   // the 16-k block of step kk
-      const uint32_t s_bits = ((sb << 4) + 0x5D00u) * 0x00010001u;          // bf16x2 of scale * 2^66
+      // the decoded scale of the 16-k block of step kk, in both halves
+      const uint32_t s_bits = __byte_perm(raw.s2[h][kk >> 1], 0u, (kk & 1) ? 0x3232u : 0x1010u);
       const __nv_bfloat162 s2 = *reinterpret_cast<const __nv_bfloat162*>(&s_bits);
       a[h] = deq((raw.v[h][kk].x >> (8 * t)) & 0xFFu, s2);
       a[h + 2] = deq((raw.v[h][kk].y >> (8 * t)) & 0xFFu, s2);

@@ -26,6 +26,9 @@
 // Forward progress: an owner spins on flags of CTAs with HIGHER block indices.  The launchers keep the grid at or
 // below (SM count x resident CTAs per SM), so every CTA of the grid becomes resident without any other CTA of the
 // same grid having to exit; CTAs of the previous kernel (PDL) never wait on this one.
+//
+// tests/streamk_model.py restates unit_begin, cta_of_unit and Walk on the CPU (and GB, the owner's gather group of
+// ts_gemm.cuh); a change here needs the same change there.
 #pragma once
 #include <stdint.h>
 

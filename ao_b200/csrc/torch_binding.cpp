@@ -172,6 +172,8 @@ TORCH_LIBRARY(ao_b200, m) {
   m.def("int4_tilepacked_linear(Tensor x, Tensor qdata, int group_size, Tensor scale_and_zero, Tensor? bias, int n_out=0, int impl=0) -> Tensor");
   m.def("launch_count() -> int", []() -> int64_t { return (int64_t)ao_b200_launch_count(); });
   m.def("debug_workspace(Tensor like) -> Tensor", [](const at::Tensor& like) { return workspace_for(like); });
+  // tests only: force the stream-K grid of every GEMM launch (0 = heuristic); returns the previous value
+  m.def("debug_set_streamk_ctas(int n) -> int", [](int64_t n) -> int64_t { return ao_b200_debug_set_streamk_ctas((int)n); });
   ao_b200_define_lowp(m);
 }
 

@@ -232,7 +232,8 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         const int b_last = streamk::cta_of_unit((long long)tile * p.KT + p.KT - 1, U, G);
         if (warp == 4) streamk::wait_flags(p.ws_flag + b + 1, b_last - b, lane);
         asm volatile("bar.sync 1, 256;" ::: "memory");
-        constexpr int GB = NACC <= 8 ? 4 : (NACC <= 16 ? 2 : 1);   // registers: GB x NACC words of partials
+        // registers: GB x NACC words of partials (restated by tests/streamk_model.py::group_width)
+        constexpr int GB = NACC <= 8 ? 4 : (NACC <= 16 ? 2 : 1);
 #pragma unroll 1
         for (int c = b + 1; c <= b_last && GB == 1; ++c) {
           const uint32_t* slot = reinterpret_cast<const uint32_t*>(p.ws_partial) + (size_t)c * (N_MMA * ROWS);
@@ -416,6 +417,12 @@ inline int launch_gemm(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm
   int grid = sm_count();
   const int min_units = ts_min_units() ? ts_min_units() : 4;
   if (units / min_units < grid) grid = units / min_units > 0 ? (int)(units / min_units) : 1;
+  if (const int forced = streamk_ctas_override()) {
+    // tests only: at most one CTA per SM (forward progress, see above) and never a CTA without units (its epilogue
+    // would run on an accumulator no wgmma wrote)
+    const int cap = units < sm_count() ? (int)units : sm_count();
+    grid = forced < 1 ? 1 : (forced > cap ? cap : forced);
+  }
   const size_t need = streamk::WS_PARTIAL_OFF + (size_t)grid * N_MMA * ROWS * 4;
   if (!ws || ws_bytes < need || (size_t)grid * 4 > streamk::WS_FLAGS_BYTES)
     return fail(AO_ERR_WORKSPACE, "%s: workspace too small (%zu < %zu)", what, ws_bytes, need);

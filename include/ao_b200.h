@@ -46,6 +46,11 @@ int ao_b200_device_ok(void);
 size_t ao_b200_workspace_bytes(int M, int N);
 /* number of kernels this library has launched since load (bench.py "gpu_launches"). */
 uint64_t ao_b200_launch_count(void);
+/* TEST ONLY: force the CTA count of the stream-K GEMM kernel behind every linear below, so that tests can reach
+ * every split-tile pattern on any SM count.  n > 0 launches clamp(n, 1, min(SM count, work units)) CTAs, n = 0
+ * restores the per-problem heuristic.  Process-wide, not thread-safe against concurrent launches; returns the
+ * previous value.  No production path calls it. */
+int ao_b200_debug_set_streamk_ctas(int n);
 
 /* int4 weight-only, tile_packed_to_4d ---------------------------------------- */
 /* Replaces aten._convert_weight_to_int4pack(uint8[N,K/2], inner_k_tiles)

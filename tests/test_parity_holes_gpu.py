@@ -91,10 +91,12 @@ def test_per_tensor_granularity(fmt, M):
 
 
 @pytest.mark.parametrize("fmt", ["int8", "fp8", "mxfp8"])
-@pytest.mark.parametrize("K", [160, 1056, 4128])
+@pytest.mark.parametrize("K", [32, 160, 1056, 4128])
 def test_k_tail_is_zero_filled(fmt, K):
     """K % 128 != 0 (reference requirements: int8 K % 8, fp8 K % 16, mxfp8 K % 32): the last chunk's tail comes from
-    TMA's out-of-bounds zero fill on both operands; results equal the exact-product restatement of the stored codes."""
+    TMA's out-of-bounds zero fill on both operands; results equal the exact-product restatement of the stored codes.
+    The SQNR bar below cannot see a wrong 32-element tail, so mxfp8 is also checked bit for bit on exactly
+    representable operands (the int8 / fp8 tails are in test_exact_gemm_gpu.py)."""
     import ao_b200  # noqa: F401
     from ao_b200.prototype.mx_formats import MXDynamicActivationMXWeightConfig
     from ao_b200.quantization import (Float8DynamicActivationFloat8WeightConfig, Int8DynamicActivationInt8WeightConfig,
@@ -118,6 +120,13 @@ def test_k_tail_is_zero_filled(fmt, K):
     x2[:, (K // 128) * 128:] = 0
     y2 = lin(x2)
     assert not torch.equal(y, y2), "the K tail did not reach the output"
+    if fmt == "mxfp8":
+        import exact_operands as ex
+
+        for m in (M, 40):
+            case = ex.build("mxfp8", m, N, K, seed=K)
+            y = case.run()
+            assert torch.equal(case.bits(y), case.bits(case.ref())), f"M={m} K={K}: {ex.first_mismatch(case, y)}"
 
 
 def test_c_abi_direct_through_ctypes():
