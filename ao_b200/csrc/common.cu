@@ -73,6 +73,10 @@ cudaError_t ensure_dynamic_smem(const void* kernel, size_t bytes) {
   std::lock_guard<std::mutex> lock(mu);
   if (done.count({kernel, dev})) return cudaSuccess;
   e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  // the whole unified memory as shared memory: a CTA of the next kernel (PDL) can only join an SM whose current
+  // shared-memory carve-out has room for it, so every such kernel asks for the same (largest) one
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   if (e == cudaSuccess) done.insert({kernel, dev});
   return e;
 }

@@ -39,6 +39,7 @@ __device__ __forceinline__ uint32_t deq_pair(uint32_t magic_bits, __nv_bfloat162
 
 struct Int4Fmt {
   static constexpr bool SS = false;
+  static constexpr bool DECODE_2CTA = true;
   static constexpr bool PROMOTE = false;
   static constexpr int X_ELEM_BYTES = 2;
   static constexpr int W_BYTES = ROWS * KCHUNK / 2;   // 8 KiB of 4-bit weights per chunk

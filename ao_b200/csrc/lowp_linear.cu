@@ -39,6 +39,8 @@ template <int KIND>
 struct SsFmt {
   static constexpr bool SS = true;
   static constexpr bool PROMOTE = KIND == KIND_F8;   // int8 sums are exact in s32
+  // e4m3 waits for each chunk's wgmmas (PROMOTE) and measured 14 % slower per decode step at two CTAs per SM
+  static constexpr bool DECODE_2CTA = !PROMOTE;
   static constexpr int X_ELEM_BYTES = 1;
   static constexpr int W_BYTES = ROWS * KCHUNK;   // 16 KiB
   static constexpr int AUX_BYTES = 0;
@@ -69,6 +71,8 @@ __device__ __forceinline__ float e8m0_to_f32(uint32_t e) {
 // mxfp8 weights as the register-A operand: e4m3 pairs x their block-32 e8m0 scale -> bf16 (exact)
 struct Mxfp8Fmt {
   static constexpr bool SS = false;
+  // at 104 consumer registers the dequant of a chunk spills inside the chunk loop: one CTA per SM
+  static constexpr bool DECODE_2CTA = false;
   static constexpr bool PROMOTE = false;
   static constexpr int X_ELEM_BYTES = 2;
   static constexpr int W_BYTES = ROWS * KCHUNK;   // 128 rows x 128 bytes, 128-byte swizzle

@@ -25,6 +25,8 @@ namespace nvf4w {
 
 struct Nvfp4Fmt {
   static constexpr bool SS = false;
+  // at 104 consumer registers the dequant of a chunk spills inside the chunk loop: one CTA per SM
+  static constexpr bool DECODE_2CTA = false;
   static constexpr bool PROMOTE = false;
   static constexpr int X_ELEM_BYTES = 2;
   static constexpr int W_BYTES = tsg::ROWS * tsg::KCHUNK / 2;   // 128 rows x 64 bytes, 64-byte swizzle

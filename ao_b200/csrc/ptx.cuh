@@ -91,6 +91,12 @@ __device__ __forceinline__ void pdl_launch_dependents() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
+// ---------------------------------------------------------------- per-warpgroup register budget (all 128 threads)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- wgmma descriptors
 // K-major operand tile in shared memory, 128-byte swizzle (what TMA SWIZZLE_128B writes): row r at byte r*128,
 // 16-byte chunks XOR-ed with (r%8); 8-row groups 1024 B apart (stride byte offset).  The tile base is 1024-byte

@@ -23,9 +23,14 @@
 // resets the flags it consumed, so the flags are all-zero again when the kernel ends), partial slots [grid][N_MMA * 128] 32-bit words at +64 KiB (slot b = CTA b's CONTRIB partial,
 // column-major: word (j, r) at j * 128 + r).
 //
-// Forward progress: an owner spins on flags of CTAs with HIGHER block indices.  The launchers keep the grid at or
-// below (SM count x resident CTAs per SM), so every CTA of the grid becomes resident without any other CTA of the
-// same grid having to exit; CTAs of the previous kernel (PDL) never wait on this one.
+// Forward progress: an owner spins on flags of CTAs with HIGHER block indices, of its own grid only.  The launchers
+// keep the grid at or below the SM count.  Decode kernels fit two CTAs per SM, so grid j+1 (PDL) shares the SMs with
+// grid j:
+//   * every CTA triggers its dependents first thing, so grid j is entirely resident before any CTA of j+1 launches;
+//     an owner of j therefore only waits on CTAs that are already running;
+//   * a CTA of j+1 touches the workspace, the flags and the activations only after griddepcontrol.wait, i.e. after
+//     grid j has completed; before that it only streams weights into its own shared memory, and j never waits on it;
+//   * CTAs of j+1 that did not find room become resident as CTAs of j exit, which they do without waiting on j+1.
 //
 // tests/streamk_model.py restates unit_begin, cta_of_unit and Walk on the CPU (and GB, the owner's gather group of
 // ts_gemm.cuh); a change here needs the same change there.

@@ -32,8 +32,16 @@ using streamk::ROWS;
 constexpr int KCHUNK = 128;
 constexpr int NUM_THREADS = 384;
 constexpr int CONSUMER_WARPS = 8;
-constexpr int SMEM_BUDGET = 200 * 1024;   // of the 227 KB a block may use on H100: one CTA per SM
 constexpr int MAX_STAGES = 12;
+// Residency.  Decode tiles (N_MMA <= 32) of the formats with Fmt::DECODE_2CTA fit two CTAs per SM: the next linear's
+// CTA (PDL) becomes resident beside the running one and fills its ring with weights during that kernel's tail,
+// instead of starting after it on an empty pipeline.  Each CTA then has half of the SM's 228 KB (less the 1 KB the driver reserves per CTA) and 80 registers
+// per thread at launch; the producer warpgroup gives registers back to the consumers (setmaxnreg).  Prefill tiles
+// keep one CTA per SM and up to 200 KB of ring.
+constexpr int SMEM_PER_SM = 228 * 1024, SMEM_RESERVED_PER_CTA = 1024;
+template <class Fmt, int N_MMA>
+constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA ? 2 : 1; }
+constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
 
 // Epilogue arithmetic, per kind (must stay what each format's reference computes, see Params)
 enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2 };
@@ -63,12 +71,16 @@ struct Cfg {
   static constexpr int X_ATOMS = Fmt::X_ELEM_BYTES;                    // 128-byte-wide swizzle atoms per chunk
   static constexpr int AUX_SLOT = (Fmt::AUX_BYTES + 1023) & ~1023;
   static constexpr int STAGE_BYTES = Fmt::W_BYTES + AUX_SLOT + X_BYTES;
-  static constexpr int STAGES_FIT = SMEM_BUDGET / STAGE_BYTES;
+  static constexpr int CTAS = ctas_per_sm<Fmt, N_MMA>();
+  // one CTA per SM: a 200 KB ring; two: the CTA's share less its barriers (3 x 8 bytes per stage) and alignment pad
+  static constexpr int STAGES_FIT = CTAS == 1 ? 200 * 1024 / STAGE_BYTES
+                                              : (SMEM_PER_SM / 2 - SMEM_RESERVED_PER_CTA - 1024) / (STAGE_BYTES + 24);
   static constexpr int STAGES = STAGES_FIT > MAX_STAGES ? MAX_STAGES : STAGES_FIT;
   static_assert(STAGES >= 2, "stage does not fit");
   static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
   static constexpr int BAR_BYTES = 3 * STAGES * 8;   // wfull, xfull, sempty per stage
   static constexpr size_t SMEM_BYTES = (size_t)BAR_OFF + BAR_BYTES + 1024;   // + the 1024-byte alignment of the base
+  static_assert(CTAS * (SMEM_BYTES + SMEM_RESERVED_PER_CTA) <= SMEM_PER_SM, "CTAs per SM do not fit");
 };
 
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
@@ -93,15 +105,15 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 }
 
 // Fmt policy:
-//   SS, PROMOTE (SS only: sum each chunk's wgmmas into the fp32 registers), X_ELEM_BYTES (2: bf16 activations,
-//   1: 8-bit), W_BYTES, AUX_BYTES (per stage)
+//   SS, PROMOTE (SS only: sum each chunk's wgmmas into the fp32 registers), DECODE_2CTA (two decode CTAs per SM, see
+//   Residency), X_ELEM_BYTES (2: bf16 activations, 1: 8-bit), W_BYTES, AUX_BYTES (per stage)
 //   static void issue_w(tm_w, tm_aux, p, w smem dst, aux smem dst, full barrier, n_tile, kc, policy)  (one thread)
 //   static uint32_t w_tx_bytes(p)
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
 //   RA:  struct Raw; static void load(p, w smem, aux smem, row_lo, lane, Raw&)   rows row_lo and row_lo + 8
 //        static void frag(p, raw, kk, a[4])                        bf16 A fragment of k16 step kk (0..7)
 template <class Fmt, int N_MMA>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(NUM_THREADS, ctas_per_sm<Fmt, N_MMA>())
 ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_aux,
                const __grid_constant__ CUtensorMap tm_x, const Params p) {
   using C = Cfg<Fmt, N_MMA>;
@@ -148,6 +160,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   const bool last_is_owner = walk.seg_kind(seg_last) == streamk::SEG_OWNER;
 
   if (wgi == 0) {
+    if constexpr (C::CTAS > 1) setmaxnreg_dec<PRODUCER_REGS>();   // all four warps, before three of them leave
     if (warp != 0) goto done;
     // ------------------------------------------------------------ TMA producer
     const uint64_t pol_w = policy_evict_first();
@@ -187,6 +200,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
     }
   } else {
     // ------------------------------------------------------------ consumers: warpgroup wg owns rows 64wg .. 64wg+63
+    if constexpr (C::CTAS > 1) setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = wgi - 1, wq = warp & 3;
     const int g = lane >> 2, t = lane & 3;
     const int row_lo = wg * 64 + wq * 16 + g;   // fragment rows row_lo and row_lo + 8 (accumulator rows as well)
@@ -368,16 +382,27 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           for (int kk = 0; kk < 8; ++kk) wgmma_fence_operand(a[kk]);
           if (pending >= 0) release(pending);
           pending = -1;
+          // two halves: the wgmmas of k16 steps 0..3 run while steps 4..7 are dequantised (same wgmmas, same order)
 #pragma unroll
-          for (int kk = 0; kk < 8; ++kk) Fmt::frag(p, raw, kk, a[kk]);
+          for (int kk = 0; kk < 4; ++kk) Fmt::frag(p, raw, kk, a[kk]);
           mbar_wait(&xfull[s], ph);
           wgmma_fence_operand(acc);
-          wgmma_fence();
 #pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {
-            // k16 step kk of the bf16 B tile: atom kk / 4 (64 k each), 32 bytes per step inside the 128-byte row
-            const uint64_t bd = wgmma_desc_k_sw128(x_s + (kk >> 2) * (N_MMA * 128) + (kk & 3) * 32);
-            MMA::ra_bf16(acc, a[kk], bd, kk == 0 ? scale_d : 1u);
+          for (int half = 0; half < 2; ++half) {
+            if (half == 1) {
+              // the raw words pass through here after the first half is issued, so its dequant cannot move above
+              uint32_t(&rw)[sizeof(raw) / 4] = *reinterpret_cast<uint32_t(*)[sizeof(raw) / 4]>(&raw);
+              wgmma_fence_operand(rw);
+#pragma unroll
+              for (int kk = 4; kk < 8; ++kk) Fmt::frag(p, raw, kk, a[kk]);
+            }
+            wgmma_fence();   // orders the fragment registers just written before the wgmmas that read them
+#pragma unroll
+            for (int kk = 4 * half; kk < 4 * half + 4; ++kk) {
+              // k16 step kk of the bf16 B tile: atom kk / 4 (64 k each), 32 bytes per step inside the 128-byte row
+              const uint64_t bd = wgmma_desc_k_sw128(x_s + (kk >> 2) * (N_MMA * 128) + (kk & 3) * 32);
+              MMA::ra_bf16(acc, a[kk], bd, kk == 0 ? scale_d : 1u);
+            }
           }
         }
         wgmma_commit();
@@ -405,8 +430,8 @@ done:
 
 // ------------------------------------------------------------------------------------------------ host side
 // Grid choice + workspace carve-up shared by the launchers of this kernel.
-//   * at most one CTA per SM (the stage ring takes most of the shared memory): the grid stays within the resident
-//     capacity, which the owner protocol needs for forward progress (streamk.cuh)
+//   * at most one CTA of the grid per SM: the grid stays within the resident capacity, which the owner protocol needs
+//     for forward progress (streamk.cuh), and a decode SM keeps room for the next kernel's CTA
 //   * never fewer than `min_units` chunks per CTA: splitting a tile over more CTAs shortens the streaming phase but
 //     lengthens the owner's gather
 template <class Fmt, int N_MMA>
