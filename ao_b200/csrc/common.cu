@@ -90,16 +90,6 @@ bool pdl_enabled() {
   return v == 1;
 }
 
-int ts_min_units() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("AO_B200_TS_MIN_UNITS");
-    v = e ? atoi(e) : 0;   // 0 = choose per problem size
-    if (v < 0 || v > 64) v = 0;
-  }
-  return v;
-}
-
 // test-only override of the stream-K grid (ao_b200_debug_set_streamk_ctas); 0 = the heuristic of launch_gemm
 static std::atomic<int> g_streamk_ctas{0};
 int streamk_ctas_override() { return g_streamk_ctas.load(std::memory_order_relaxed); }
@@ -135,8 +125,8 @@ int ao_b200_device_ok(void) {
 size_t ao_b200_workspace_bytes(int M, int N) {
   (void)M;
   (void)N;
-  // semaphores (64 KiB) + split-K partials: at most ~2*SMs tiles of 128x128 fp32 are ever
-  // split (see choose_splits in each kernel file); 24 MiB covers every configuration.
+  // the split-tile flags (64 KiB), then at most (SM count) x 128 x 128 32-bit words of stream-K partials, then (the
+  // block-scaled linears, from the next MiB on) the bf16 activation slab: as many rows as fit in what is left.
   return (size_t)64 * 1024 + (size_t)24 * 1024 * 1024;
 }
 

@@ -68,7 +68,6 @@ cudaError_t ensure_dynamic_smem(const void* kernel, size_t bytes);
 
 // PDL can be disabled globally (AO_B200_NO_PDL=1) for debugging.
 bool pdl_enabled();
-int ts_min_units();    // AO_B200_TS_MIN_UNITS: minimum chunks per CTA of ts_gemm.cuh grids, 0 = by problem size
 int streamk_ctas_override();   // ao_b200_debug_set_streamk_ctas (tests only): forced ts_gemm.cuh grid, 0 = none
 int sm_count();
 

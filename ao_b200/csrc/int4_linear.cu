@@ -5,7 +5,7 @@
 // Replaces aten._weight_int4pack_mm as called from the reference handler
 // (torchao/quantization/quantize_/workflows/int4/int4_tile_packed_to_4d_tensor.py:243-299).
 // The GEMM itself is the persistent wgmma kernel of ts_gemm.cuh; this file supplies the int4 format policy (how a
-// 128-row x 128-k chunk is fetched and turned into bf16 wgmma A fragments) and the launcher.
+// 128-row x 128-k chunk is fetched and turned into bf16 wgmma A fragments) and the C entry point.
 //
 // qdata layout (int32 [N/8][K/128][32][4], inner_k_tiles = 8), word `wd` of lane `t`:
 //   row n = 8*n8 + t/4;  k0 = 128*ko + 32*wd + 2*(t%4);
@@ -44,6 +44,26 @@ struct Int4Fmt {
   static constexpr int X_ELEM_BYTES = 2;
   static constexpr int W_BYTES = ROWS * KCHUNK / 2;   // 8 KiB of 4-bit weights per chunk
   static constexpr int AUX_BYTES = 2048;              // (s, z) pairs: up to 4 groups x 128 rows x 4 B
+  static constexpr int EPI = tsg::EPI_FLOAT;
+  static constexpr int ACC_EXP2 = 0;
+  static constexpr int MAX_N_MMA = 128;
+  // the packed weights ({32 words, 4 row-pairs, 16 n8-tiles} box, 128-byte swizzle) and the (scale, zero) pairs
+  static int make_maps(const int32_t* qdata, const uint16_t* sz, int N, int K, int g, CUtensorMap* tm_w,
+                       CUtensorMap* tm_sz) {
+    const int KT = K / 128;
+    {
+      const uint64_t dims[3] = {32, (uint64_t)4 * KT, (uint64_t)N / 8};
+      const uint64_t str[2] = {128, (uint64_t)KT * 512};
+      const uint32_t box[3] = {32, 4, 16};
+      int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_INT32, 3, qdata, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+      if (rc) return rc;
+    }
+    const int gpc = g <= 128 ? 128 / g : 1;
+    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)K / g};
+    const uint64_t str[1] = {(uint64_t)N * 4};
+    const uint32_t box[2] = {128, (uint32_t)gpc};
+    return make_tmap(tm_sz, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, sz, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
   __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params& p) {
     const int gpc = p.group_size <= KCHUNK ? KCHUNK / p.group_size : 1;
     return W_BYTES + gpc * 512;
@@ -147,54 +167,6 @@ __global__ void int4_linear_simple_kernel(const __nv_bfloat16* __restrict__ x,
   }
 }
 
-
-// tensor maps of the packed weights ({32 words, 4 row-pairs, 16 n8-tiles} box, 128-byte swizzle), the (scale, zero)
-// pairs and the activations (box = 64 k x `x_rows` tokens)
-static int make_maps(const uint16_t* x, int ldx, int M, int K, const int32_t* qdata, const uint16_t* sz, int g, int N,
-                     int x_rows, CUtensorMap* tm_w, CUtensorMap* tm_sz, CUtensorMap* tm_x) {
-  const int KT = K / 128;
-  {
-    const uint64_t dims[3] = {32, (uint64_t)4 * KT, (uint64_t)N / 8};
-    const uint64_t str[2] = {128, (uint64_t)KT * 512};
-    const uint32_t box[3] = {32, 4, 16};
-    int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_INT32, 3, qdata, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
-  const int gpc = g <= 128 ? 128 / g : 1;
-  {
-    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)K / g};
-    const uint64_t str[1] = {(uint64_t)N * 4};
-    const uint32_t box[2] = {128, (uint32_t)gpc};
-    int rc = make_tmap(tm_sz, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, sz, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-    if (rc) return rc;
-  }
-  {
-    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
-    const uint64_t str[1] = {(uint64_t)ldx * 2};
-    const uint32_t box[2] = {64, (uint32_t)x_rows};
-    int rc = make_tmap(tm_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
-  return AO_OK;
-}
-
-template <int N_MMA>
-static int launch_tc(const uint16_t* x, int ldx, int M, int K, const int32_t* qdata, const uint16_t* sz, int g, int N,
-                     const uint16_t* bias, uint16_t* y, int N_out, void* ws, size_t ws_bytes,
-                     cudaStream_t stream) {
-  CUtensorMap tm_w, tm_sz, tm_x;
-  if (int rc = make_maps(x, ldx, M, K, qdata, sz, g, N, N_MMA, &tm_w, &tm_sz, &tm_x)) return rc;
-  tsg::Params p{};
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.epi = tsg::EPI_FLOAT;
-  p.M = M; p.N = N; p.N_out = N_out; p.K = K; p.group_size = g;
-  p.n_tiles = ceil_div(N_out, ROWS);
-  p.m_blocks = ceil_div(M, N_MMA);
-  p.KT = K / 128;
-  return tsg::launch_gemm<Int4Fmt, N_MMA>(p, tm_w, tm_sz, tm_x, ws, ws_bytes, "int4 linear", stream);
-}
-
 }  // namespace int4k
 }  // namespace ao
 
@@ -225,17 +197,13 @@ extern "C" int ao_int4_tilepacked_linear_strided(const uint16_t* x, int ldx, int
                          reinterpret_cast<__nv_bfloat16*>(y), M, N, N_out, K, group_size, ldx));
     return AO_OK;
   }
-  if (M <= 16)
-    return int4k::launch_tc<16>(x, ldx, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
-                                workspace_bytes, st);
-  if (M <= 32)
-    return int4k::launch_tc<32>(x, ldx, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
-                                workspace_bytes, st);
-  if (M <= 64)
-    return int4k::launch_tc<64>(x, ldx, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
-                                workspace_bytes, st);
-  return int4k::launch_tc<128>(x, ldx, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
-                               workspace_bytes, st);
+  CUtensorMap tm_w, tm_sz;
+  if (int rc = int4k::Int4Fmt::make_maps(qdata, scale_and_zero, N, K, group_size, &tm_w, &tm_sz)) return rc;
+  tsg::Params p{};
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.M = M; p.N = N; p.N_out = N_out; p.K = K; p.group_size = group_size;
+  return tsg::run<int4k::Int4Fmt>(p, tm_w, tm_sz, x, ldx, workspace, workspace_bytes, "int4 linear", st);
 }
 
 extern "C" int ao_int4_tilepacked_linear(const uint16_t* x, int M, int K, const int32_t* qdata,

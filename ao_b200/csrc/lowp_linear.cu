@@ -3,6 +3,7 @@
 //   e4m3 x e4m3 -> f32    (wgmma e4m3, both operands TMA tiles)    replaces torch._scaled_mm rowwise
 //   mxfp8 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm block-scaled
 //   nvfp4 block-16 e4m3   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm fp4 + pts/bias kernels
+//   nvfp4 weight x bf16   (bf16 wgmma, weights dequantised exactly)      replaces F.linear on the dequantised weight
 // Reference call sites: int8/kernels.py:18-76,114-144 + int8_tensor.py:305-359;
 // float8/inference.py:86-123; mx_formats/mx_tensor.py:759-843; nvfp4_tensor.py:487-578.
 //
@@ -20,6 +21,8 @@
 #include <cuda_fp8.h>
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "common.h"
 #include "nvfp4_fmt.cuh"
 #include "ptx.cuh"
@@ -34,6 +37,14 @@ enum Kind { KIND_I8 = 0, KIND_F8 = 1, KIND_MXF8 = 2, KIND_NVF4 = 3 };
 using tsg::KCHUNK;
 using tsg::ROWS;
 
+// K-major byte weights W[N][K] in 128-row x 128-k boxes, 128-byte swizzle (int8, e4m3, mxfp8)
+static int kmajor_byte_map(const uint8_t* wq, int N, int K, CUtensorMap* tm) {
+  const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
+  const uint64_t str[1] = {(uint64_t)K};
+  const uint32_t box[2] = {KCHUNK, ROWS};
+  return make_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
 // int8 / e4m3: both operands straight from the TMA tiles (128-byte swizzle, 128 k per chunk = four k32 wgmmas)
 template <int KIND>
 struct SsFmt {
@@ -44,6 +55,15 @@ struct SsFmt {
   static constexpr int X_ELEM_BYTES = 1;
   static constexpr int W_BYTES = ROWS * KCHUNK;   // 16 KiB
   static constexpr int AUX_BYTES = 0;
+  static constexpr int EPI = KIND == KIND_I8 ? tsg::EPI_I8 : tsg::EPI_F8;
+  static constexpr int ACC_EXP2 = 0;
+  static constexpr int MAX_N_MMA = KIND == KIND_F8 ? 64 : 128;   // e4m3 keeps a second accumulator per chunk
+  // no aux operand: the weight map stands in for it, so that the kernel's descriptor prefetch reads a valid map
+  static int make_maps(const uint8_t* wq, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    if (int rc = kmajor_byte_map(wq, N, K, tm_w)) return rc;
+    *tm_aux = *tm_w;
+    return AO_OK;
+  }
   __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES; }
   __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap*, const tsg::Params&,
                                                  uint8_t* w_dst, uint8_t*, uint64_t* bar, int n_tile, int kc,
@@ -77,7 +97,17 @@ struct Mxfp8Fmt {
   static constexpr int X_ELEM_BYTES = 2;
   static constexpr int W_BYTES = ROWS * KCHUNK;   // 128 rows x 128 bytes, 128-byte swizzle
   static constexpr int AUX_BYTES = 512;           // one blocked scale tile (4 scales = 128 k per row)
+  static constexpr int EPI = tsg::EPI_FLOAT;
   static constexpr int ACC_EXP2 = 0;
+  static constexpr int MAX_N_MMA = 128;
+  // the weights and the blocked scale tiles, one 512-byte tile per box
+  static int make_maps(const uint8_t* wq, const uint8_t* w_sf, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
+    if (int rc = kmajor_byte_map(wq, N, K, tm_w)) return rc;
+    const uint64_t dims[2] = {128, (uint64_t)ceil_div(N, ROWS) * (uint64_t)ceil_div(K / 32, 4)};
+    const uint64_t str[1] = {512};
+    const uint32_t box[2] = {128, 1};
+    return make_tmap(tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
   __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES + AUX_BYTES; }
   __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap* tm_sf, const tsg::Params& p,
                                                  uint8_t* w_dst, uint8_t* aux_dst, uint64_t* bar, int n_tile, int kc,
@@ -164,56 +194,21 @@ __global__ void __launch_bounds__(256) dequant_act_kernel(const uint8_t* __restr
   dst[1] = reinterpret_cast<const uint4*>(o)[1];
 }
 
-template <class Fmt, int N_MMA>
-static int launch_gemm(tsg::Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const void* x, int x_elem,
-                       int ld_bytes, void* ws, size_t ws_bytes, cudaStream_t st) {
-  CUtensorMap tm_x;
-  {
-    const uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.M};
-    const uint64_t str[1] = {(uint64_t)ld_bytes};
-    const uint32_t box[2] = {(uint32_t)(128 / x_elem), (uint32_t)N_MMA};
-    int rc = make_tmap(&tm_x, x_elem == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, x, dims,
-                       str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
-  p.m_blocks = ceil_div(p.M, N_MMA);
-  return tsg::launch_gemm<Fmt, N_MMA>(p, tm_w, tm_aux, tm_x, ws, ws_bytes, "lowp linear", st);
-}
-
-// MAX_N: widest token tile (fp8 keeps a second accumulator per chunk: 64 tokens)
-template <class Fmt, int MAX_N = 128>
-static int dispatch_m(tsg::Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const void* x, int x_elem,
-                      int ld_bytes, void* ws, size_t ws_bytes, cudaStream_t st) {
-  if (p.M <= 16) return launch_gemm<Fmt, 16>(p, tm_w, tm_aux, x, x_elem, ld_bytes, ws, ws_bytes, st);
-  if (p.M <= 32) return launch_gemm<Fmt, 32>(p, tm_w, tm_aux, x, x_elem, ld_bytes, ws, ws_bytes, st);
-  if (p.M <= 64 || MAX_N == 64) return launch_gemm<Fmt, 64>(p, tm_w, tm_aux, x, x_elem, ld_bytes, ws, ws_bytes, st);
-  return launch_gemm<Fmt, (MAX_N == 64 ? 64 : 128)>(p, tm_w, tm_aux, x, x_elem, ld_bytes, ws, ws_bytes, st);
-}
-
 // int8 / fp8 rowwise
 template <int KIND>
 static int rowwise(const uint8_t* xq, const float* x_scale, int M, int K, const uint8_t* wq, const float* w_scale, int N,
                    const uint16_t* bias, uint16_t* y, int32_t* i32_out, void* ws, size_t ws_bytes, void* stream) {
-  CUtensorMap tm_w;
-  {
-    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
-    const uint64_t str[1] = {(uint64_t)K};
-    const uint32_t box[2] = {KCHUNK, ROWS};
-    int rc = make_tmap(&tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
+  using Fmt = SsFmt<KIND>;
+  CUtensorMap tm_w, tm_aux;
+  if (int rc = Fmt::make_maps(wq, N, K, &tm_w, &tm_aux)) return rc;
   tsg::Params p{};
   p.row_scale = x_scale;
   p.w_scale = w_scale;
   p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   p.y = reinterpret_cast<__nv_bfloat16*>(y);
   p.i32_out = i32_out;
-  p.epi = KIND == KIND_I8 ? tsg::EPI_I8 : tsg::EPI_F8;
   p.M = M; p.N = N; p.N_out = N; p.K = K;
-  p.n_tiles = ceil_div(N, ROWS);
-  p.KT = ceil_div(K, KCHUNK);   // a K tail is zero-filled by TMA (out-of-bounds box elements) on both operands
-  return dispatch_m<SsFmt<KIND>, (KIND == KIND_F8 ? 64 : 128)>(p, tm_w, tm_w, xq, 1, K, ws, ws_bytes,
-                                                                 reinterpret_cast<cudaStream_t>(stream));
+  return tsg::run<Fmt>(p, tm_w, tm_aux, xq, K, ws, ws_bytes, "lowp linear", reinterpret_cast<cudaStream_t>(stream));
 }
 
 // mxfp8 / nvfp4: activation slabs dequantised into the workspace behind the partial slots, one GEMM per slab
@@ -221,26 +216,12 @@ template <int KIND>
 static int block_scaled(const uint8_t* xq, const uint8_t* x_sf, const float* a_pts, int M, int K, const uint8_t* wq,
                         const uint8_t* w_sf, const float* b_pts, int N, const uint16_t* bias, uint16_t* y, void* ws,
                         size_t ws_bytes, void* stream) {
+  using Fmt = std::conditional_t<KIND == KIND_NVF4, nvf4w::Nvfp4Fmt, Mxfp8Fmt>;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUtensorMap tm_w, tm_sf;
   const int sf_per_row = KIND == KIND_MXF8 ? K / 32 : K / 16;
   const int sf_col_blocks = ceil_div(sf_per_row, 4);
-  if (KIND == KIND_NVF4) {
-    if (int rc = nvf4w::make_weight_maps(wq, w_sf, N, K, &tm_w, &tm_sf)) return rc;
-  } else {
-    {
-      const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
-      const uint64_t str[1] = {(uint64_t)K};
-      const uint32_t box[2] = {KCHUNK, ROWS};
-      int rc = make_tmap(&tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-      if (rc) return rc;
-    }
-    const uint64_t dims[2] = {128, (uint64_t)ceil_div(N, ROWS) * (uint64_t)sf_col_blocks};
-    const uint64_t str[1] = {512};
-    const uint32_t box[2] = {128, 1};
-    int rc = make_tmap(&tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-    if (rc) return rc;
-  }
+  CUtensorMap tm_w, tm_sf;
+  if (int rc = Fmt::make_maps(wq, w_sf, N, K, &tm_w, &tm_sf)) return rc;
   // the partial slots take at most (SMs x 128 x 128) words; the slab starts on the next MiB (restated by
   // tests/test_exact_gemm_gpu.py::test_block_scaled_activation_slabs, which sizes workspaces to given slab heights)
   const size_t act_off = (streamk::WS_PARTIAL_OFF + (size_t)sm_count() * ROWS * 128 * 4 + (1u << 20) - 1) & ~(size_t)((1u << 20) - 1);
@@ -258,21 +239,11 @@ static int block_scaled(const uint8_t* xq, const uint8_t* x_sf, const float* a_p
     tsg::Params p{};
     p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
     p.y = reinterpret_cast<__nv_bfloat16*>(y) + (size_t)m0 * N;
-    p.epi = tsg::EPI_FLOAT;
     p.out_scale = KIND == KIND_NVF4 ? b_pts : nullptr;
     p.out_scale2 = KIND == KIND_NVF4 ? a_pts : nullptr;
     p.aux_col_blocks = sf_col_blocks;
     p.M = rows; p.N = N; p.N_out = N; p.K = K;
-    p.n_tiles = ceil_div(N, ROWS);
-    p.KT = ceil_div(K, KCHUNK);   // mxfp8: a K tail is zero-filled by TMA on both operands
-    int rc;
-    if (KIND == KIND_NVF4) {
-      p.acc_exp2 = nvf4w::Nvfp4Fmt::ACC_EXP2;
-      rc = dispatch_m<nvf4w::Nvfp4Fmt>(p, tm_w, tm_sf, xb, 2, K * 2, ws, act_off, st);
-    } else {
-      rc = dispatch_m<Mxfp8Fmt>(p, tm_w, tm_sf, xb, 2, K * 2, ws, act_off, st);
-    }
-    if (rc) return rc;
+    if (int rc = tsg::run<Fmt>(p, tm_w, tm_sf, xb, K, ws, act_off, "lowp linear", st)) return rc;
   }
   return AO_OK;
 }
@@ -342,4 +313,41 @@ extern "C" int ao_nvfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked
   AO_REQUIRE(xq && x_scale_blocked && wq && w_scale_blocked && y, "nvfp4 linear: null pointer");
   return lowp::block_scaled<lowp::KIND_NVF4>(xq, x_scale_blocked, a_pts, M, K, wq, w_scale_blocked, b_pts, N, bias, y,
                                              workspace, workspace_bytes, stream);
+}
+
+// nvfp4 weights x bf16 activations = F.linear(x, NVFP4Tensor.dequantize()) (nvfp4_tensor.py:199-231, weight-only
+// handler inference_workflow.py:356-400).  The optional per-token x_scale is applied in the epilogue, so that
+// e4m3-rowwise activations (ao_fp8_fakequant_rowwise: values exact in bf16, the scale a row factor) run on the same
+// kernel; b_pts is one per-tensor scale or (b_pts_per_row) one per output feature.
+extern "C" int ao_nvfp4_weight_linear_ex(const uint16_t* x, int ldx, const float* x_scale, int M, int K, const uint8_t* wq,
+                                         const uint8_t* w_scale_blocked, const float* b_pts, int b_pts_per_row, int N,
+                                         const uint16_t* bias, uint16_t* y, void* workspace, size_t workspace_bytes,
+                                         void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "nvfp4 weight linear: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(K % 128 == 0, "nvfp4 weight linear: K=%d must be a multiple of 128", K);
+  AO_REQUIRE(N % 16 == 0, "nvfp4 weight linear: N=%d must be a multiple of 16 (inference_workflow.py:248-251)", N);
+  AO_REQUIRE(ldx >= K && ldx % 8 == 0, "nvfp4 weight linear: ldx=%d must be >= K=%d and a multiple of 8", ldx, K);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && wq && w_scale_blocked && y, "nvfp4 weight linear: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "nvfp4 weight linear: x must be 16-byte aligned");
+  CUtensorMap tm_w, tm_sf;
+  if (int rc = nvf4w::Nvfp4Fmt::make_maps(wq, w_scale_blocked, N, K, &tm_w, &tm_sf)) return rc;
+  tsg::Params p{};
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.row_scale = x_scale;
+  p.out_scale = b_pts;
+  p.out_scale_per_row = b_pts_per_row;
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.aux_col_blocks = ceil_div(K / 16, 4);
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<nvf4w::Nvfp4Fmt>(p, tm_w, tm_sf, x, ldx, workspace, workspace_bytes, "nvfp4 weight linear",
+                                   reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ao_nvfp4_weight_linear(const uint16_t* x, const float* x_scale, int M, int K, const uint8_t* wq,
+                                      const uint8_t* w_scale_blocked, const float* b_pts, int N,
+                                      const uint16_t* bias, uint16_t* y, void* workspace, size_t workspace_bytes,
+                                      void* stream) {
+  return ao_nvfp4_weight_linear_ex(x, K, x_scale, M, K, wq, w_scale_blocked, b_pts, 0, N, bias, y, workspace, workspace_bytes,
+                                   stream);
 }

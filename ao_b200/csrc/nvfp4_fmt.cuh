@@ -5,7 +5,7 @@
 // e2m1 -> bf16 without a table: nibble x = (s e1 e0 m) placed at bf16 bits 15|8:6 is the bf16 number
 // value(x) * 2^-126 (denormal for e = 0, which bf16 multiplies handle exactly); ONE exact multiply by
 // (block_scale * 2^66) gives value(x) * block_scale * 2^-60, and the 2^60 is taken back out of the fp32 accumulator in the
-// epilogue (Params::acc_exp2; power-of-two factors commute with every rounding on the way).  The scale byte placed at
+// epilogue (ACC_EXP2; power-of-two factors commute with every rounding on the way).  The scale byte placed at
 // bf16 bits 10:4 is the bf16 number block_scale * 2^-120 for EVERY byte 0x00..0x7E: normal bytes map exponent to
 // exponent, and the subnormal bytes 0x01..0x07 (m * 2^-9) and the zero byte become bf16 subnormals / zero, which bf16
 // multiplies handle exactly.  Two exact multiplies (by 2^127, then 2^59) give bf16(block_scale * 2^66), once per
@@ -31,7 +31,23 @@ struct Nvfp4Fmt {
   static constexpr int X_ELEM_BYTES = 2;
   static constexpr int W_BYTES = tsg::ROWS * tsg::KCHUNK / 2;   // 128 rows x 64 bytes, 64-byte swizzle
   static constexpr int AUX_BYTES = 1024;                        // two blocked scale tiles (64 k each)
-  static constexpr int ACC_EXP2 = 60;   // the accumulators hold the result * 2^-60 (Params::acc_exp2)
+  static constexpr int EPI = tsg::EPI_FLOAT;
+  static constexpr int ACC_EXP2 = 60;   // the accumulators hold the result * 2^-60
+  static constexpr int MAX_N_MMA = 128;
+  // the packed weights (128 rows x 64 bytes, 64B swizzle) and the blocked scale tiles
+  static int make_maps(const uint8_t* wq, const uint8_t* w_sf, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
+    {
+      const uint64_t dims[2] = {(uint64_t)K / 2, (uint64_t)N};
+      const uint64_t str[1] = {(uint64_t)K / 2};
+      const uint32_t box[2] = {64, 128};
+      int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B);
+      if (rc) return rc;
+    }
+    const uint64_t dims[2] = {128, (uint64_t)ceil_div(N, tsg::ROWS) * (uint64_t)ceil_div(K / 16, 4)};
+    const uint64_t str[1] = {512};
+    const uint32_t box[2] = {128, 2};
+    return make_tmap(tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
   __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES + AUX_BYTES; }
   __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap* tm_sf, const tsg::Params& p,
                                                  uint8_t* w_dst, uint8_t* aux_dst, uint64_t* bar, int n_tile, int kc,
@@ -90,21 +106,6 @@ struct Nvfp4Fmt {
     }
   }
 };
-
-// tensor maps of the packed weights (128 rows x 64 bytes, 64B swizzle) and of the blocked scale tiles
-inline int make_weight_maps(const uint8_t* wq, const uint8_t* w_sf, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
-  {
-    const uint64_t dims[2] = {(uint64_t)K / 2, (uint64_t)N};
-    const uint64_t str[1] = {(uint64_t)K / 2};
-    const uint32_t box[2] = {64, 128};
-    int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B);
-    if (rc) return rc;
-  }
-  const uint64_t dims[2] = {128, (uint64_t)ceil_div(N, tsg::ROWS) * (uint64_t)ceil_div(K / 16, 4)};
-  const uint64_t str[1] = {512};
-  const uint32_t box[2] = {128, 2};
-  return make_tmap(tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-}
 
 }  // namespace nvf4w
 }  // namespace ao

@@ -43,7 +43,7 @@ template <class Fmt, int N_MMA>
 constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA ? 2 : 1; }
 constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
 
-// Epilogue arithmetic, per kind (must stay what each format's reference computes, see Params)
+// Epilogue arithmetic, per kind (Fmt::EPI; must stay what each format's reference computes, see Params)
 enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2 };
 
 struct Params {
@@ -52,10 +52,7 @@ struct Params {
   const float* out_scale;   // EPI_FLOAT: optional device scalar, or (out_scale_per_row) one value per output feature
   const float* out_scale2;  // EPI_FLOAT: optional second device scalar multiplied into out_scale (nvfp4 a_pts * b_pts)
   int out_scale_per_row;
-  int acc_exp2;             // the accumulators hold the result * 2^-acc_exp2 (format policy folds a power of two into
-                            // its dequant multiply); undone in the epilogue together with out_scale
   const float* w_scale;     // EPI_I8 / EPI_F8: per-output-feature weight scale [N]
-  int epi;
   __nv_bfloat16* y;         // [M, N_out]
   int32_t* i32_out;         // EPI_I8: raw int32 accumulators [M, N] instead of y
   float* ws_partial;        // [grid][N_MMA*128]   CTA b's CONTRIB partial (streamk.cuh)
@@ -106,7 +103,10 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 
 // Fmt policy:
 //   SS, PROMOTE (SS only: sum each chunk's wgmmas into the fp32 registers), DECODE_2CTA (two decode CTAs per SM, see
-//   Residency), X_ELEM_BYTES (2: bf16 activations, 1: 8-bit), W_BYTES, AUX_BYTES (per stage)
+//   Residency), X_ELEM_BYTES (2: bf16 activations, 1: 8-bit), W_BYTES, AUX_BYTES (per stage), EPI (epilogue kind),
+//   ACC_EXP2 (the accumulators hold the result * 2^-ACC_EXP2: a power of two folded into the dequant multiply, undone
+//   in the EPI_FLOAT epilogue together with out_scale), MAX_N_MMA (widest token tile: 64 or 128)
+//   static int make_maps(...)  host: the weight and aux tensor maps of one GEMM (arguments per format)
 //   static void issue_w(tm_w, tm_aux, p, w smem dst, aux smem dst, full barrier, n_tile, kc, policy)  (one thread)
 //   static uint32_t w_tx_bytes(p)
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
@@ -252,7 +252,10 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         for (int c = b + 1; c <= b_last && GB == 1; ++c) {
           const uint32_t* slot = reinterpret_cast<const uint32_t*>(p.ws_partial) + (size_t)c * (N_MMA * ROWS);
 #pragma unroll
-          for (int q = 0; q < NACC / 4; ++q)
+          for (int q = 0; q < NACC / 4; ++q) {
+            // a warp-uniform exit every 16 tokens (the rest of the tile is past M).  The branch also bounds the loads the
+            // compiler hoists above their adds to 8 words; hoisting all NACC of them spills at N_MMA = 128
+            if (q % 2 == 0 && m0 + 8 * q >= p.M) break;
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -260,10 +263,11 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
                 const int col = 8 * q + 2 * t + cc, r = row_lo + 8 * h, j = 4 * q + 2 * h + cc;
                 if (m0 + col < p.M) {
                   const uint32_t o = __ldcg(slot + col * ROWS + r);
-                  if (p.epi == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o);
+                  if constexpr (Fmt::EPI == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o);
                   else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o));
                 }
               }
+          }
         }
 #pragma unroll 1
         for (int c0 = b + 1; c0 <= b_last && GB > 1; c0 += GB) {
@@ -291,11 +295,10 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
               for (int h = 0; h < 2; ++h)
 #pragma unroll
                 for (int cc = 0; cc < 2; ++cc) {
-                  const int col = 8 * q + 2 * t + cc, j = 4 * q + 2 * h + cc;
-                  if (m0 + col < p.M) {
-                    if (p.epi == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o[gi][j]);
-                    else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o[gi][j]));
-                  }
+                  // tokens past M add the 0 loaded for them and are never written
+                  const int j = 4 * q + 2 * h + cc;
+                  if constexpr (Fmt::EPI == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o[gi][j]);
+                  else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o[gi][j]));
                 }
           }
         }
@@ -307,10 +310,10 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         if (n >= p.N_out) continue;
         const float bias = p.bias ? __bfloat162float(p.bias[n]) : 0.f;
         float osc = 1.f, sw = 1.f;
-        if (p.epi == EPI_FLOAT) {
+        if constexpr (Fmt::EPI == EPI_FLOAT) {
           osc = (p.out_scale ? (p.out_scale_per_row ? p.out_scale[n] : *p.out_scale) : 1.f);
           if (p.out_scale2) osc *= *p.out_scale2;
-          osc *= __int_as_float((127 + p.acc_exp2) << 23);
+          osc *= __int_as_float((127 + Fmt::ACC_EXP2) << 23);
         } else {
           sw = p.w_scale ? p.w_scale[n] : 1.f;
         }
@@ -322,11 +325,11 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
             if (m >= p.M) continue;
             const uint32_t raw = v[4 * q + 2 * h + c];
             __nv_bfloat16* dst = p.y ? p.y + (size_t)m * p.N_out + n : nullptr;
-            if (p.epi == EPI_FLOAT) {
+            if constexpr (Fmt::EPI == EPI_FLOAT) {
               float x = __uint_as_float(raw);
               if (p.row_scale) x *= p.row_scale[m];
               *dst = __float2bfloat16_rn(x * osc + bias);
-            } else if (p.epi == EPI_I8) {
+            } else if constexpr (Fmt::EPI == EPI_I8) {
               if (p.i32_out) {
                 p.i32_out[(size_t)m * p.N_out + n] = (int32_t)raw;
               } else {
@@ -429,18 +432,28 @@ done:
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-// Grid choice + workspace carve-up shared by the launchers of this kernel.
+// Activation tensor map, grid choice, workspace carve-up and launch at one token-tile width.
 //   * at most one CTA of the grid per SM: the grid stays within the resident capacity, which the owner protocol needs
 //     for forward progress (streamk.cuh), and a decode SM keeps room for the next kernel's CTA
 //   * never fewer than `min_units` chunks per CTA: splitting a tile over more CTAs shortens the streaming phase but
 //     lengthens the owner's gather
 template <class Fmt, int N_MMA>
-inline int launch_gemm(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const CUtensorMap& tm_x,
+inline int launch_gemm(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const void* x, int ldx,
                        void* ws, size_t ws_bytes, const char* what, cudaStream_t stream) {
   using C = Cfg<Fmt, N_MMA>;
+  CUtensorMap tm_x;   // box: 128 bytes of k (one swizzle atom) x N_MMA tokens
+  {
+    const uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.M};
+    const uint64_t str[1] = {(uint64_t)ldx * Fmt::X_ELEM_BYTES};
+    const uint32_t box[2] = {128 / Fmt::X_ELEM_BYTES, N_MMA};
+    int rc = make_tmap(&tm_x, Fmt::X_ELEM_BYTES == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8,
+                       2, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+  }
+  p.m_blocks = ceil_div(p.M, N_MMA);
   const long long units = (long long)p.n_tiles * p.m_blocks * p.KT;
   int grid = sm_count();
-  const int min_units = ts_min_units() ? ts_min_units() : 4;
+  constexpr int min_units = 4;
   if (units / min_units < grid) grid = units / min_units > 0 ? (int)(units / min_units) : 1;
   if (const int forced = streamk_ctas_override()) {
     // tests only: at most one CTA per SM (forward progress, see above) and never a CTA without units (its epilogue
@@ -457,6 +470,21 @@ inline int launch_gemm(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm
   AO_CUDA_CHECK(ensure_dynamic_smem(reinterpret_cast<const void*>(kern), C::SMEM_BYTES));
   AO_CUDA_CHECK(launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, pdl_enabled(), tm_w, tm_aux, tm_x, p));
   return AO_OK;
+}
+
+// Y = X * W^T for every format: the caller sets M, N, N_out, K and its format's Params fields and builds the weight
+// and aux maps (Fmt::make_maps); x is [M][ldx] activations of Fmt::X_ELEM_BYTES each.  The token count picks the
+// token tile; more than Fmt::MAX_N_MMA tokens run as several blocks of that width.
+template <class Fmt>
+inline int run(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const void* x, int ldx, void* ws,
+               size_t ws_bytes, const char* what, cudaStream_t stream) {
+  static_assert(Fmt::MAX_N_MMA == 64 || Fmt::MAX_N_MMA == 128, "token tile");
+  p.n_tiles = ceil_div(p.N_out, ROWS);
+  p.KT = ceil_div(p.K, KCHUNK);   // a K tail is zero-filled by TMA (out-of-bounds box elements) on both operands
+  if (p.M <= 16) return launch_gemm<Fmt, 16>(p, tm_w, tm_aux, x, ldx, ws, ws_bytes, what, stream);
+  if (p.M <= 32) return launch_gemm<Fmt, 32>(p, tm_w, tm_aux, x, ldx, ws, ws_bytes, what, stream);
+  if (p.M <= 64) return launch_gemm<Fmt, 64>(p, tm_w, tm_aux, x, ldx, ws, ws_bytes, what, stream);
+  return launch_gemm<Fmt, Fmt::MAX_N_MMA>(p, tm_w, tm_aux, x, ldx, ws, ws_bytes, what, stream);
 }
 
 }  // namespace tsg
