@@ -70,6 +70,11 @@ struct SsFmt {
                                                  uint64_t policy) {
     tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
   }
+  // grouped kernels: 128 rows from `row` of the [E * N, K] map of all experts' weights
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, uint8_t* w_dst, uint64_t* bar, int row,
+                                                      int kc, uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, row, policy);
+  }
   template <int N_MMA>
   __device__ static __forceinline__ void mma(uint32_t (&acc)[N_MMA / 2], uint32_t w_s, uint32_t x_s, int wg,
                                              uint32_t scale_d) {
@@ -288,6 +293,34 @@ extern "C" int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, in
   AO_REQUIRE(xq && x_scale && wq && w_scale && y, "fp8 linear: null pointer");
   return lowp::rowwise<lowp::KIND_F8>(xq, x_scale, M, K, wq, w_scale, N, bias, y, nullptr, workspace, workspace_bytes,
                                       stream);
+}
+
+// torch._grouped_mm(x, W.transpose(-2, -1), offs) on rowwise e4m3 operands: expert e's rows [offs[e-1], offs[e]) of
+// xq against its weights wq[e] (the stored [E, N, K] qdata), the dense kernel's epilogue with w_scale[e, :].  offs
+// stays on the device (grouped schedule, ts_gemm.cuh).
+extern "C" int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale, int M, int K,
+                                         const uint8_t* wq, const float* w_scale, int E, int N,
+                                         const int32_t* offs, uint16_t* y, void* workspace,
+                                         size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "fp8 grouped mm: E=%d experts must be in [1, %d]", E, tsg::MAX_EXPERTS);
+  AO_REQUIRE(K % 16 == 0, "fp8 grouped mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
+  AO_REQUIRE(N % 16 == 0, "fp8 grouped mm: N=%d must be a multiple of 16", N);
+  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "fp8 grouped mm: E*N=%lld weight rows exceed the int32 range", (long long)E * N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(xq && x_scale && wq && w_scale && offs && y && workspace, "fp8 grouped mm: null pointer");
+  using Fmt = tsg::Grouped<lowp::SsFmt<lowp::KIND_F8>>;
+  CUtensorMap tm_w, tm_aux;
+  if (int rc = Fmt::make_maps(wq, E * N, K, &tm_w, &tm_aux)) return rc;
+  tsg::Params p{};
+  p.row_scale = x_scale;
+  p.w_scale = w_scale;
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.offs = offs;
+  p.E = E;
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<Fmt>(p, tm_w, tm_aux, xq, K, workspace, workspace_bytes, "fp8 grouped mm",
+                             reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,

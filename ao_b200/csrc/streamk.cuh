@@ -32,6 +32,15 @@
 //     grid j has completed; before that it only streams weights into its own shared memory, and j never waits on it;
 //   * CTAs of j+1 that did not find room become resident as CTAs of j exit, which they do without waiting on j+1.
 //
+// Device-side grid (grouped GEMM, ts_gemm.cuh Grouped<Fmt>).  The units per expert come from offs, which only the
+// device reads, so the host launches a grid sized for an upper bound of U.  With more CTAs than units, unit_begin
+// gives some CTA an empty range: an owner would then wait for a flag that CTA never raises, and that CTA's epilogue
+// would run on an accumulator no wgmma wrote.  So every CTA first derives U from offs and the effective grid the host
+// would have picked for it, G_eff = min(G, max(1, U / MIN_UNITS)) (forced grids: min(G, U); U = 0: no CTA).  CTAs
+// b >= G_eff leave at once, before they touch the workspace; the split uses G_eff, and G_eff <= U gives every
+// remaining CTA at least one unit.  All CTAs compute the same G_eff, so owners and contributors agree on the split.
+// The forward-progress argument above holds unchanged for the CTAs below G_eff.
+//
 // tests/streamk_model.py restates unit_begin, cta_of_unit and Walk on the CPU (and GB, the owner's gather group of
 // ts_gemm.cuh); a change here needs the same change there.
 #pragma once

@@ -50,8 +50,14 @@ struct Params {
   const __nv_bfloat16* bias;
   const float* row_scale;   // EPI_FLOAT: optional per-token scale [M]; EPI_I8 / EPI_F8: the activation scale [M]
   const float* out_scale;   // EPI_FLOAT: optional device scalar, or (out_scale_per_row) one value per output feature
-  const float* out_scale2;  // EPI_FLOAT: optional second device scalar multiplied into out_scale (nvfp4 a_pts * b_pts)
+  // The grouped fields share storage and padding with the dense ones, so Params keeps its 120 bytes: a larger
+  // parameter block changed the code ptxas generates for every dense instantiation.
+  union {
+    const float* out_scale2;  // EPI_FLOAT: optional second device scalar multiplied into out_scale (nvfp4 a_pts * b_pts)
+    const int* offs;          // Grouped<Fmt> (EPI_F8 only): [E] on the device, see below
+  };
   int out_scale_per_row;
+  int grid_forced;          // Grouped<Fmt>: the host grid was forced (ao_b200_debug_set_streamk_ctas): no MIN_UNITS rule
   const float* w_scale;     // EPI_I8 / EPI_F8: per-output-feature weight scale [N]
   __nv_bfloat16* y;         // [M, N_out]
   int32_t* i32_out;         // EPI_I8: raw int32 accumulators [M, N] instead of y
@@ -60,7 +66,90 @@ struct Params {
   int M, N, N_out, K, group_size;
   int n_tiles, m_blocks, KT;   // KT = chunks of 128 k
   int aux_col_blocks;          // blocked block-scale layouts: 4-scale column blocks per 128-row block
+  // Grouped<Fmt> (see Grouped schedule below): expert e < E owns rows [offs[e-1], offs[e]) of x and y (offs[-1] = 0), its
+  // weights are rows e*N .. e*N+N-1 of the weight map and its weight scales w_scale[e*N ..]
+  int E;
 };
+static_assert(sizeof(Params) == 120, "Params layout (see above)");
+
+// Grouped schedule (torch._grouped_mm, 2-D x 3-D).  The m-blocks are per expert: ceil(rows_e / N_MMA) blocks of
+// N_MMA tokens starting at the expert's first row, so a tile never mixes two experts' weights.  Only the device knows
+// offs, so every CTA derives the split from it after griddepcontrol.wait: the tile index stays j * n_tiles + n_tile,
+// with j enumerating the (expert, m-block) pairs, U = n_tiles * J * KT and the grid the host heuristic would have
+// picked for that U (streamk.cuh, "Device-side grid").
+constexpr int MAX_EXPERTS = 1024;   // one row end and one m-block prefix per expert in shared memory
+constexpr int MIN_UNITS = 4;        // never fewer chunks per CTA (launch_gemm)
+
+// ts_gemm_kernel<Grouped<Fmt>, N_MMA>: Fmt (a shared-memory A policy) under the grouped schedule.  A wrapper rather
+// than a kernel template parameter, so the dense kernels keep their names and their code.
+template <class F>
+struct Grouped : F {};
+template <class F>
+struct IsGrouped {
+  static constexpr bool value = false;
+};
+template <class F>
+struct IsGrouped<Grouped<F>> {
+  static constexpr bool value = true;
+};
+
+struct GroupTile {
+  int e, row0, row_end;   // the expert, the tile's first row and the expert's end row (rows >= row_end: not stored)
+};
+
+// One warp: end[e] = min(M, max(0, offs[0..e])) (each offs[e] clamped into [end[e-1], M]: a malformed offs never
+// reaches a row outside [0, M)) and mbp[e] = the m-blocks of experts 0 .. e-1, mbp[E] = J
+template <int N_MMA>
+__device__ __forceinline__ void grouped_schedule(const Params& p, int* end, int* mbp, int lane) {
+  int run_end = 0, run_mb = 0;
+  for (int base = 0; base < p.E; base += 32) {
+    const int e = base + lane;
+    int r = e < p.E ? p.offs[e] : 0;
+    r = r > run_end ? r : run_end;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int o = __shfl_up_sync(0xffffffffu, r, d);
+      if (lane >= d && o > r) r = o;
+    }
+    if (r > p.M) r = p.M;
+    int start = __shfl_up_sync(0xffffffffu, r, 1);
+    if (lane == 0) start = run_end;
+    const int mb = e < p.E ? (r - start + N_MMA - 1) / N_MMA : 0;
+    int s = mb;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int o = __shfl_up_sync(0xffffffffu, s, d);
+      if (lane >= d) s += o;
+    }
+    if (e < p.E) {
+      end[e] = r;
+      mbp[e + 1] = run_mb + s;
+    }
+    run_end = __shfl_sync(0xffffffffu, r, 31);
+    run_mb += __shfl_sync(0xffffffffu, s, 31);
+  }
+  if (lane == 0) mbp[0] = 0;
+}
+
+// The (expert, m-block) pair j < J: the largest e with mbp[e] <= j (an empty expert shares its prefix with the next)
+template <int N_MMA>
+__device__ __forceinline__ GroupTile group_tile(const int* end, const int* mbp, int E, int j) {
+  int lo = 0, hi = E - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (mbp[mid] <= j) lo = mid;
+    else hi = mid - 1;
+  }
+  return {lo, (lo > 0 ? end[lo - 1] : 0) + (j - mbp[lo]) * N_MMA, end[lo]};
+}
+
+// The grid of a grouped launch once U is known: what launch_gemm picks for U units, never above the launched grid
+// (sized from an upper bound of U), never a CTA without units, no CTA at all when every expert is empty
+__device__ __forceinline__ int grouped_grid(int G, long long U, int forced) {
+  if (U == 0) return 0;
+  const long long cap = forced ? U : (U / MIN_UNITS > 0 ? U / MIN_UNITS : 1);
+  return cap < G ? (int)cap : G;
+}
 
 template <class Fmt, int N_MMA>
 struct Cfg {
@@ -110,12 +199,16 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 //   static void issue_w(tm_w, tm_aux, p, w smem dst, aux smem dst, full barrier, n_tile, kc, policy)  (one thread)
 //   static uint32_t w_tx_bytes(p)
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
+//        static void issue_w_rows(tm_w, w smem dst, full barrier, row, kc, policy)   grouped: from weight row `row`
 //   RA:  struct Raw; static void load(p, w smem, aux smem, row_lo, lane, Raw&)   rows row_lo and row_lo + 8
 //        static void frag(p, raw, kk, a[4])                        bf16 A fragment of k16 step kk (0..7)
+// Grouped<Fmt>: the grouped schedule above (shared-memory A formats only); the dense kernels compile without any of it.
 template <class Fmt, int N_MMA>
 __global__ void __launch_bounds__(NUM_THREADS, ctas_per_sm<Fmt, N_MMA>())
 ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_aux,
                const __grid_constant__ CUtensorMap tm_x, const Params p) {
+  constexpr bool GROUPED = IsGrouped<Fmt>::value;
+  static_assert(!GROUPED || Fmt::SS, "grouped schedule: shared-memory A formats only");
   using C = Cfg<Fmt, N_MMA>;
   using MMA = Wgmma<N_MMA>;
   constexpr int S = C::STAGES;
@@ -131,8 +224,26 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   // warp-uniform and warpgroup-uniform (wgmma in code it must treat as divergent is serialised)
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const int wgi = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
-  const int G = gridDim.x, b = blockIdx.x;
-  const long long U = (long long)p.n_tiles * p.m_blocks * p.KT;
+  const int b = blockIdx.x;
+  int G = gridDim.x;
+  long long U;
+  const int* g_end = nullptr;   // grouped: the schedule table in shared memory
+  const int* g_mbp = nullptr;
+  if constexpr (GROUPED) {
+    // which weights a unit needs depends on offs, the previous kernel's output: no weight request before the wait
+    __shared__ int s_end[MAX_EXPERTS], s_mbp[MAX_EXPERTS + 1];
+    pdl_launch_dependents();
+    pdl_wait();
+    if (warp == 0) grouped_schedule<N_MMA>(p, s_end, s_mbp, lane);
+    __syncthreads();
+    g_end = s_end;
+    g_mbp = s_mbp;
+    U = (long long)p.n_tiles * s_mbp[p.E] * p.KT;
+    G = grouped_grid(G, U, p.grid_forced);
+    if (b >= G) return;   // a CTA past the device-side grid has no units and owns no flag
+  } else {
+    U = (long long)p.n_tiles * p.m_blocks * p.KT;
+  }
   const int u0 = streamk::unit_begin(b, U, G), u1 = streamk::unit_begin(b + 1, U, G);
   const int nunits = u1 - u0;
   const streamk::Walk walk(u0, nunits, p.KT);
@@ -154,7 +265,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
     tma_prefetch_desc(&tm_x);
   }
   __syncthreads();
-  pdl_launch_dependents();
+  if constexpr (!GROUPED) pdl_launch_dependents();
 
   const int seg_last = walk.nseg - 1;
   const bool last_is_owner = walk.seg_kind(seg_last) == streamk::SEG_OWNER;
@@ -169,12 +280,22 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       const int s = i % S;
       uint8_t* st = stage(s);
       mbar_expect_tx(&wfull[s], Fmt::w_tx_bytes(p));
-      Fmt::issue_w(&tm_w, &tm_aux, p, st, st + Fmt::W_BYTES, &wfull[s], tile_of(i) % p.n_tiles, kc_of(i), pol_w);
+      if constexpr (GROUPED) {
+        // expert e's feature n is weight row e * N + n; a tile tail past N reads the next expert's rows (or the
+        // map's zero fill), whose outputs the epilogue skips (n >= N_out)
+        const int tile = tile_of(i), n_tile = tile % p.n_tiles;
+        const int e = group_tile<N_MMA>(g_end, g_mbp, p.E, tile / p.n_tiles).e;
+        Fmt::issue_w_rows(&tm_w, st, &wfull[s], e * p.N + n_tile * ROWS, kc_of(i), pol_w);
+      } else {
+        Fmt::issue_w(&tm_w, &tm_aux, p, st, st + Fmt::W_BYTES, &wfull[s], tile_of(i) % p.n_tiles, kc_of(i), pol_w);
+      }
     };
     auto issue_x = [&](int i) {
       const int s = i % S;
       uint8_t* xs = stage(s) + Fmt::W_BYTES + C::AUX_SLOT;
-      const int m0 = (tile_of(i) / p.n_tiles) * N_MMA;
+      int m0 = (tile_of(i) / p.n_tiles) * N_MMA;
+      // grouped: from the expert's rows on (rows of the next expert in the box are loaded but never stored)
+      if constexpr (GROUPED) m0 = group_tile<N_MMA>(g_end, g_mbp, p.E, tile_of(i) / p.n_tiles).row0;
       mbar_expect_tx(&xfull[s], C::X_BYTES);
 #pragma unroll
       for (int a = 0; a < C::X_ATOMS; ++a)
@@ -221,7 +342,14 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       const int tile = walk.seg_tile(seg);
       const int kind = walk.seg_kind(seg);
       const int n_tile = tile % p.n_tiles, m_blk = tile / p.n_tiles;
-      const int m0 = m_blk * N_MMA;
+      int m0 = m_blk * N_MMA, m_end = p.M;   // tokens m0 .. min(m0 + N_MMA, m_end) - 1 are this tile's
+      const float* w_scale = p.w_scale;
+      if constexpr (GROUPED) {
+        const GroupTile gt = group_tile<N_MMA>(g_end, g_mbp, p.E, m_blk);
+        m0 = gt.row0;
+        m_end = gt.row_end;
+        w_scale += (size_t)gt.e * p.N;
+      }
       if (kind == streamk::SEG_CONTRIB) {
         // publish the partial (column-major slot: word (token j, row r) at j * 128 + r), then one gpu-scope release
         uint32_t* slot = reinterpret_cast<uint32_t*>(p.ws_partial) + (size_t)b * (N_MMA * ROWS);
@@ -232,7 +360,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
 #pragma unroll
             for (int c = 0; c < 2; ++c) {
               const int col = 8 * q + 2 * t + c, r = row_lo + 8 * h;
-              if (m0 + col < p.M) __stcg(&slot[col * ROWS + r], v[4 * q + 2 * h + c]);
+              if (m0 + col < m_end) __stcg(&slot[col * ROWS + r], v[4 * q + 2 * h + c]);
             }
         asm volatile("bar.sync 1, 256;" ::: "memory");   // all 128 rows stored (cta-scope order) ...
         if (warp == 4 && lane == 0) streamk::st_release_u32(p.ws_flag + b, 1u);   // ... then one gpu-scope release
@@ -255,13 +383,13 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           for (int q = 0; q < NACC / 4; ++q) {
             // a warp-uniform exit every 16 tokens (the rest of the tile is past M).  The branch also bounds the loads the
             // compiler hoists above their adds to 8 words; hoisting all NACC of them spills at N_MMA = 128
-            if (q % 2 == 0 && m0 + 8 * q >= p.M) break;
+            if (q % 2 == 0 && m0 + 8 * q >= m_end) break;
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
               for (int cc = 0; cc < 2; ++cc) {
                 const int col = 8 * q + 2 * t + cc, r = row_lo + 8 * h, j = 4 * q + 2 * h + cc;
-                if (m0 + col < p.M) {
+                if (m0 + col < m_end) {
                   const uint32_t o = __ldcg(slot + col * ROWS + r);
                   if constexpr (Fmt::EPI == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o);
                   else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o));
@@ -283,7 +411,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
 #pragma unroll
                 for (int cc = 0; cc < 2; ++cc) {
                   const int col = 8 * q + 2 * t + cc, r = row_lo + 8 * h, j = 4 * q + 2 * h + cc;
-                  o[gi][j] = m0 + col < p.M ? __ldcg(slot + col * ROWS + r) : 0u;
+                  o[gi][j] = m0 + col < m_end ? __ldcg(slot + col * ROWS + r) : 0u;
                 }
           }
 #pragma unroll
@@ -315,14 +443,14 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           if (p.out_scale2) osc *= *p.out_scale2;
           osc *= __int_as_float((127 + Fmt::ACC_EXP2) << 23);
         } else {
-          sw = p.w_scale ? p.w_scale[n] : 1.f;
+          sw = w_scale ? w_scale[n] : 1.f;
         }
 #pragma unroll
         for (int q = 0; q < NACC / 4; ++q)
 #pragma unroll
           for (int c = 0; c < 2; ++c) {
             const int m = m0 + 8 * q + 2 * t + c;
-            if (m >= p.M) continue;
+            if (m >= m_end) continue;
             const uint32_t raw = v[4 * q + 2 * h + c];
             __nv_bfloat16* dst = p.y ? p.y + (size_t)m * p.N_out + n : nullptr;
             if constexpr (Fmt::EPI == EPI_FLOAT) {
@@ -435,8 +563,10 @@ done:
 // Activation tensor map, grid choice, workspace carve-up and launch at one token-tile width.
 //   * at most one CTA of the grid per SM: the grid stays within the resident capacity, which the owner protocol needs
 //     for forward progress (streamk.cuh), and a decode SM keeps room for the next kernel's CTA
-//   * never fewer than `min_units` chunks per CTA: splitting a tile over more CTAs shortens the streaming phase but
+//   * never fewer than MIN_UNITS chunks per CTA: splitting a tile over more CTAs shortens the streaming phase but
 //     lengthens the owner's gather
+//   * Grouped<Fmt>: the grid and the partial slots are sized for an upper bound of the units (each expert adds at most
+//     one partial m-block); the kernel cuts the grid to the same rule for the units offs gives (grouped_grid)
 template <class Fmt, int N_MMA>
 inline int launch_gemm(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const void* x, int ldx,
                        void* ws, size_t ws_bytes, const char* what, cudaStream_t stream) {
@@ -451,11 +581,13 @@ inline int launch_gemm(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm
     if (rc) return rc;
   }
   p.m_blocks = ceil_div(p.M, N_MMA);
+  if constexpr (IsGrouped<Fmt>::value) p.m_blocks += p.E < p.M ? p.E : p.M;   // >= sum over experts of ceil(rows_e / N_MMA)
   const long long units = (long long)p.n_tiles * p.m_blocks * p.KT;
   int grid = sm_count();
-  constexpr int min_units = 4;
-  if (units / min_units < grid) grid = units / min_units > 0 ? (int)(units / min_units) : 1;
-  if (const int forced = streamk_ctas_override()) {
+  if (units / MIN_UNITS < grid) grid = units / MIN_UNITS > 0 ? (int)(units / MIN_UNITS) : 1;
+  const int forced = streamk_ctas_override();
+  p.grid_forced = forced != 0;
+  if (forced) {
     // tests only: at most one CTA per SM (forward progress, see above) and never a CTA without units (its epilogue
     // would run on an accumulator no wgmma wrote)
     const int cap = units < sm_count() ? (int)units : sm_count();
@@ -475,6 +607,8 @@ inline int launch_gemm(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm
 // Y = X * W^T for every format: the caller sets M, N, N_out, K and its format's Params fields and builds the weight
 // and aux maps (Fmt::make_maps); x is [M][ldx] activations of Fmt::X_ELEM_BYTES each.  The token count picks the
 // token tile; more than Fmt::MAX_N_MMA tokens run as several blocks of that width.
+// Grouped<Fmt> (Params::offs, E): an expert never holds more than M rows, so the width chosen from M streams each
+// active expert's weights once for M <= 64.
 template <class Fmt>
 inline int run(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, const void* x, int ldx, void* ws,
                size_t ws_bytes, const char* what, cudaStream_t stream) {

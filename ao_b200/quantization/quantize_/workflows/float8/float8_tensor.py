@@ -12,6 +12,7 @@ from dataclasses import dataclass
 from typing import List, Optional
 
 import torch
+from torch.utils._python_dispatch import return_and_correct_aliasing
 
 from ao_b200.float8.inference import FP8Granularity, Float8MMConfig, _is_rowwise_scaled, _is_tensorwise_scaled
 from ao_b200.quantization.granularity import PerRow, PerTensor
@@ -144,6 +145,50 @@ def _(func, types, args, kwargs):
     if bs[dim] > qd.shape[dim]:
         bs[dim] = qd.shape[dim]
     return Float8Tensor(qd, sc, bs, self.mm_config, self.act_quant_kwargs, self.kernel_preference, self.dtype)
+
+
+@implements(aten.transpose.int)
+def _(func, types, args, kwargs):
+    """A view with qdata, scale and block_size swapped (float8_tensor.py:842-860): how a 3-D expert weight [E, N, K]
+    reaches torch._grouped_mm as mat_b [E, K, N]."""
+    self, dim0, dim1 = args
+    bs = list(self.block_size)
+    bs[dim0], bs[dim1] = bs[dim1], bs[dim0]
+    new = Float8Tensor(self.qdata.transpose(dim0, dim1), self.scale.transpose(dim0, dim1), bs, self.mm_config,
+                       self.act_quant_kwargs, self.kernel_preference, self.dtype)
+    return return_and_correct_aliasing(func, args, kwargs, new)
+
+
+@implements(aten._grouped_mm.default)
+def _(func, types, args, kwargs):
+    """torch._grouped_mm(x, W.transpose(-2, -1), offs=offs) with a rowwise Float8Tensor expert weight W [E, N, K]
+    (the reference's handler, float8_tensor.py:1085-1122): the routed tokens are quantized per row and the grouped
+    GEMM runs on the stored qdata with w_scale[e, n].  Only the 2-D x 3-D form with PerRow activations."""
+    mat_a, mat_b = args[0], args[1]
+    offs = args[2] if len(args) > 2 else kwargs.get("offs", None)
+    assert isinstance(mat_b, Float8Tensor)
+    assert offs is not None, "offs is required for _grouped_mm"
+    assert mat_b.qdata.stride(-2) < mat_b.qdata.stride(-1), "mat_b must be the transposed [E, N, K] weight"
+    act_quant_kwargs = mat_b.act_quant_kwargs
+    if act_quant_kwargs is None:
+        raise NotImplementedError("Float8 weight-only _grouped_mm is outside this engine's scope; use "
+                                  "Float8DynamicActivationFloat8WeightConfig")
+    if not isinstance(act_quant_kwargs.granularity, PerRow):
+        raise NotImplementedError(f"_grouped_mm only supports PerRow granularity, got {act_quant_kwargs.granularity}")
+    if mat_a.dim() != 2 or mat_b.dim() != 3:
+        raise NotImplementedError(f"_grouped_mm: only 2-D mat_a x 3-D mat_b, got {mat_a.dim()}-D x {mat_b.dim()}-D")
+    bias = args[3] if len(args) > 3 else kwargs.get("bias", None)
+    assert bias is None, "_grouped_mm with bias is not supported"
+    E, K, N = mat_b.shape
+    assert mat_a.shape[-1] == K, f"_grouped_mm: mat_a has K={mat_a.shape[-1]}, mat_b K={K}"
+    xq_t = Float8Tensor.from_hp(mat_a, act_quant_kwargs.float8_dtype, act_quant_kwargs.granularity,
+                                act_quant_kwargs.mm_config, act_quant_kwargs.hp_value_lb, act_quant_kwargs.hp_value_ub,
+                                act_quant_kwargs.kernel_preference)
+    wq = mat_b.qdata.transpose(-2, -1)   # back to the stored [E, N, K]
+    y = torch.ops.ao_b200.fp8_rowwise_grouped_mm(xq_t.qdata.contiguous(), xq_t.scale.reshape(-1).float().contiguous(),
+                                                 wq.contiguous(), mat_b.scale.reshape(E, N).float().contiguous(),
+                                                 offs.to(torch.int32))
+    return y.to(mat_a.dtype)
 
 
 Float8Tensor.__module__ = "ao_b200.quantization"

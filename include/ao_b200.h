@@ -128,6 +128,18 @@ int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, int M, int K,
                           const uint8_t* wq, const float* w_scale, int N,
                           const uint16_t* bias, uint16_t* y, void* workspace,
                           size_t workspace_bytes, void* stream);
+/* Replaces torchao's aten._grouped_mm handler for a rowwise Float8Tensor expert weight, i.e.
+ * torch._scaled_grouped_mm / F.scaled_grouped_mm rowwise (float8_tensor.py:1085-1122), 2-D x 3-D form:
+ * for offs[e-1] <= m < offs[e] (offs[-1] = 0):
+ *   y[m, :] = bf16( (Xq[m] Wq[e]^T) * x_scale[m] * w_scale[e, :] ), f32 accumulate.
+ * xq e4m3 [M,K] (tokens sorted by expert); wq e4m3 [E][N][K] (K-major, the stored qdata); x_scale f32 [M];
+ * w_scale f32 [E][N]; offs int32 [E] on the device, cumulative row ends.  The host never reads offs (no sync,
+ * CUDA-graph capturable); the kernel clamps each offs[e] into [offs[e-1], M].  Rows from offs[E-1] on are not
+ * written.  1 <= E <= 1024, K % 16 == 0, N % 16 == 0, no bias.                                             */
+int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale, int M, int K,
+                              const uint8_t* wq, const float* w_scale, int E, int N,
+                              const int32_t* offs, uint16_t* y, void* workspace,
+                              size_t workspace_bytes, void* stream);
 
 /* mxfp8 (e4m3 data, e8m0 block-32 scales) --------------------------------------- */
 /* Replaces MXTensor.to_mx(x, e4m3, 32, RCEIL, is_swizzled_scales) for activations
