@@ -185,8 +185,9 @@ int ao_nvfp4_weight_linear_ex(const uint16_t* x, int ldx, const float* x_scale, 
                               int b_pts_per_row, int N, const uint16_t* bias, uint16_t* y,
                               void* workspace, size_t workspace_bytes, void* stream);
 /* Per-token e4m3 quantisation that keeps the codes as bf16 values (exact): xq = bf16(e4m3(x/s)),
- * s = f32(bf16(amax/448)) -- the values Float8Tensor.from_hp(x, PerRow()) stores
- * (quant_primitives.py:2172-2287), in the operand type the bf16 MMA consumes. */
+ * s = f32(bf16(amax/448)) -- the codes of ao_fp8_quantize_rowwise, i.e. the values Float8Tensor.from_hp(x, PerRow())
+ * stores (quant_primitives.py:2172-2287), in the operand type the bf16 MMA consumes.  An all-zero row (s = 0) gives
+ * zeros where the e4m3 codes are NaN (0/0). */
 int ao_fp8_fakequant_rowwise(const uint16_t* x, int M, int K, uint16_t* xq_bf16, float* scale,
                              void* stream);
 
@@ -206,7 +207,7 @@ int ao_fp8_fakequant_rowwise_ld(const uint16_t* x, int ldx, int M, int K, uint16
 /* Producer-fused per-token quantizers (SURVEY section 8f-1: "fused with the preceding RMSNorm / SiLU where possible").
  * They replace, for a dynamic-activation linear that follows an RMSNorm or a SiLU-gated product, the norm / activation
  * kernel(s) + Int8Tensor.from_hp(x, PerRow()) / Float8Tensor.from_hp(x, PerRow()) (int8_tensor.py:176-248,
- * float8_tensor.py:235-242) by one kernel; the quantization arithmetic is that of ao_int8/fp8_quantize_rowwise on the
+ * float8_tensor.py:235-242) by one kernel; the scales and codes are those ao_int8/fp8_quantize_rowwise give for the
  * bf16 values the producer would have written (HF LlamaRMSNorm / LlamaMLP rounding points).  fmt: 0 int8, 1 e4m3.     */
 int ao_rmsnorm_quantize_rowwise(const uint16_t* x, int ldx, const uint16_t* weight, float eps, int M, int K,
                                 int fmt, uint8_t* q, float* scale, void* stream);

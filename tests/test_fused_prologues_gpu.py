@@ -27,6 +27,10 @@ def test_silu_mul_quant_bit_exact(fmt, M, K):
     gen = torch.Generator(device="cuda").manual_seed(M + K)
     gu = (torch.randn(M, 2 * K, device="cuda", generator=gen) * 2).to(torch.bfloat16)
     gate, up = gu[:, :K], gu[:, K:]          # column slices of one fused gate|up output: row pitch 2K
+    if M > 1:                                # -0.0, NaN and inf in y, each in a row of its own; the others stay finite
+        up[0, 1::7] = -0.0
+        up[M // 2, 5] = float("nan")
+        up[M - 1, 9] = float("inf")
     y = torch.nn.functional.silu(gate) * up
     q_ref, s_ref = (ops.int8_quantize_rowwise if fmt == 0 else ops.fp8_quantize_rowwise)(y)
     q, s = ops.silu_mul_quantize_rowwise(gate, up, fmt)

@@ -69,7 +69,7 @@ def test_activation_quantizers_bit_exact(ops, M, K):
 def test_rowwise_quantizers_large_sample_vs_torch(ops, M, K):
     """Millions of quotients per case against the reference arithmetic written with torch ops on the GPU (true IEEE
     division, quant_primitives.py:2172-2287 / :1487-1583): the e4m3 kernel forms x / s as x * (1 / s) plus one FMA residual
-    correction, which must round exactly like the division; K = 32768 takes the two-pass kernel."""
+    correction, which must round exactly like the division; K = 32768 and fakequant take the one-CTA kernel."""
     g = torch.Generator(device="cuda").manual_seed(M + K)
     x = (torch.randn(M, K, device="cuda", generator=g) * torch.logspace(-3, 3, M, device="cuda").unsqueeze(1)).to(torch.bfloat16)
     q, s = ops.fp8_quantize_rowwise(x)
@@ -78,11 +78,46 @@ def test_rowwise_quantizers_large_sample_vs_torch(ops, M, K):
     ref = (x.float() / sc).clamp(-448.0, 448.0).to(torch.float8_e4m3fn)
     assert torch.equal(s.reshape(-1), sc.reshape(-1))
     assert torch.equal(q.view(torch.uint8), ref.view(torch.uint8))
+    qf, sf = ops.fp8_fakequant_rowwise(x)    # one CTA per row at every K, same reciprocal form
+    assert torch.equal(sf.reshape(-1), sc.reshape(-1))
+    assert torch.equal(qf, ref.to(torch.bfloat16))
     q8, s8 = ops.int8_quantize_rowwise(x)
     sc8 = torch.clamp((amax / 127.5).float(), min=torch.finfo(torch.float32).eps)
     ref8 = torch.clamp(torch.round(x.float() * (1.0 / sc8)), -128, 127).to(torch.int8)
     assert torch.equal(s8.reshape(-1), sc8.reshape(-1))
     assert torch.equal(q8, ref8)
+
+
+@pytest.mark.parametrize("fmt", ["int8", "fp8"])
+def test_rowwise_paths_agree_on_special_values(ops, fmt):
+    """The register kernel (K <= 16384), the one-CTA kernel (K > 16384) and fakequant share one scale rule and one
+    encoder: the same rows give the same scales and codes on each.  Rows: -0.0 among normals, one NaN, +inf, -inf,
+    bf16 subnormals (both signs) among normals, all zeros."""
+    o = _o()
+    K = 16384
+    g = torch.Generator(device="cuda").manual_seed(3)
+    x = torch.randn(6, K, device="cuda", generator=g).to(torch.bfloat16)
+    x[0, ::7] = -0.0
+    x[1, 5] = float("nan")
+    x[2, 9] = float("inf")
+    x[3, 11] = float("-inf")
+    x[4, ::5] = 2.0 ** -130
+    x[4, 1::5] = -(2.0 ** -133)
+    x[5] = 0
+    quant = ops.int8_quantize_rowwise if fmt == "int8" else ops.fp8_quantize_rowwise
+    q, s = quant(x)
+    qp, sp = quant(torch.nn.functional.pad(x, (0, 8)))   # K = 16392: one CTA per row; the zero columns keep amax
+    assert torch.equal(sp, s)
+    assert torch.equal(qp[:, :K].view(torch.uint8), q.view(torch.uint8))
+    if fmt == "fp8":
+        qf, sf = ops.fp8_fakequant_rowwise(x)
+        assert torch.equal(sf, s)
+        assert torch.equal(qf[:5].float(), q[:5].float())   # row 5: zeros where the e4m3 codes are NaN (0/0)
+    finite = [0, 4, 5]
+    xb = o.bf16_bits(x[finite])
+    qo, so = o.int8_quantize_rowwise(xb) if fmt == "int8" else o.fp8_quantize_rowwise(xb)
+    assert np.array_equal(q.view(torch.uint8)[finite].cpu().numpy(), qo.view(np.uint8))
+    assert np.array_equal(s[finite].cpu().numpy().reshape(-1), so)
 
 
 SHAPES = [(1, 128, 512), (16, 256, 1024), (32, 4096, 4096), (7, 1024, 4096), (32, 14336, 4096), (32, 4096, 14336),
