@@ -71,8 +71,9 @@ struct SsFmt {
     tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
   }
   // grouped kernels: 128 rows from `row` of the [E * N, K] map of all experts' weights
-  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, uint8_t* w_dst, uint64_t* bar, int row,
-                                                      int kc, uint64_t policy) {
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, const CUtensorMap*, const tsg::Params&,
+                                                      uint8_t* w_dst, uint8_t*, uint64_t* bar, int row, int kc,
+                                                      uint64_t policy) {
     tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, row, policy);
   }
   template <int N_MMA>
@@ -383,4 +384,36 @@ extern "C" int ao_nvfp4_weight_linear(const uint16_t* x, const float* x_scale, i
                                       void* stream) {
   return ao_nvfp4_weight_linear_ex(x, K, x_scale, M, K, wq, w_scale_blocked, b_pts, 0, N, bias, y, workspace, workspace_bytes,
                                    stream);
+}
+
+// torch._grouped_mm(x, W.transpose(-2, -1), offs) on NVFP4 expert weights (nvfp4_tensor.py:709-753), 2-D x 3-D:
+// expert e's rows [offs[e-1], offs[e]) of x (bf16; for NVFP4 activations the exactly dequantised codes of
+// ao_nvfp4_fakequant_grouped) against wq[e] (the stored [E, N, K/2] qdata) with its blocked scales, the nvfp4-weight
+// epilogue y = acc * x_scale[m] * w_pts[e].  offs stays on the device (grouped schedule, ts_gemm.cuh).
+extern "C" int ao_nvfp4_grouped_mm(const uint16_t* x, const float* x_scale, int M, int K, const uint8_t* wq,
+                                   const uint8_t* w_scale_blocked, const float* w_pts, int E, int N,
+                                   const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "nvfp4 grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "nvfp4 grouped mm: E=%d experts must be in [1, %d]", E, tsg::MAX_EXPERTS);
+  AO_REQUIRE(K % 128 == 0, "nvfp4 grouped mm: K=%d must be a multiple of 128", K);
+  // every expert's weights and scales start on a 128-row block of the stacked [E * N, ..] tensors
+  AO_REQUIRE(N % 128 == 0, "nvfp4 grouped mm: N=%d must be a multiple of 128", N);
+  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "nvfp4 grouped mm: E*N=%lld weight rows exceed the int32 range", (long long)E * N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && wq && w_scale_blocked && w_pts && offs && y && workspace, "nvfp4 grouped mm: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "nvfp4 grouped mm: x must be 16-byte aligned");
+  using Fmt = tsg::Grouped<nvf4w::Nvfp4Fmt>;
+  CUtensorMap tm_w, tm_sf;
+  if (int rc = Fmt::make_maps(wq, w_scale_blocked, E * N, K, &tm_w, &tm_sf)) return rc;
+  tsg::Params p{};
+  p.row_scale = x_scale;
+  p.out_scale = w_pts;
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.offs = offs;
+  p.E = E;
+  p.aux_col_blocks = ceil_div(K / 16, 4);
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<Fmt>(p, tm_w, tm_sf, x, K, workspace, workspace_bytes, "nvfp4 grouped mm",
+                       reinterpret_cast<cudaStream_t>(stream));
 }

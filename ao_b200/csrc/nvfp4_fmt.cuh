@@ -1,6 +1,7 @@
 // NVFP4 weights (e2m1 pairs, even k in the low nibble; e4m3 block-16 scales in the blocked 128 x 4 tile layout)
 // as the register-A operand of ts_gemm.cuh: each consumer thread turns the bytes of its two fragment rows into the
-// bf16 wgmma A fragment.  Used by the nvfp4-weight linear and by the nvfp4 x nvfp4 linear.
+// bf16 wgmma A fragment.  Used by the nvfp4-weight linear, the nvfp4 x nvfp4 linear and (Grouped<Nvfp4Fmt>) the nvfp4
+// expert GEMM.
 //
 // e2m1 -> bf16 without a table: nibble x = (s e1 e0 m) placed at bf16 bits 15|8:6 is the bf16 number
 // value(x) * 2^-126 (denormal for e = 0, which bf16 multiplies handle exactly); ONE exact multiply by
@@ -56,6 +57,16 @@ struct Nvfp4Fmt {
     // two consecutive blocked scale tiles (128 rows x 4 scales each = 64 k per tile): the blocked scale tensor is a
     // [row block][column block] array of contiguous 512-byte tiles = a 2-D tensor of 128 words x tiles
     tma_load_2d(aux_dst, tm_sf, bar, 0, n_tile * p.aux_col_blocks + kc * 2, policy);
+  }
+  // grouped kernels: the 128 weight rows from `row` of the [E * N, K / 2] map of all experts' weights, and their scale
+  // tiles at row block row / 128 of the blocked [E * N, K / 16] scales.  Expert e's n-tile t is row e * N + 128 t, so
+  // this is row block e * N / 128 + t: the launcher requires N % 128 == 0, which is also what keeps every expert's
+  // scales in whole 128-row blocks of one blocked tensor
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, const CUtensorMap* tm_sf,
+                                                      const tsg::Params& p, uint8_t* w_dst, uint8_t* aux_dst,
+                                                      uint64_t* bar, int row, int kc, uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * 64, row, policy);
+    tma_load_2d(aux_dst, tm_sf, bar, 0, (row / tsg::ROWS) * p.aux_col_blocks + kc * 2, policy);
   }
   // the thread's two fragment rows: bytes 8kk .. 8kk+7 of each (k16 step kk: byte 8kk + t holds k pair 16kk + 2t,
   // byte 8kk + 4 + t the pair 8 further), and the eight block scales of each row, decoded once per chunk: s2[h][j] =

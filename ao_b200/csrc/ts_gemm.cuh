@@ -49,12 +49,13 @@ enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2 };
 struct Params {
   const __nv_bfloat16* bias;
   const float* row_scale;   // EPI_FLOAT: optional per-token scale [M]; EPI_I8 / EPI_F8: the activation scale [M]
-  const float* out_scale;   // EPI_FLOAT: optional device scalar, or (out_scale_per_row) one value per output feature
+  const float* out_scale;   // EPI_FLOAT: optional device scalar, or (out_scale_per_row) one value per output feature;
+                            // Grouped<Fmt>: one value per expert [E] (nvfp4: the per-expert weight scale)
   // The grouped fields share storage and padding with the dense ones, so Params keeps its 120 bytes: a larger
   // parameter block changed the code ptxas generates for every dense instantiation.
   union {
     const float* out_scale2;  // EPI_FLOAT: optional second device scalar multiplied into out_scale (nvfp4 a_pts * b_pts)
-    const int* offs;          // Grouped<Fmt> (EPI_F8 only): [E] on the device, see below
+    const int* offs;          // Grouped<Fmt>: [E] on the device, see below (the grouped epilogue never reads out_scale2)
   };
   int out_scale_per_row;
   int grid_forced;          // Grouped<Fmt>: the host grid was forced (ao_b200_debug_set_streamk_ctas): no MIN_UNITS rule
@@ -80,8 +81,9 @@ static_assert(sizeof(Params) == 120, "Params layout (see above)");
 constexpr int MAX_EXPERTS = 1024;   // one row end and one m-block prefix per expert in shared memory
 constexpr int MIN_UNITS = 4;        // never fewer chunks per CTA (launch_gemm)
 
-// ts_gemm_kernel<Grouped<Fmt>, N_MMA>: Fmt (a shared-memory A policy) under the grouped schedule.  A wrapper rather
-// than a kernel template parameter, so the dense kernels keep their names and their code.
+// ts_gemm_kernel<Grouped<Fmt>, N_MMA>: Fmt under the grouped schedule, for a shared-memory A format (fp8) or a
+// register-A one (nvfp4).  A wrapper rather than a kernel template parameter, so the dense kernels keep their names and
+// their code.
 template <class F>
 struct Grouped : F {};
 template <class F>
@@ -198,17 +200,18 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 //   static int make_maps(...)  host: the weight and aux tensor maps of one GEMM (arguments per format)
 //   static void issue_w(tm_w, tm_aux, p, w smem dst, aux smem dst, full barrier, n_tile, kc, policy)  (one thread)
 //   static uint32_t w_tx_bytes(p)
+//   static void issue_w_rows(tm_w, tm_aux, p, w smem dst, aux smem dst, full barrier, row, kc, policy)
+//                                                                  grouped only: the 128 weight rows from `row` of the
+//                                                                  [E * N, K] map of all experts, and their aux tiles
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
-//        static void issue_w_rows(tm_w, w smem dst, full barrier, row, kc, policy)   grouped: from weight row `row`
 //   RA:  struct Raw; static void load(p, w smem, aux smem, row_lo, lane, Raw&)   rows row_lo and row_lo + 8
 //        static void frag(p, raw, kk, a[4])                        bf16 A fragment of k16 step kk (0..7)
-// Grouped<Fmt>: the grouped schedule above (shared-memory A formats only); the dense kernels compile without any of it.
+// Grouped<Fmt>: the grouped schedule above; the dense kernels compile without any of it.
 template <class Fmt, int N_MMA>
 __global__ void __launch_bounds__(NUM_THREADS, ctas_per_sm<Fmt, N_MMA>())
 ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_aux,
                const __grid_constant__ CUtensorMap tm_x, const Params p) {
   constexpr bool GROUPED = IsGrouped<Fmt>::value;
-  static_assert(!GROUPED || Fmt::SS, "grouped schedule: shared-memory A formats only");
   using C = Cfg<Fmt, N_MMA>;
   using MMA = Wgmma<N_MMA>;
   constexpr int S = C::STAGES;
@@ -232,6 +235,8 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   if constexpr (GROUPED) {
     // which weights a unit needs depends on offs, the previous kernel's output: no weight request before the wait
     __shared__ int s_end[MAX_EXPERTS], s_mbp[MAX_EXPERTS + 1];
+    // the static tables sit beside the ring, which Cfg::SMEM_BYTES does not count: both within the 227 KB a CTA may use
+    static_assert(C::SMEM_BYTES + sizeof(s_end) + sizeof(s_mbp) <= 227 * 1024, "grouped tables do not fit beside the ring");
     pdl_launch_dependents();
     pdl_wait();
     if (warp == 0) grouped_schedule<N_MMA>(p, s_end, s_mbp, lane);
@@ -285,7 +290,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         // map's zero fill), whose outputs the epilogue skips (n >= N_out)
         const int tile = tile_of(i), n_tile = tile % p.n_tiles;
         const int e = group_tile<N_MMA>(g_end, g_mbp, p.E, tile / p.n_tiles).e;
-        Fmt::issue_w_rows(&tm_w, st, &wfull[s], e * p.N + n_tile * ROWS, kc_of(i), pol_w);
+        Fmt::issue_w_rows(&tm_w, &tm_aux, p, st, st + Fmt::W_BYTES, &wfull[s], e * p.N + n_tile * ROWS, kc_of(i), pol_w);
       } else {
         Fmt::issue_w(&tm_w, &tm_aux, p, st, st + Fmt::W_BYTES, &wfull[s], tile_of(i) % p.n_tiles, kc_of(i), pol_w);
       }
@@ -344,11 +349,13 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       const int n_tile = tile % p.n_tiles, m_blk = tile / p.n_tiles;
       int m0 = m_blk * N_MMA, m_end = p.M;   // tokens m0 .. min(m0 + N_MMA, m_end) - 1 are this tile's
       const float* w_scale = p.w_scale;
+      const float* out_scale = p.out_scale;
       if constexpr (GROUPED) {
         const GroupTile gt = group_tile<N_MMA>(g_end, g_mbp, p.E, m_blk);
         m0 = gt.row0;
         m_end = gt.row_end;
         w_scale += (size_t)gt.e * p.N;
+        out_scale += gt.e;
       }
       if (kind == streamk::SEG_CONTRIB) {
         // publish the partial (column-major slot: word (token j, row r) at j * 128 + r), then one gpu-scope release
@@ -439,8 +446,13 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         const float bias = p.bias ? __bfloat162float(p.bias[n]) : 0.f;
         float osc = 1.f, sw = 1.f;
         if constexpr (Fmt::EPI == EPI_FLOAT) {
-          osc = (p.out_scale ? (p.out_scale_per_row ? p.out_scale[n] : *p.out_scale) : 1.f);
-          if (p.out_scale2) osc *= *p.out_scale2;
+          if constexpr (GROUPED) {
+            // the expert's own scale (required); never out_scale2, whose storage holds offs
+            osc = *out_scale;
+          } else {
+            osc = (p.out_scale ? (p.out_scale_per_row ? p.out_scale[n] : *p.out_scale) : 1.f);
+            if (p.out_scale2) osc *= *p.out_scale2;
+          }
           osc *= __int_as_float((127 + Fmt::ACC_EXP2) << 23);
         } else {
           sw = w_scale ? w_scale[n] : 1.f;

@@ -74,6 +74,17 @@ def _nvfp4_kernel_compat(weight, k_multiple: int) -> bool:
     return True
 
 
+def _nvfp4_expert_rows_compat(weight) -> bool:
+    """The grouped expert GEMM reads each expert's weights and blocked scales as whole 128-row blocks of the stacked
+    [E * N, ..] tensors (ts_gemm.cuh, Grouped<Nvfp4Fmt>), so it needs out_features % 128 == 0; the reference's 3-D
+    blocked scale layout has the same requirement (to_blocked over E * N rows).  Other layers stay unquantized."""
+    if weight.shape[-2] % 128 != 0:
+        logger.info(f"Skipping NVFP4 quantization: expert out_features={weight.shape[-2]} is not a multiple of 128; "
+                    f"weight shape {tuple(weight.shape)} stays {weight.dtype}")
+        return False
+    return True
+
+
 @dataclass
 class NVFP4DynamicActivationNVFP4WeightConfig(AOBaseConfig):
     use_triton_kernel: bool = True   # accepted for compatibility; the CUDA quantizer is always used
@@ -93,10 +104,21 @@ def _nvfp4_inference_linear_transform(module, config, *, parameter_name="weight"
     _check_nvfp4_shape(weight)
     if torch.cuda.is_available():
         require_sm90()
-    assert weight.dim() == 2, "3D (MoE) weights are out of scope"
-    if not _nvfp4_kernel_compat(weight, 256):
-        return module
-    pts = per_tensor_amax_to_scale(torch.max(torch.abs(weight))) if config.use_dynamic_per_tensor_scale else None
+    if weight.dim() == 3:
+        # MoE expert weights [E, N, K] for torch._grouped_mm: one per-tensor scale per expert [E, 1, 1] (reference
+        # :307-319).  The grouped kernel quantizes each expert's routed tokens with their own dynamic scale, so the
+        # static form has nothing to run on (the reference's handler would fail at the first forward)
+        if not config.use_dynamic_per_tensor_scale:
+            raise NotImplementedError("NVFP4DynamicActivationNVFP4WeightConfig on 3-D (MoE) weights needs "
+                                      "use_dynamic_per_tensor_scale=True")
+        if not _nvfp4_kernel_compat(weight, 128) or not _nvfp4_expert_rows_compat(weight):
+            return module
+        pts = per_tensor_amax_to_scale(torch.amax(torch.abs(weight), dim=(1, 2))).view(-1, 1, 1)
+    else:
+        assert weight.dim() == 2, f"NVFP4: 2-D or 3-D weights only, got {weight.dim()}-D"
+        if not _nvfp4_kernel_compat(weight, 256):
+            return module
+        pts = per_tensor_amax_to_scale(torch.max(torch.abs(weight))) if config.use_dynamic_per_tensor_scale else None
     act = QuantizeTensorToNVFP4Kwargs(use_dynamic_per_tensor_scale=config.use_dynamic_per_tensor_scale,
                                       use_triton_kernel=config.use_triton_kernel, is_swizzled_scales=True)
     qw = NVFP4Tensor.to_nvfp4(weight.contiguous(), per_tensor_scale=pts, is_swizzled_scales=True,

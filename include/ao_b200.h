@@ -184,6 +184,27 @@ int ao_nvfp4_weight_linear_ex(const uint16_t* x, int ldx, const float* x_scale, 
                               const uint8_t* wq, const uint8_t* w_scale_blocked, const float* b_pts,
                               int b_pts_per_row, int N, const uint16_t* bias, uint16_t* y,
                               void* workspace, size_t workspace_bytes, void* stream);
+/* Replaces torchao's aten._grouped_mm handler for an NVFP4Tensor expert weight (nvfp4_tensor.py:709-753), 2-D x 3-D
+ * form: for offs[e-1] <= m < offs[e] (offs[-1] = 0)
+ *   y[m, :] = bf16( (sum_k x[m,k] * e2m1(Wq[e])[:,k] * blockscale[e][:,k/16]) * x_scale[m] * w_pts[e] ),
+ * weights dequantised exactly inside the wgmma kernel.  x bf16 [M,K] (tokens sorted by expert; for NVFP4 activations
+ * the xhat of ao_nvfp4_fakequant_grouped); x_scale f32 [M] or NULL; wq uint8 [E][N][K/2] (the stored qdata);
+ * w_scale_blocked: each expert's [N, K/16] e4m3 scales in the blocked layout, one after the other; w_pts f32 [E];
+ * offs int32 [E] on the device, cumulative row ends.  The host never reads offs (no sync, CUDA-graph capturable); the
+ * kernel clamps each offs[e] into [offs[e-1], M].  Rows from offs[E-1] on are not written.
+ * 1 <= E <= 1024, K % 128 == 0, N % 128 == 0, no bias.                                                              */
+int ao_nvfp4_grouped_mm(const uint16_t* x, const float* x_scale, int M, int K, const uint8_t* wq,
+                        const uint8_t* w_scale_blocked, const float* w_pts, int E, int N,
+                        const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes, void* stream);
+/* The activations of the above, each expert's rows quantized to NVFP4 with that expert's own per-tensor scale
+ * a_pts[e] = amax(|x[rows of e]|) / (448 * 6), exactly as ao_nvfp4_quantize(x[rows of e], a_pts[e]) quantizes them,
+ * the rows of e being [end[e-1], end[e]) with end[e] = min(M, max(0, offs[0..e])) as in the GEMM.
+ * xhat bf16 [M,K] = each element's e2m1 code times its e4m3 block scale (exact in bf16); x_scale f32 [M] = a_pts of
+ * the row's expert.  An all-zero expert and the rows past end[E-1] get xhat = 0 and x_scale = 0.  x has row pitch ldx
+ * (elements; ldx >= K, ldx % 8 == 0, x 16-byte aligned); row_amax: f32 [M] device scratch.  K % 16 == 0, E >= 1.
+ * Two kernels; offs is never read on the host.                                                                      */
+int ao_nvfp4_fakequant_grouped(const uint16_t* x, int ldx, int M, int K, const int32_t* offs, int E,
+                               uint16_t* xhat, float* x_scale, float* row_amax, void* stream);
 /* Per-token e4m3 quantisation that keeps the codes as bf16 values (exact): xq = bf16(e4m3(x/s)),
  * s = f32(bf16(amax/448)) -- the codes of ao_fp8_quantize_rowwise, i.e. the values Float8Tensor.from_hp(x, PerRow())
  * stores (quant_primitives.py:2172-2287), in the operand type the bf16 MMA consumes.  An all-zero row (s = 0) gives

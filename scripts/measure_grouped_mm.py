@@ -1,8 +1,10 @@
 #!/usr/bin/env python
 """Times the fp8 rowwise grouped GEMM (torch.ops.ao_b200.fp8_rowwise_grouped_mm) against torch's rowwise
-F.scaled_grouped_mm on identical operands, for MoE expert shapes.
+F.scaled_grouped_mm on identical operands, for MoE expert shapes; with --fmt nvfp4, the NVFP4 expert path (the
+per-expert activation quantizer nvfp4_fakequant_grouped plus nvfp4_grouped_mm) against the fp8 path with its
+quantizer (fp8_quantize_rowwise plus fp8_rowwise_grouped_mm) and bf16 torch._grouped_mm on the unquantized weights.
 
-  python scripts/measure_grouped_mm.py [--replays 20] [--out FILE]
+  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4] [--replays 20] [--out FILE]
 
   * shapes: Mixtral-8x7B experts (E=8, 4096 -> 14336 and 14336 -> 4096, top-2) and Qwen3-30B-A3B experts (E=128,
     2048 -> 768 and 768 -> 2048, top-8);
@@ -14,7 +16,10 @@ Reported per case: µs, the output's SQNR against torch's on the written rows ("
 GB/s over the bytes the GEMM needs (weights and scales of experts with at least one row,
 activations, their scales, outputs, offs), and which data-sheet roofline term bounds it (H100 SXM: 3.35 TB/s HBM3,
 1979 TFLOP/s dense fp8; figures for a 700 W card) with the time that term gives.  One JSON line per case, then one with
-the card's name, power limit and maximum SM clock.
+the card's name, power limit and maximum SM clock.  --fmt nvfp4 reports µs and GB/s of the three paths over the bytes
+the NVFP4 path needs (0.5625 bytes per weight of the active experts, the bf16 activations read once, the outputs) and
+the output's SQNR against bf16 torch._grouped_mm; its roofline term is the HBM time of those bytes (the bf16 wgmma
+roofline, 989 TFLOP/s, is never the bound at these shapes up to 128 tokens).
 """
 from __future__ import annotations
 
@@ -80,8 +85,78 @@ def time_graph(fn_of_copy, copies, replays):
     return t0.elapsed_time(t1) * 1e3 / (replays * rounds * copies)
 
 
+def sqnr_db(ref, out):
+    import torch
+
+    d = (out.double() - ref.double()).norm()
+    return round(float(20 * torch.log10(ref.double().norm() / d)), 1) if d > 0 else "identical"
+
+
+def measure_nvfp4(a, ops, dev, lines):
+    """The NVFP4 expert path (prologue + GEMM) against fp8 (prologue + GEMM) and bf16 torch._grouped_mm."""
+    import torch
+
+    from ao_b200.prototype.mx_formats import per_tensor_amax_to_scale
+
+    for name, E, N, K, topk in SHAPES:
+        g = torch.Generator(device=dev).manual_seed(E * N + K)
+        bf16_expert = N * K * 2
+        copies = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * N * K * 0.5625)) + 1)
+        copies_bf16 = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * bf16_expert)) + 1)
+        w4, s4, p4, w8, s8, wb = [], [], [], [], [], []
+        for c in range(max(copies, copies_bf16)):
+            w = (torch.randn(E, N, K, device=dev, generator=g) * 0.05).to(torch.bfloat16)
+            if c < copies:
+                pts = per_tensor_amax_to_scale(torch.amax(torch.abs(w), dim=(1, 2)))
+                qs = [ops.nvfp4_quantize(w[e], pts[e].reshape(1), True) for e in range(E)]
+                w4.append(torch.stack([q for q, _ in qs]))
+                s4.append(torch.stack([s for _, s in qs]))
+                p4.append(pts)
+                q, s = ops.fp8_quantize_rowwise(w.reshape(E * N, K))
+                w8.append(q.reshape(E, N, K))
+                s8.append(s.reshape(E, N))
+            if c < copies_bf16:
+                wb.append(w)
+            del w
+        for T in TOKENS:
+            for skewed in (False, True):
+                rows = routing(T, E, topk, skewed, seed=T * 131 + E + skewed)
+                M = sum(rows)
+                offs = torch.tensor(rows, dtype=torch.int64).cumsum(0).to(torch.int32).to(dev)
+                x = torch.randn(M, K, device=dev, generator=g).to(torch.bfloat16)
+                active = sum(1 for r in rows if r)
+                need = int(active * N * K * 0.5625) + M * K * 2 + M * N * 2 + E * 8
+                rec = dict(fmt="nvfp4", shape=name, E=E, N=N, K=K, topk=topk, tokens=T,
+                           routing="skewed" if skewed else "balanced", rows=M, active_experts=active, bytes=need,
+                           weight_copies=copies, roofline_us=round(need / HBM_BPS * 1e6, 2))
+
+                def ours(c):
+                    xhat, xs = ops.nvfp4_fakequant_grouped(x, offs)
+                    return ops.nvfp4_grouped_mm(xhat, xs, w4[c], s4[c], p4[c], offs)
+
+                def fp8(c):
+                    xq, sx = ops.fp8_quantize_rowwise(x)
+                    return ops.fp8_rowwise_grouped_mm(xq, sx.reshape(-1), w8[c], s8[c], offs)
+
+                def bf16(c):
+                    return torch._grouped_mm(x, wb[c].transpose(-2, -1), offs=offs)
+
+                n = int(offs[-1])
+                y_ref = bf16(0)
+                rec["sqnr_vs_bf16_db"] = sqnr_db(y_ref[:n], ours(0)[:n])
+                for key, fn, cp in (("ours", ours, copies), ("fp8", fp8, copies), ("bf16", bf16, copies_bf16)):
+                    us = time_graph(fn, cp, a.replays)
+                    rec[f"{key}_us"] = round(us, 2)
+                    rec[f"{key}_GBps"] = round(need / us * 1e-3, 1)
+                print(json.dumps(rec), flush=True)
+                lines.append(rec)
+        del w4, s4, p4, w8, s8, wb
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--fmt", choices=["fp8", "nvfp4"], default="fp8")
     ap.add_argument("--replays", type=int, default=20)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -94,7 +169,7 @@ def main():
     ops = torch.ops.ao_b200
     dev = torch.device("cuda", 0)
     lines = []
-    for name, E, N, K, topk in SHAPES:
+    for name, E, N, K, topk in (SHAPES if a.fmt == "fp8" else []):
         g = torch.Generator(device=dev).manual_seed(E * N + K)
         w_bytes_expert = N * K + N * 4
         min_active = min(topk, E) * w_bytes_expert
@@ -145,6 +220,8 @@ def main():
                 lines.append(rec)
         del wq, sw
         torch.cuda.empty_cache()
+    if a.fmt == "nvfp4":
+        measure_nvfp4(a, ops, dev, lines)
     info = dict(card=card(), torch=torch.__version__)
     print(json.dumps(info), flush=True)
     if a.out:
