@@ -106,6 +106,10 @@ int sm_count() {
   return n;
 }
 
+// Launched without the PDL attribute and never triggering its dependents: it starts only once every earlier kernel on
+// the stream has completed, and the next kernel starts only once it has ended (ao_b200_pdl_fence).
+__global__ void pdl_fence_kernel() {}
+
 }  // namespace ao
 
 extern "C" {
@@ -133,5 +137,10 @@ size_t ao_b200_workspace_bytes(int M, int N) {
 uint64_t ao_b200_launch_count(void) { return ao::g_launch_count.load(); }
 
 int ao_b200_debug_set_streamk_ctas(int n) { return ao::g_streamk_ctas.exchange(n > 0 ? n : 0); }
+
+int ao_b200_pdl_fence(void* stream) {
+  AO_CUDA_CHECK(ao::launch(ao::pdl_fence_kernel, dim3(1), dim3(1), 0, reinterpret_cast<cudaStream_t>(stream), false));
+  return AO_OK;
+}
 
 }  // extern "C"

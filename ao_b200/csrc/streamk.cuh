@@ -29,7 +29,9 @@
 //   * every CTA triggers its dependents first thing, so grid j is entirely resident before any CTA of j+1 launches;
 //     an owner of j therefore only waits on CTAs that are already running;
 //   * a CTA of j+1 touches the workspace, the flags and the activations only after griddepcontrol.wait, i.e. after
-//     grid j has completed; before that it only streams weights into its own shared memory, and j never waits on it;
+//     grid j has completed; before that it only streams weights into its own shared memory, and j never waits on it
+//     (the weights must be complete before grid j starts: a weight quantized by this library is separated from its
+//     first linear by ao_b200_pdl_fence, which quantize_ launches);
 //   * CTAs of j+1 that did not find room become resident as CTAs of j exit, which they do without waiting on j+1.
 //
 // Device-side grid (grouped GEMM, ts_gemm.cuh Grouped<Fmt>).  The units per expert come from offs, which only the

@@ -174,6 +174,8 @@ TORCH_LIBRARY(ao_b200, m) {
   m.def("debug_workspace(Tensor like) -> Tensor", [](const at::Tensor& like) { return workspace_for(like); });
   // tests only: force the stream-K grid of every GEMM launch (0 = heuristic); returns the previous value
   m.def("debug_set_streamk_ctas(int n) -> int", [](int64_t n) -> int64_t { return ao_b200_debug_set_streamk_ctas((int)n); });
+  // on the current device's current stream: orders a weight written by the quantizers before the linears that read it
+  m.def("pdl_fence() -> ()", []() { AO_CALL(ao_b200_pdl_fence(cur_stream())); });
   ao_b200_define_lowp(m);
 }
 

@@ -308,7 +308,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
     };
     const int pre = nunits < S ? nunits : S;
     for (int i = 0; i < pre; ++i) {
-      if (elect_one()) issue_w(i);   // weights never depend on the previous kernel
+      if (elect_one()) issue_w(i);   // weights are complete before the previous kernel starts (ao_b200_pdl_fence)
       __syncwarp();
     }
     pdl_wait();   // activations are the previous kernel's output

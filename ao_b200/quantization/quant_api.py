@@ -99,6 +99,7 @@ def quantize_(model: torch.nn.Module, config: AOBaseConfig,
                     child = module_fqn.split(".")[-1]
                     parent = named_modules[module_fqn.removesuffix(child).removesuffix(".")]
                     setattr(parent, child, replacement)
+        _fence_quantized_weights(model)
         return
     if not isinstance(config, AOBaseConfig):
         raise AssertionError("quantize_ expects an AOBaseConfig workflow configuration object")
@@ -107,6 +108,17 @@ def quantize_(model: torch.nn.Module, config: AOBaseConfig,
         raise KeyError(f"no quantize handler registered for {type(config).__name__}")
     handler = _QUANTIZE_CONFIG_HANDLER[type(config)]
     _replace_with_custom_fn_if_matches_filter(model, handler, filter_fn, device=device, extra_args=(config,))
+    _fence_quantized_weights(model)
+
+
+def _fence_quantized_weights(model: torch.nn.Module):
+    """The GEMM behind a quantized linear starts loading its weights before it waits for the kernel ahead of it
+    (programmatic dependent launch), and the weight quantizers let the next kernels start early.  One
+    torch.ops.ao_b200.pdl_fence per device that holds CUDA parameters, on its current stream, makes the weights just
+    written complete before the first linear (or the activation quantizer ahead of it) starts."""
+    for d in {p.device for p in model.parameters() if p.is_cuda}:
+        with torch.cuda.device(d):
+            torch.ops.ao_b200.pdl_fence()
 
 
 # ---------------------------------------------------------------------------------------------

@@ -19,7 +19,17 @@
  *     (tensor maps are built on the host and passed by value);
  *   - `workspace` is caller-owned scratch for split-K partials + flags; it
  *     must be zero-initialised once (kernels restore the flags to zero) and
- *     must not be shared by linears running concurrently on different streams.
+ *     must not be shared by linears running concurrently on different streams;
+ *   - kernels are launched with programmatic dependent launch (PDL): each one
+ *     lets the next kernel on the stream start early and waits for its
+ *     predecessor before reading activations, scales, offs or the workspace.
+ *     The dense GEMMs behind every linear below request their first WEIGHT
+ *     tiles (wq and the weight scales) before that wait, so weights must be
+ *     complete before the GEMM's predecessor starts.  A buffer written by this
+ *     library's quantizers (ao_*_quantize*) and then read as the weights of a
+ *     linear must be separated from that linear by ao_b200_pdl_fence, by any
+ *     launch without PDL (e.g. a torch kernel) or by an event / stream sync.
+ *     The grouped GEMMs read no weight before the wait.
  */
 #ifndef AO_B200_H_
 #define AO_B200_H_
@@ -51,6 +61,10 @@ uint64_t ao_b200_launch_count(void);
  * restores the per-problem heuristic.  Process-wide, not thread-safe against concurrent launches; returns the
  * previous value.  No production path calls it. */
 int ao_b200_debug_set_streamk_ctas(int n);
+/* Launches one empty kernel without PDL that never lets its dependents start early: the next kernel on `stream` starts
+ * only after every kernel before the fence has completed and its writes are visible.  Call it between quantizing a
+ * weight with this library and the first linear that reads it (quantize_ does). */
+int ao_b200_pdl_fence(void* stream);
 
 /* int4 weight-only, tile_packed_to_4d ---------------------------------------- */
 /* Replaces aten._convert_weight_to_int4pack(uint8[N,K/2], inner_k_tiles)

@@ -45,6 +45,23 @@ def test_c_abi_argument_validation_without_gpu():
     assert lib.ao_int4_tilepacked_linear(None, 0, 1024, None, None, 32, 128, None, None, 128, None, ctypes.c_size_t(0), 0, None) == 0
 
 
+def test_pdl_fence_on_the_null_stream():
+    """ao_b200_pdl_fence(NULL) launches its empty kernel on the legacy default stream; without a device it reports the
+    failed launch instead of crashing.  torch.ops.ao_b200.pdl_fence is its registration."""
+    import ao_b200  # noqa: F401
+
+    lib = ctypes.CDLL(os.path.join(ROOT, "ao_b200", "lib", "libao_b200.so"))
+    lib.ao_b200_last_error.restype = ctypes.c_char_p
+    lib.ao_b200_pdl_fence.argtypes = [ctypes.c_void_p]
+    rc = lib.ao_b200_pdl_fence(None)
+    if torch.cuda.is_available():
+        assert rc == 0, lib.ao_b200_last_error()
+        torch.cuda.synchronize()
+    else:
+        assert rc == -2 and b"pdl_fence_kernel" in lib.ao_b200_last_error()
+    assert torch.ops.ao_b200.pdl_fence.default._schema.returns == []
+
+
 def test_torch_ops_registered_with_meta_kernels():
     import ao_b200  # noqa: F401
 
