@@ -47,22 +47,34 @@ struct Int4Fmt {
   static constexpr int EPI = tsg::EPI_FLOAT;
   static constexpr int ACC_EXP2 = 0;
   static constexpr int MAX_N_MMA = 128;
-  // the packed weights ({32 words, 4 row-pairs, 16 n8-tiles} box, 128-byte swizzle) and the (scale, zero) pairs
-  static int make_maps(const int32_t* qdata, const uint16_t* sz, int N, int K, int g, CUtensorMap* tm_w,
-                       CUtensorMap* tm_sz) {
+  static constexpr bool EXPERT_SCALE = false;   // grouped: y = acc, no scale, bias or row scale
+  // the packed weights of `rows` rows ({32 words, 4 row-pairs, 16 n8-tiles} box, 128-byte swizzle)
+  static int make_w_map(const int32_t* qdata, int rows, int K, CUtensorMap* tm_w) {
     const int KT = K / 128;
-    {
-      const uint64_t dims[3] = {32, (uint64_t)4 * KT, (uint64_t)N / 8};
-      const uint64_t str[2] = {128, (uint64_t)KT * 512};
-      const uint32_t box[3] = {32, 4, 16};
-      int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_INT32, 3, qdata, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-      if (rc) return rc;
-    }
+    const uint64_t dims[3] = {32, (uint64_t)4 * KT, (uint64_t)rows / 8};
+    const uint64_t str[2] = {128, (uint64_t)KT * 512};
+    const uint32_t box[3] = {32, 4, 16};
+    return make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_INT32, 3, qdata, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+  }
+  // the (scale, zero) pairs as uint32 [groups][N]: box {128 features, the groups of one 128-k chunk}
+  static int make_sz_map(const uint16_t* sz, int N, long long groups, int g, CUtensorMap* tm_sz) {
     const int gpc = g <= 128 ? 128 / g : 1;
-    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)K / g};
+    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)groups};
     const uint64_t str[1] = {(uint64_t)N * 4};
     const uint32_t box[2] = {128, (uint32_t)gpc};
     return make_tmap(tm_sz, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, sz, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
+  static int make_maps(const int32_t* qdata, const uint16_t* sz, int N, int K, int g, CUtensorMap* tm_w,
+                       CUtensorMap* tm_sz) {
+    if (int rc = make_w_map(qdata, N, K, tm_w)) return rc;
+    return make_sz_map(sz, N, K / g, g, tm_sz);
+  }
+  // grouped: the stacked experts' qdata [E, N/8, K/128, 32, 4] is one tensor of E*N/8 n8-tiles with the dense strides;
+  // their scale_and_zero [E, K/g, N, 2] is uint32 [E*K/g][N] (expert e's groups at rows e*K/g ..)
+  static int make_grouped_maps(const int32_t* qdata, const uint16_t* sz, int E, int N, int K, int g, CUtensorMap* tm_w,
+                               CUtensorMap* tm_sz) {
+    if (int rc = make_w_map(qdata, E * N, K, tm_w)) return rc;
+    return make_sz_map(sz, N, (long long)E * (K / g), g, tm_sz);
   }
   __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params& p) {
     const int gpc = p.group_size <= KCHUNK ? KCHUNK / p.group_size : 1;
@@ -73,6 +85,16 @@ struct Int4Fmt {
                                                  uint64_t* bar, int n_tile, int kc, uint64_t policy) {
     tma_load_3d(w_dst, tm_w, bar, 0, 4 * kc, n_tile * (ROWS / 8), policy);
     tma_load_2d(aux_dst, tm_sz, bar, n_tile * ROWS, (kc * KCHUNK) / p.group_size, policy);
+  }
+  // grouped kernels: the 128 weight rows from `row` = e*N + 128t of all experts' n8-tiles, and expert e's (scale, zero)
+  // pairs of features 128t .. 128t+127 (the map zero-fills those past N; a weight tail past N reads the next expert's
+  // rows, or the map's zero fill after the last, and the epilogue skips their outputs)
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, const CUtensorMap* tm_sz,
+                                                      const tsg::Params& p, uint8_t* w_dst, uint8_t* aux_dst,
+                                                      uint64_t* bar, int row, int kc, uint64_t policy) {
+    const int e = row / p.N;
+    tma_load_3d(w_dst, tm_w, bar, 0, 4 * kc, row / 8, policy);
+    tma_load_2d(aux_dst, tm_sz, bar, row - e * p.N, e * (p.K / p.group_size) + (kc * KCHUNK) / p.group_size, policy);
   }
   // the thread's two fragment rows: 16 bytes (4 tinygemm words = 128 k) each, and the (s, z) pair of every 32-k word
   struct Raw {
@@ -213,4 +235,38 @@ extern "C" int ao_int4_tilepacked_linear(const uint16_t* x, int M, int K, const 
                                          void* stream) {
   return ao_int4_tilepacked_linear_strided(x, K, M, K, qdata, scale_and_zero, group_size, N, bias, y, N_out, workspace,
                                            workspace_bytes, impl, stream);
+}
+
+// torch._grouped_mm(x, W.transpose(-2, -1), offs) on 3-D int4 tile-packed expert weights, 2-D x 3-D: expert e's rows
+// [offs[e-1], offs[e]) of x against qdata[e] with its scale_and_zero[e], y = acc in bf16.  N is the padded feature
+// count (the expert stride of qdata and scale_and_zero), N_out <= N the columns of y.  offs stays on the device
+// (grouped schedule, ts_gemm.cuh).
+extern "C" int ao_int4_tilepacked_grouped_mm(const uint16_t* x, int M, int K, const int32_t* qdata,
+                                             const uint16_t* scale_and_zero, int group_size, int E, int N, int N_out,
+                                             const int32_t* offs, uint16_t* y, void* workspace,
+                                             size_t workspace_bytes, void* stream) {
+  using namespace ao;
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int4 grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(K % 1024 == 0, "int4 grouped mm: K=%d must be a multiple of 1024 (format pads K)", K);
+  AO_REQUIRE(N % 8 == 0, "int4 grouped mm: N=%d must be a multiple of 8", N);
+  AO_REQUIRE(N_out > 0 && N_out <= N, "int4 grouped mm: N_out=%d out of range (N=%d)", N_out, N);
+  AO_REQUIRE(group_size == 32 || group_size == 64 || group_size == 128 || group_size == 256,
+             "int4 grouped mm: group_size=%d not in {32,64,128,256}", group_size);
+  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "int4 grouped mm: E=%d experts must be in [1, %d]", E, tsg::MAX_EXPERTS);
+  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "int4 grouped mm: E*N=%lld weight rows exceed the int32 range", (long long)E * N);
+  AO_REQUIRE((long long)E * (K / group_size) <= 0x7FFFFFFF, "int4 grouped mm: E*K/g=%lld scale rows exceed the int32 range",
+             (long long)E * (K / group_size));
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && qdata && scale_and_zero && offs && y && workspace, "int4 grouped mm: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "int4 grouped mm: x must be 16-byte aligned");
+  using Fmt = tsg::Grouped<int4k::Int4Fmt>;
+  CUtensorMap tm_w, tm_sz;
+  if (int rc = Fmt::make_grouped_maps(qdata, scale_and_zero, E, N, K, group_size, &tm_w, &tm_sz)) return rc;
+  tsg::Params p{};
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.offs = offs;
+  p.E = E;
+  p.M = M; p.N = N; p.N_out = N_out; p.K = K; p.group_size = group_size;
+  return tsg::run<Fmt>(p, tm_w, tm_sz, x, K, workspace, workspace_bytes, "int4 grouped mm",
+                       reinterpret_cast<cudaStream_t>(stream));
 }

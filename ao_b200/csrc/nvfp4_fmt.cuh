@@ -35,6 +35,7 @@ struct Nvfp4Fmt {
   static constexpr int EPI = tsg::EPI_FLOAT;
   static constexpr int ACC_EXP2 = 60;   // the accumulators hold the result * 2^-60
   static constexpr int MAX_N_MMA = 128;
+  static constexpr bool EXPERT_SCALE = true;   // grouped: the per-expert weight scale w_pts[e]
   // the packed weights (128 rows x 64 bytes, 64B swizzle) and the blocked scale tiles
   static int make_maps(const uint8_t* wq, const uint8_t* w_sf, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
     {

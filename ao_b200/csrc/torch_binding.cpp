@@ -143,6 +143,35 @@ Tensor int4_tilepacked_linear(const Tensor& x, const Tensor& qdata, int64_t grou
   return y;
 }
 
+// torch._grouped_mm on 3-D int4 expert weights (2-D x 3-D): x bf16 [M, K] (contiguous), qdata int32
+// [E, N/8, K/128, 32, 4], scale_and_zero bf16 [E, K/g, N, 2], offs int32 [E] -> y [M, n_out] (n_out <= 0: N).  Rows
+// from offs[E-1] on are left unwritten, as torch leaves them; offs is never read on the host.
+Tensor int4_tilepacked_grouped_mm(const Tensor& x, const Tensor& qdata, int64_t group_size, const Tensor& scale_and_zero,
+                                  const Tensor& offs, int64_t n_out) {
+  TORCH_CHECK(x.is_cuda(), "ao_b200: x must be a CUDA tensor");
+  check_cuda(qdata, "qdata");
+  check_cuda(scale_and_zero, "scale_and_zero");
+  check_cuda(offs, "offs");
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2, "ao_b200: x must be bf16 [M, K]");
+  TORCH_CHECK(x.size(0) <= 1 || (x.stride(0) == x.size(1) && x.stride(1) == 1), "ao_b200: x must be contiguous");
+  TORCH_CHECK(qdata.scalar_type() == at::kInt && qdata.dim() == 5 && qdata.size(3) == 32 && qdata.size(4) == 4, "ao_b200: qdata must be int32 [E, N/8, K/128, 32, 4]");
+  TORCH_CHECK(scale_and_zero.scalar_type() == at::kBFloat16 && scale_and_zero.dim() == 4 && scale_and_zero.size(3) == 2, "ao_b200: scale_and_zero must be bf16 [E, K/g, N, 2]");
+  TORCH_CHECK(offs.scalar_type() == at::kInt && offs.dim() == 1, "ao_b200: offs must be int32 [E]");
+  TORCH_CHECK(offs.device() == x.device(), "ao_b200: offs must be on the device of x");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int64_t M = x.size(0), K = x.size(1), E = qdata.size(0), N = qdata.size(1) * 8;
+  TORCH_CHECK(qdata.size(2) * 128 == K, "ao_b200: x has K=", K, " but qdata encodes K=", qdata.size(2) * 128);
+  TORCH_CHECK(scale_and_zero.size(0) == E && scale_and_zero.size(1) * group_size == K && scale_and_zero.size(2) == N, "ao_b200: scale_and_zero shape does not match (E, K/g, N)");
+  TORCH_CHECK(offs.size(0) == E, "ao_b200: offs must have E=", E, " elements");
+  if (n_out <= 0) n_out = N;
+  TORCH_CHECK(n_out <= N, "ao_b200: n_out > N");
+  Tensor y = at::empty({M, n_out}, x.options());
+  if (M == 0) return y;
+  Tensor ws = workspace_for(x);
+  AO_CALL(ao_int4_tilepacked_grouped_mm(bf16_ptr(x), (int)M, (int)K, qdata.data_ptr<int32_t>(), bf16_ptr(scale_and_zero), (int)group_size, (int)E, (int)N, (int)n_out, offs.data_ptr<int32_t>(), bf16_ptr_mut(y), ws.data_ptr(), (size_t)ws.numel(), cur_stream()));
+  return y;
+}
+
 // ------------------------------------------------------------------ meta kernels
 Tensor int4_pack_tile4d_meta(const Tensor& q_u8, int64_t ikt) {
   return at::empty({q_u8.size(0) / 8, q_u8.size(1) * 2 / (ikt * 16), 32, ikt / 2}, q_u8.options().dtype(at::kInt));
@@ -159,6 +188,11 @@ Tensor int4_tilepacked_linear_meta(const Tensor& x, const Tensor& qdata, int64_t
   if (n_out <= 0) n_out = qdata.size(0) * 8;
   return at::empty({x.size(0), n_out}, x.options());
 }
+Tensor int4_tilepacked_grouped_mm_meta(const Tensor& x, const Tensor& qdata, int64_t, const Tensor&, const Tensor&,
+                                       int64_t n_out) {
+  if (n_out <= 0) n_out = qdata.size(1) * 8;
+  return at::empty({x.size(0), n_out}, x.options());
+}
 
 }  // namespace
 
@@ -170,6 +204,7 @@ TORCH_LIBRARY(ao_b200, m) {
   m.def("int4_dequant_tile4d(Tensor qdata, Tensor scale_and_zero, int group_size) -> Tensor");
   m.def("int4_hqq_quantize(Tensor w, int group_size) -> (Tensor, Tensor, Tensor)");
   m.def("int4_tilepacked_linear(Tensor x, Tensor qdata, int group_size, Tensor scale_and_zero, Tensor? bias, int n_out=0, int impl=0) -> Tensor");
+  m.def("int4_tilepacked_grouped_mm(Tensor x, Tensor qdata, int group_size, Tensor scale_and_zero, Tensor offs, int n_out) -> Tensor");
   m.def("launch_count() -> int", []() -> int64_t { return (int64_t)ao_b200_launch_count(); });
   m.def("debug_workspace(Tensor like) -> Tensor", [](const at::Tensor& like) { return workspace_for(like); });
   // tests only: force the stream-K grid of every GEMM launch (0 = heuristic); returns the previous value
@@ -185,6 +220,7 @@ TORCH_LIBRARY_IMPL(ao_b200, CUDA, m) {
   m.impl("int4_dequant_tile4d", &int4_dequant_tile4d);
   m.impl("int4_hqq_quantize", &int4_hqq_quantize);
   m.impl("int4_tilepacked_linear", &int4_tilepacked_linear);
+  m.impl("int4_tilepacked_grouped_mm", &int4_tilepacked_grouped_mm);
   ao_b200_impl_lowp_cuda(m);
 }
 
@@ -194,5 +230,6 @@ TORCH_LIBRARY_IMPL(ao_b200, Meta, m) {
   m.impl("int4_dequant_tile4d", &int4_dequant_tile4d_meta);
   m.impl("int4_hqq_quantize", &int4_hqq_quantize_meta);
   m.impl("int4_tilepacked_linear", &int4_tilepacked_linear_meta);
+  m.impl("int4_tilepacked_grouped_mm", &int4_tilepacked_grouped_mm_meta);
   ao_b200_impl_lowp_meta(m);
 }

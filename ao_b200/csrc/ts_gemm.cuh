@@ -37,10 +37,27 @@ constexpr int MAX_STAGES = 12;
 // CTA (PDL) becomes resident beside the running one and fills its ring with weights during that kernel's tail,
 // instead of starting after it on an empty pipeline.  Each CTA then has half of the SM's 228 KB (less the 1 KB the driver reserves per CTA) and 80 registers
 // per thread at launch; the producer warpgroup gives registers back to the consumers (setmaxnreg).  Prefill tiles
-// keep one CTA per SM and up to 200 KB of ring.
+// keep one CTA per SM and up to 200 KB of ring.  Grouped<Fmt> kernels (below) always run one CTA per SM: they cannot
+// request weights before griddepcontrol.wait (which weights depends on offs), so a second resident CTA gains nothing,
+// and their 8 KB schedule tables do not fit beside a ring sized to half of the SM.
 constexpr int SMEM_PER_SM = 228 * 1024, SMEM_RESERVED_PER_CTA = 1024;
+
+// ts_gemm_kernel<Grouped<Fmt>, N_MMA>: Fmt under the grouped schedule (see Grouped schedule below), for a shared-memory
+// A format (fp8) or a register-A one (nvfp4, int4).  A wrapper rather than a kernel template parameter, so the dense
+// kernels keep their names and their code.
+template <class F>
+struct Grouped : F {};
+template <class F>
+struct IsGrouped {
+  static constexpr bool value = false;
+};
+template <class F>
+struct IsGrouped<Grouped<F>> {
+  static constexpr bool value = true;
+};
+
 template <class Fmt, int N_MMA>
-constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA ? 2 : 1; }
+constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA && !IsGrouped<Fmt>::value ? 2 : 1; }
 constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
 
 // Epilogue arithmetic, per kind (Fmt::EPI; must stay what each format's reference computes, see Params)
@@ -80,20 +97,6 @@ static_assert(sizeof(Params) == 120, "Params layout (see above)");
 // picked for that U (streamk.cuh, "Device-side grid").
 constexpr int MAX_EXPERTS = 1024;   // one row end and one m-block prefix per expert in shared memory
 constexpr int MIN_UNITS = 4;        // never fewer chunks per CTA (launch_gemm)
-
-// ts_gemm_kernel<Grouped<Fmt>, N_MMA>: Fmt under the grouped schedule, for a shared-memory A format (fp8) or a
-// register-A one (nvfp4).  A wrapper rather than a kernel template parameter, so the dense kernels keep their names and
-// their code.
-template <class F>
-struct Grouped : F {};
-template <class F>
-struct IsGrouped {
-  static constexpr bool value = false;
-};
-template <class F>
-struct IsGrouped<Grouped<F>> {
-  static constexpr bool value = true;
-};
 
 struct GroupTile {
   int e, row0, row_end;   // the expert, the tile's first row and the expert's end row (rows >= row_end: not stored)
@@ -203,6 +206,7 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 //   static void issue_w_rows(tm_w, tm_aux, p, w smem dst, aux smem dst, full barrier, row, kc, policy)
 //                                                                  grouped only: the 128 weight rows from `row` of the
 //                                                                  [E * N, K] map of all experts, and their aux tiles
+//   EXPERT_SCALE (grouped EPI_FLOAT only): the epilogue multiplies by out_scale[e] (nvfp4: yes, int4: no scale at all)
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
 //   RA:  struct Raw; static void load(p, w smem, aux smem, row_lo, lane, Raw&)   rows row_lo and row_lo + 8
 //        static void frag(p, raw, kk, a[4])                        bf16 A fragment of k16 step kk (0..7)
@@ -235,8 +239,11 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   if constexpr (GROUPED) {
     // which weights a unit needs depends on offs, the previous kernel's output: no weight request before the wait
     __shared__ int s_end[MAX_EXPERTS], s_mbp[MAX_EXPERTS + 1];
-    // the static tables sit beside the ring, which Cfg::SMEM_BYTES does not count: both within the 227 KB a CTA may use
+    // the static tables sit beside the ring, which Cfg::SMEM_BYTES does not count: both within the 227 KB a CTA may use,
+    // and every resident CTA's ring, tables and reserve within the SM
     static_assert(C::SMEM_BYTES + sizeof(s_end) + sizeof(s_mbp) <= 227 * 1024, "grouped tables do not fit beside the ring");
+    static_assert(C::CTAS * (C::SMEM_BYTES + sizeof(s_end) + sizeof(s_mbp) + SMEM_RESERVED_PER_CTA) <= SMEM_PER_SM,
+                  "grouped CTAs per SM do not fit");
     pdl_launch_dependents();
     pdl_wait();
     if (warp == 0) grouped_schedule<N_MMA>(p, s_end, s_mbp, lane);
@@ -447,8 +454,9 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         float osc = 1.f, sw = 1.f;
         if constexpr (Fmt::EPI == EPI_FLOAT) {
           if constexpr (GROUPED) {
-            // the expert's own scale (required); never out_scale2, whose storage holds offs
-            osc = *out_scale;
+            // the expert's own scale where the format has one (required then); never out_scale2, whose storage holds
+            // offs
+            if constexpr (Fmt::EXPERT_SCALE) osc = *out_scale;
           } else {
             osc = (p.out_scale ? (p.out_scale_per_row ? p.out_scale[n] : *p.out_scale) : 1.f);
             if (p.out_scale2) osc *= *p.out_scale2;

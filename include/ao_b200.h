@@ -112,6 +112,19 @@ int ao_int4_tilepacked_linear_strided(const uint16_t* x, int ldx, int M, int K, 
                                       const uint16_t* bias, uint16_t* y, int N_out,
                                       void* workspace, size_t workspace_bytes, int impl,
                                       void* stream);
+/* torch._grouped_mm(x, W.transpose(-2, -1), offs) for a 3-D Int4TilePackedTo4dTensor expert weight W [E, N_out, K],
+ * 2-D x 3-D form: for offs[e-1] <= m < offs[e] (offs[-1] = 0)
+ *   y[m, n] = bf16( sum_k x[m,k] * bf16((q[e][n,k]-8)*s + z) ),  n < N_out, f32 accumulate,
+ * weights dequantised inside the wgmma kernel exactly as ao_int4_tilepacked_linear does.  x bf16 [M,K] (tokens sorted
+ * by expert, rows contiguous); qdata int32 [E][N/8][K/128][32][4]; scale_and_zero bf16 [E][K/g][N][2]; N the padded
+ * feature count (the expert stride), N_out <= N the row stride of y [M, N_out]; offs int32 [E] on the device,
+ * cumulative row ends.  The host never reads offs (no sync, CUDA-graph capturable); the kernel clamps each offs[e]
+ * into [offs[e-1], M].  Rows from offs[E-1] on are not written.
+ * 1 <= E <= 1024, K % 1024 == 0, N % 8 == 0, g in {32,64,128,256}, no bias.                                         */
+int ao_int4_tilepacked_grouped_mm(const uint16_t* x, int M, int K, const int32_t* qdata,
+                                  const uint16_t* scale_and_zero, int group_size, int E, int N, int N_out,
+                                  const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes,
+                                  void* stream);
 /* int8 dynamic activation x int8 weight --------------------------------------- */
 /* Per-token symmetric int8 quantisation of activations: replaces
  * Int8Tensor.from_hp(x, PerRow()) on the hot path (int8_tensor.py:176-248 via

@@ -4,7 +4,7 @@ F.scaled_grouped_mm on identical operands, for MoE expert shapes; with --fmt nvf
 per-expert activation quantizer nvfp4_fakequant_grouped plus nvfp4_grouped_mm) against the fp8 path with its
 quantizer (fp8_quantize_rowwise plus fp8_rowwise_grouped_mm) and bf16 torch._grouped_mm on the unquantized weights.
 
-  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4] [--replays 20] [--out FILE]
+  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4] [--group-size 32] [--replays 20] [--out FILE]
 
   * shapes: Mixtral-8x7B experts (E=8, 4096 -> 14336 and 14336 -> 4096, top-2) and Qwen3-30B-A3B experts (E=128,
     2048 -> 768 and 768 -> 2048, top-8);
@@ -19,7 +19,11 @@ activations, their scales, outputs, offs), and which data-sheet roofline term bo
 the card's name, power limit and maximum SM clock.  --fmt nvfp4 reports µs and GB/s of the three paths over the bytes
 the NVFP4 path needs (0.5625 bytes per weight of the active experts, the bf16 activations read once, the outputs) and
 the output's SQNR against bf16 torch._grouped_mm; its roofline term is the HBM time of those bytes (the bf16 wgmma
-roofline, 989 TFLOP/s, is never the bound at these shapes up to 128 tokens).
+roofline, 989 TFLOP/s, is never the bound at these shapes up to 128 tokens).  --fmt int4 --group-size {32,128}: the
+int4 expert GEMM (int4_tilepacked_grouped_mm on 3-D Int4TilePackedTo4dTensor weights) against the dense int4 linear of
+each active expert (the select loop, captured with the routing fixed, without its host syncs), the fp8 path with its
+quantizer and bf16 torch._grouped_mm; bytes are the int4 path's (0.5 + 4 / g bytes per weight of the active experts,
+K and N as padded, the bf16 activations read once, the outputs).
 """
 from __future__ import annotations
 
@@ -154,9 +158,82 @@ def measure_nvfp4(a, ops, dev, lines):
         torch.cuda.empty_cache()
 
 
+def measure_int4(a, ops, dev, lines):
+    """The int4 expert GEMM against the per-expert dense int4 linears, fp8 (prologue + GEMM) and bf16."""
+    import torch
+
+    from ao_b200.quantization import Int4TilePackedTo4dTensor
+
+    gs = a.group_size
+    for name, E, N, K, topk in SHAPES:
+        g = torch.Generator(device=dev).manual_seed(E * N + K)
+        Np, Kp = -(-N // 8) * 8, -(-K // 1024) * 1024
+        per_weight = 0.5 + 4.0 / gs
+        copies = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * Np * Kp * per_weight)) + 1)
+        copies8 = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * N * K)) + 1)
+        copies_bf16 = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * N * K * 2)) + 1)
+        w4, w8, s8, wb = [], [], [], []
+        for c in range(max(copies, copies8, copies_bf16)):
+            w = (torch.randn(E, N, K, device=dev, generator=g) * 0.05).to(torch.bfloat16)
+            if c < copies:
+                w4.append(Int4TilePackedTo4dTensor.from_hp(w, [1, 1, gs]))
+            if c < copies8:
+                q, s = ops.fp8_quantize_rowwise(w.reshape(E * N, K))
+                w8.append(q.reshape(E, N, K))
+                s8.append(s.reshape(E, N))
+            if c < copies_bf16:
+                wb.append(w)
+            del w
+        for T in TOKENS:
+            for skewed in (False, True):
+                rows = routing(T, E, topk, skewed, seed=T * 131 + E + skewed)
+                M = sum(rows)
+                offs = torch.tensor(rows, dtype=torch.int64).cumsum(0).to(torch.int32).to(dev)
+                x = torch.randn(M, K, device=dev, generator=g).to(torch.bfloat16)
+                xp = torch.nn.functional.pad(x, (0, Kp - K)).contiguous()
+                active = sum(1 for r in rows if r)
+                need = int(active * Np * Kp * per_weight) + M * Kp * 2 + M * N * 2 + E * 4
+                rec = dict(fmt=f"int4 g{gs}", shape=name, E=E, N=N, K=K, topk=topk, tokens=T,
+                           routing="skewed" if skewed else "balanced", rows=M, active_experts=active, bytes=need,
+                           weight_copies=copies, roofline_us=round(need / HBM_BPS * 1e6, 2))
+                spans, start = [], 0
+                for e, r in enumerate(rows):
+                    if r:
+                        spans.append((e, start, start + r))
+                    start += r
+
+                def ours(c):
+                    return torch._grouped_mm(x, w4[c].transpose(-2, -1), offs=offs)
+
+                def loop(c):
+                    w = w4[c]
+                    for e, s0, s1 in spans:
+                        ops.int4_tilepacked_linear(xp[s0:s1], w.qdata[e], gs, w.scale_and_zero[e], None, N, 0)
+
+                def fp8(c):
+                    xq, sx = ops.fp8_quantize_rowwise(x)
+                    return ops.fp8_rowwise_grouped_mm(xq, sx.reshape(-1), w8[c], s8[c], offs)
+
+                def bf16(c):
+                    return torch._grouped_mm(x, wb[c].transpose(-2, -1), offs=offs)
+
+                n = int(offs[-1])
+                rec["sqnr_vs_bf16_db"] = sqnr_db(bf16(0)[:n], ours(0)[:n])
+                for key, fn, cp in (("ours", ours, copies), ("expert_loop", loop, copies), ("fp8", fp8, copies8),
+                                    ("bf16", bf16, copies_bf16)):
+                    us = time_graph(fn, cp, a.replays)
+                    rec[f"{key}_us"] = round(us, 2)
+                    rec[f"{key}_GBps"] = round(need / us * 1e-3, 1)
+                print(json.dumps(rec), flush=True)
+                lines.append(rec)
+        del w4, w8, s8, wb
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--fmt", choices=["fp8", "nvfp4"], default="fp8")
+    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4"], default="fp8")
+    ap.add_argument("--group-size", type=int, choices=[32, 64, 128, 256], default=32)
     ap.add_argument("--replays", type=int, default=20)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -222,6 +299,8 @@ def main():
         torch.cuda.empty_cache()
     if a.fmt == "nvfp4":
         measure_nvfp4(a, ops, dev, lines)
+    if a.fmt == "int4":
+        measure_int4(a, ops, dev, lines)
     info = dict(card=card(), torch=torch.__version__)
     print(json.dumps(info), flush=True)
     if a.out:
