@@ -58,12 +58,16 @@ def fp32_exact(t, what):
 def premise(X, W, bias_acc=None, chunk=False):
     """Asserts max(|X| @ |W|^T) + |bias| < 2^24 u (u = the quantum of every product); returns u.  chunk: the e4m3
     wgmma chain of one 128-k chunk adds in the tensor core's reduced-precision accumulator (DESIGN.md §1), so each
-    chunk's sum is also kept under 2^13 u, an assumed width under which that adder is exact."""
+    chunk's sum is also kept under 2^13 u, an assumed width under which that adder is exact.  Above ANALYTIC_ABOVE
+    elements of M x N x KT the chunk sums are bounded by 128 max|X| max|W| instead of materialised."""
     u = lowbit(X) * lowbit(W)
     extra = float(bias_acc.abs().max()) if bias_acc is not None else 0.0
     top = float((X.abs() @ W.abs().t()).max()) + extra
     assert top < 2.0**24 * u, f"premise: sums reach {top / u:.0f} u >= 2^24 u"
-    if chunk:
+    if chunk and X.shape[0] * W.shape[0] * -(-X.shape[1] // 128) > ANALYTIC_ABOVE:
+        top_c = 128 * float(X.abs().max()) * float(W.abs().max())
+        assert top_c < 2.0**13 * u, f"premise: a 128-k chunk may reach {top_c / u:.0f} u >= 2^13 u"
+    elif chunk:
         K = X.shape[1]
         KT = -(-K // 128)
         Xp = torch.nn.functional.pad(X.abs(), (0, KT * 128 - K)).reshape(X.shape[0], KT, 128)
@@ -105,11 +109,13 @@ class Case:
     """One linear with exact operands at token count M_max.  run(M) launches it on the first M tokens; ref(M) is the
     expected output (bf16, or int32 for int8_mm_i32).  fmt / n_plan give the work split of tests/streamk_model.py."""
 
-    def __init__(self, op, fmt, M, N, K, n_plan, y64, launch, out_int=False):
+    def __init__(self, op, fmt, M, N, K, n_plan, y64, launch, out_int=False, ref=None):
         self.op, self.fmt, self.M, self.N, self.K, self.n_plan = op, fmt, M, N, K, n_plan
         self.launch = launch
         self.out_int = out_int
-        if out_int:
+        if ref is not None:   # already rounded (served(): built block by block)
+            self.ref_full = ref
+        elif out_int:
             self.ref_full = y64.to(torch.int32)
         else:
             fp32_exact(y64, f"{op}: the fp64 reference")   # so the cast below rounds once
@@ -128,23 +134,34 @@ class Case:
         self.bits(y).fill_(POISON_I32 if self.out_int else POISON_BF16)
 
 
-def build(op, M, N, K, seed=0, n_out=None, w_bytes=None):
+def int4_weights(n, K, group_size, g):
+    """n exact int4 weight rows: codes 0..15, s = ODD 2^-9, z = -24..24 2^-9.  Returns (W fp64 [n, K], qdata
+    [n/8, K/128, 32, 4], scale_and_zero bf16 [n, K/g, 2]); asserts that bf16(fma(q - 8, s, z)) is W itself."""
+    o = ops()
+    q = randint(0, 15, (n, K), g)
+    s = pick(ODD, (n, K // group_size), g) * 2.0**-9
+    z = randint(-24, 24, (n, K // group_size), g).double() * 2.0**-9
+    W = (q.double() - 8) * s.repeat_interleave(group_size, 1) + z.repeat_interleave(group_size, 1)
+    qdata = o.int4_pack_tile4d(((q[:, 0::2] << 4) | q[:, 1::2]).to(torch.uint8).contiguous(), 8)
+    sz = torch.stack([s, z], -1).to(torch.bfloat16)
+    assert torch.equal(o.int4_dequant_tile4d(qdata, sz.transpose(0, 1).contiguous(), group_size).double(), W), \
+        "premise: int4 weights not exact in bf16"
+    return W, qdata, sz
+
+
+def build(op, M, N, K, seed=0, n_out=None, w_bytes=None, group_size=64):
     """op: int4 | int8_dyn | int8_mm_i32 | fp8 | mxfp8 | nvfp4 | nvfp4w | nvfp4w_xs | nvfp4w_rowpts.
     n_out: int4 output features (<= N).  w_bytes: nvfp4 weight scale bytes [N, K/16] (default: a window of normal
-    bytes with mantissa bits set)."""
+    bytes with mantissa bits set).  group_size: int4 (32, 64, 128 or 256).  The value windows are fixed and the
+    premise is checked on the drawn values: for the test shapes (K <= 16384, M x N small); served() picks the windows
+    from K instead."""
     o = ops()
     g = gen(seed * 7919 + M * 31 + N * 7 + K)
     if op == "int4":
-        grp = 64
+        grp = group_size
         n_out = n_out or N
-        q = randint(0, 15, (N, K), g)
-        s = pick(ODD, (N, K // grp), g) * 2.0**-9
-        z = randint(-24, 24, (N, K // grp), g).double() * 2.0**-9
-        W = (q.double() - 8) * s.repeat_interleave(grp, 1) + z.repeat_interleave(grp, 1)
-        qdata = o.int4_pack_tile4d(((q[:, 0::2] << 4) | q[:, 1::2]).to(torch.uint8).contiguous(), 8)
-        sz = torch.stack([s, z], -1).to(torch.bfloat16).transpose(0, 1).contiguous()
-        # premise: bf16(fma(q - 8, s, z)) is exact, so the kernel's weights are W itself
-        assert torch.equal(o.int4_dequant_tile4d(qdata, sz, grp).double(), W), "premise: int4 weights not exact in bf16"
+        W, qdata, sz = int4_weights(N, K, grp, g)
+        sz = sz.transpose(0, 1).contiguous()
         X = randint(-8, 8, (M, K), g).double() * 2.0**-3
         x = X.to(torch.bfloat16)
         W = W[:n_out]
@@ -267,3 +284,309 @@ def first_mismatch(case, y, M=None):
 def sm_count():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
+
+
+# ------------------------------------------------------------------------------------------------ served shapes
+# At the shapes the library serves (K up to 28672, thousands of tokens, tens of thousands of features) the fixed
+# windows of build() are no longer exact by construction, and the checks that need M x N x KT or a whole fp64 weight
+# in memory do not fit.  served() draws from windows picked from K so that the analytic bound holds, checks the
+# premise block by block, and builds the fp64 reference W_BLOCK output features at a time.
+ANALYTIC_ABOVE = 1 << 26   # elements of M x N x KT above which the 128-k chunk sums are bounded, not materialised
+W_BLOCK = 4096             # output features per block of the fp64 reference
+BIAS_UNITS = 127 * 16      # bias_for(): |bias| <= 2032 output quanta
+I4_W = (2.0**-2, 2.0**-9)  # int4 W = (q - 8) s + z, s = ODD 2^-9, z = -24..24 2^-9: |W| <= 128 2^-9
+
+
+def span(values):
+    """(max |v|, the largest power of two that divides every v) of a set of exactly representable numbers."""
+    import math
+
+    low = None
+    for v in values:
+        if v == 0:
+            continue
+        m, e = math.frexp(abs(v))
+        mi = int(m * 2**53)
+        b = (mi & -mi) * 2.0 ** (e - 53)
+        low = b if low is None else min(low, b)
+    return max(abs(v) for v in values), low or 1.0
+
+
+def units(factors):
+    """max |product| / its quantum for a product of independent factors, each (max, quantum)."""
+    r = 1.0
+    for mx, low in factors:
+        r *= mx / low
+    return r
+
+
+def _codes(r, scale=1.0):
+    return [c * scale for c in range(-r, r + 1)]
+
+
+def _e4m3(byte):
+    s, e, m = byte >> 7, (byte >> 3) & 15, byte & 7
+    v = (m / 8.0) * 2.0**-6 if e == 0 else (1 + m / 8.0) * 2.0 ** (e - 7)
+    return -v if s else v
+
+
+E2M1_UPTO1 = [0, 1, 2, 8, 9, 10]   # codes of 0, +-0.5, +-1
+
+
+def served_candidates(op):
+    """The value windows of op in the order served() tries them: widest first.  Each is a dict of the value sets
+    (plain Python lists); factors() turns one into the (max, quantum) of X, W and the epilogue."""
+    if op == "int4":
+        return [dict(xr=r) for r in (8, 4, 2, 1)]
+    if op in ("int8_dyn", "int8_mm_i32"):
+        return [dict(r=r) for r in (127, 96, 63, 45, 34, 24, 16, 8)]
+    if op == "fp8":
+        return [dict(xr=a, wr=b, odd=[3, 5, 7]) for a, b in ((7, 7), (6, 6), (5, 4), (3, 3), (2, 2), (1, 1))]
+    if op == "mxfp8":
+        return [dict(dx=dx, dw=dw) for dx, dw in ((3, 3), (3, 2), (2, 2), (2, 1), (1, 1), (1, 0), (0, 0))]
+    if op == "nvfp4":
+        x4, x2 = list(range(0x38, 0x3C)), [0x38, 0x3C]
+        w4, w2 = list(range(0x30, 0x34)), [0x30, 0x34]
+        return [dict(xb=x4, wb=w4, pts=(0.75, 1.0)), dict(xb=x4, wb=w2, pts=(0.75, 0.5)),
+                dict(xb=x2, wb=w2, pts=(0.75, 0.5)), dict(xb=x2, wb=w2, pts=(0.5, 2.0))]
+    if op in ("nvfp4w", "nvfp4w_xs", "nvfp4w_rowpts"):
+        return [dict(xr=3, wb=list(range(0x30, 0x34)), odd=[3, 5, 7], bp=1.25),
+                dict(xr=1, wb=[0x30, 0x34], odd=[3, 5, 7], bp=1.25),
+                dict(xr=1, wb=[0x30, 0x34], odd=[3], bp=0.75)]
+    raise ValueError(op)
+
+
+def factors(op, win):
+    """(X factors, W factors, epilogue factors) of a window, each a list of (max, quantum)."""
+    if op == "int4":
+        return [span(_codes(win["xr"], 2.0**-3))], [I4_W], []
+    if op in ("int8_dyn", "int8_mm_i32"):
+        return [span(_codes(win["r"]))], [span(_codes(win["r"]))], []
+    if op == "fp8":
+        sc = [o * 2.0**-8 for o in win["odd"]]
+        return ([span(_codes(win["xr"], 0.25))], [span(_codes(win["wr"], 0.125))],
+                [span(sc), span([v * 2.0**-1 for v in sc])])
+    if op == "mxfp8":
+        return ([span(_codes(7, 0.25)), span([2.0**e for e in range(-2, -2 + win["dx"] + 1)])],
+                [span(_codes(7, 0.125)), span([2.0**e for e in range(-3, -3 + win["dw"] + 1)])], [])
+    if op == "nvfp4":
+        return ([span([E2M1[c] for c in E2M1_UPTO1]), span([_e4m3(b) for b in win["xb"]])],
+                [span(E2M1), span([_e4m3(b) for b in win["wb"]])], [span([win["pts"][0]]), span([win["pts"][1]])])
+    if op in ("nvfp4w", "nvfp4w_xs", "nvfp4w_rowpts"):
+        epi = [] if op == "nvfp4w" else [span([o * 2.0**-6 for o in win["odd"]])]
+        epi.append(span([o * 2.0**-4 for o in win["odd"]]) if op == "nvfp4w_rowpts" else span([win["bp"]]))
+        return [span(_codes(win["xr"], 0.5))], [span(E2M1), span([_e4m3(b) for b in win["wb"]])], epi
+    raise ValueError(op)
+
+
+def bound(op, K, win):
+    """(sum bound, chunk bound or None) in output quanta: K max|X| max|W| (times the epilogue's scales) plus the bias,
+    and 128 max|X| max|W| for the e4m3 chunk.  Exact when the first is < 2^24 and the second < 2^13."""
+    xf, wf, ef = factors(op, win)
+    xw = units(xf) * units(wf)
+    if op in ("int8_dyn", "int8_mm_i32"):
+        return K * xw, None   # the int32 sum converts to fp32 exactly; the epilogue rounds as the reference does
+    return K * xw * units(ef) + BIAS_UNITS, (128 * xw if op == "fp8" else None)
+
+
+def exact(op, K, win):
+    s, c = bound(op, K, win)
+    return s < 2.0**24 and (c is None or c < 2.0**13)
+
+
+def window(op, K):
+    """The widest window of op that is exact at K."""
+    for win in served_candidates(op):
+        if exact(op, K, win):
+            return win
+    raise AssertionError(f"premise: no window of {op} is exact at K={K}")
+
+
+def _quantum(fs):
+    q = 1.0
+    for _, low in fs:
+        q *= low
+    return q
+
+
+def _reference(op, X, n, wblock, epi, chunk):
+    """The bf16 (int32) reference [M, n], W_BLOCK features at a time: wblock(n0, n1) -> fp64 W rows; epi(acc, n0, n1)
+    -> fp64 output.  The premise is checked on the drawn values of each block as well."""
+    M = X.shape[0]
+    ref = torch.empty(M, n, dtype=torch.int32 if op == "int8_mm_i32" else torch.bfloat16, device=DEV)
+    for n0 in range(0, n, W_BLOCK):
+        n1 = min(n, n0 + W_BLOCK)
+        W = wblock(n0, n1)
+        premise(X, W, chunk=chunk)
+        y = epi(X @ W.t(), n0, n1)
+        del W
+        if op == "int8_mm_i32":
+            ref[:, n0:n1] = y.to(torch.int32)
+        else:
+            fp32_exact(y, f"{op}: the fp64 reference")
+            ref[:, n0:n1] = y.float().to(torch.bfloat16)
+    return ref
+
+
+def served(op, M, N, K, seed=0, group_size=32, n_out=None, x_seed=None):
+    """A Case of op at a served shape: windows from window(op, K), weights drawn and packed W_BLOCK rows at a time,
+    the fp64 reference built per block (no whole fp64 weight is ever resident).  x_seed: other activations (and
+    activation scales and bias) with the same weights; case.inputs lists those tensors in a fixed order, so a CUDA
+    graph captured on one case can be replayed on another's inputs copied into them."""
+    o = ops()
+    win = window(op, K)
+    xf, wf, ef = factors(op, win)
+    Q = _quantum(xf) * _quantum(wf) * _quantum(ef)   # the output quantum: the bias is a multiple of it
+    gx = gen((seed if x_seed is None else 1000003 + x_seed) * 7919 + M * 31 + N * 7 + K)
+    gw = gen(seed * 7919 + N * 7 + K + 1)
+    parts = []
+
+    def blocks(n, make):
+        """Runs make(n0, n1) for every block once, in order (the weight generator is sequential)."""
+        def wblock(n0, n1):
+            W, packed = make(n1 - n0)
+            parts.append(packed)
+            return W
+        return wblock
+
+    if op == "int4":
+        g = group_size
+        n_out = n_out or N
+        X = randint(-win["xr"], win["xr"], (M, K), gx).double() * 2.0**-3
+        bias = bias_for(N, Q, gx)
+
+        def make(nb):
+            W, qd, sz = int4_weights(nb, K, g, gw)
+            return W, (qd, sz)
+        # every one of the N packed rows is drawn; the rows past n_out are computed by the tail tile and not stored
+        ref = _reference(op, X, N, blocks(N, make), lambda acc, n0, n1: acc + bias[n0:n1], False)[:, :n_out].contiguous()
+        qdata = torch.cat([p[0] for p in parts], 0).contiguous()
+        sz = torch.cat([p[1] for p in parts], 0).transpose(0, 1).contiguous()
+        x, b = X.to(torch.bfloat16), bias[:n_out].to(torch.bfloat16)
+        c = Case(op, "int4", M, N, K, n_out, None, lambda m: o.int4_tilepacked_linear(x[:m], qdata, g, sz, b, n_out, 1),
+                 ref=ref)
+        c.inputs = [x, b]
+        return c
+    if op in ("int8_dyn", "int8_mm_i32"):
+        r = win["r"]
+        xq = randint(-r, r, (M, K), gx).to(torch.int8)
+        sx = (pick(ODD, (M, 1), gx) * 2.0**-14).float()
+        sw = (pick(ODD, (N,), gw) * 2.0**-10).float()
+        b = (randint(-127, 127, (N,), gx).double() * 2.0**-8).to(torch.bfloat16)
+
+        def make(nb):
+            wq = randint(-r, r, (nb, K), gw).to(torch.int8)
+            return wq.double(), wq
+
+        def epi(acc, n0, n1):
+            assert float(acc.abs().max()) < 2.0**24, "premise: int32 sums must convert to fp32 exactly"
+            if op == "int8_mm_i32":
+                return acc
+            t = (acc.float() * sx).to(torch.bfloat16).float()   # the reference's order: bf16 between the two scales
+            fp32_exact(t.double() * sw[n0:n1].double(), "int8: bf16(acc * x_scale) * w_scale")
+            return (t * sw[n0:n1] + b[n0:n1].float()).double()
+        ref = _reference(op, xq.double(), N, blocks(N, make), epi, False)
+        wq = torch.cat(parts, 0)
+        if op == "int8_mm_i32":
+            c = Case(op, "int8", M, N, K, N, None, lambda m: o.int8_mm_i32(xq[:m], wq), out_int=True, ref=ref)
+        else:
+            c = Case(op, "int8", M, N, K, N, None, lambda m: o.int8_dyn_linear(xq[:m], sx[:m], wq, sw, b), ref=ref)
+        c.inputs = [xq, sx, b]
+        return c
+    if op == "fp8":
+        X = randint(-win["xr"], win["xr"], (M, K), gx).double() * 2.0**-2
+        rs = pick(win["odd"], (M,), gx) * 2.0**-8
+        sw = pick(win["odd"], (N,), gw) * 2.0**-9
+        bias = bias_for(N, Q, gx)
+
+        def make(nb):
+            W = randint(-win["wr"], win["wr"], (nb, K), gw).double() * 2.0**-3
+            return W, W.to(torch.float8_e4m3fn)
+
+        def epi(acc, n0, n1):
+            sc = rs[:, None] * sw[None, n0:n1]
+            fp32_exact(sc, "fp8: x_scale * w_scale")
+            prod = acc * sc
+            fp32_exact(prod, "fp8: acc * scales")
+            return prod + bias[n0:n1]
+        ref = _reference(op, X, N, blocks(N, make), epi, True)
+        xq, wq = X.to(torch.float8_e4m3fn), torch.cat(parts, 0)
+        rsf, swf, b = rs.float(), sw.float(), bias.to(torch.bfloat16)
+        c = Case(op, "fp8", M, N, K, N, None, lambda m: o.fp8_rowwise_linear(xq[:m], rsf[:m], wq, swf, b), ref=ref)
+        c.inputs = [xq, rsf, b]
+        return c
+    if op == "mxfp8":
+        Xc = randint(-7, 7, (M, K), gx).double() * 2.0**-2
+        xb = randint(125, 125 + win["dx"], (M, K // 32), gx)
+        X = Xc * pow2(xb - 127).repeat_interleave(32, 1)
+        bias = bias_for(N, Q, gx)
+
+        def make(nb):
+            Wc = randint(-7, 7, (nb, K), gw).double() * 2.0**-3
+            wb = randint(124, 124 + win["dw"], (nb, K // 32), gw)
+            return Wc * pow2(wb - 127).repeat_interleave(32, 1), (Wc.to(torch.float8_e4m3fn), wb.to(torch.uint8))
+        ref = _reference(op, X, N, blocks(N, make), lambda acc, n0, n1: acc + bias[n0:n1], False)
+        xq, wq = Xc.to(torch.float8_e4m3fn), torch.cat([p[0] for p in parts], 0)
+        xsb, wsb = to_blocked(xb.to(torch.uint8)), to_blocked(torch.cat([p[1] for p in parts], 0))
+        b = bias.to(torch.bfloat16)
+        cache = {}
+
+        def run(m):
+            if m not in cache:
+                cache[m] = to_blocked(xb[:m].to(torch.uint8))
+            return o.mxfp8_linear(xq[:m], cache[m], wq, wsb, b)
+        return Case(op, "mxfp8", M, N, K, N, None, run, ref=ref)
+    if op == "nvfp4":
+        xc = pick(E2M1_UPTO1, (M, K), gx).long()
+        xbytes = pick(win["xb"], (M, K // 16), gx).to(torch.uint8)
+        X = e2m1_value(xc) * e4m3_bytes_value(xbytes).repeat_interleave(16, 1)
+        a, bp = win["pts"]
+        bias = bias_for(N, Q, gx)
+
+        def make(nb):
+            wc = randint(0, 15, (nb, K), gw)
+            wbytes = pick(win["wb"], (nb, K // 16), gw).to(torch.uint8)
+            return e2m1_value(wc) * e4m3_bytes_value(wbytes).repeat_interleave(16, 1), (pack_e2m1(wc), wbytes)
+
+        def epi(acc, n0, n1):
+            prod = acc * (a * bp)
+            fp32_exact(prod, "nvfp4: acc * a_pts * b_pts")
+            return prod + bias[n0:n1]
+        ref = _reference(op, X, N, blocks(N, make), epi, False)
+        xq, wq = pack_e2m1(xc), torch.cat([p[0] for p in parts], 0)
+        wsb = to_blocked(torch.cat([p[1] for p in parts], 0))
+        a_pts, b_pts = torch.tensor([a], device=DEV), torch.tensor([bp], device=DEV)
+        b = bias.to(torch.bfloat16)
+        cache = {}
+
+        def run(m):
+            if m not in cache:
+                cache[m] = to_blocked(xbytes[:m])
+            return o.nvfp4_linear(xq[:m], cache[m], a_pts, wq, wsb, b_pts, b)
+        return Case(op, "nvfp4", M, N, K, N, None, run, ref=ref)
+    if op in ("nvfp4w", "nvfp4w_xs", "nvfp4w_rowpts"):
+        X = randint(-win["xr"], win["xr"], (M, K), gx).double() * 0.5
+        rs = pick(win["odd"], (M,), gx) * 2.0**-6 if op != "nvfp4w" else None
+        bp = (pick(win["odd"], (N,), gw) * 2.0**-4 if op == "nvfp4w_rowpts"
+              else torch.tensor([win["bp"]], dtype=torch.float64, device=DEV))
+        bias = bias_for(N, Q, gx)
+
+        def make(nb):
+            wc = randint(0, 15, (nb, K), gw)
+            wbytes = pick(win["wb"], (nb, K // 16), gw).to(torch.uint8)
+            return e2m1_value(wc) * e4m3_bytes_value(wbytes).repeat_interleave(16, 1), (pack_e2m1(wc), wbytes)
+
+        def epi(acc, n0, n1):
+            if rs is not None:
+                acc = acc * rs[:, None]
+                fp32_exact(acc, "nvfp4w: acc * x_scale")
+            prod = acc * (bp[n0:n1] if bp.numel() > 1 else bp).reshape(1, -1)
+            fp32_exact(prod, "nvfp4w: acc * b_pts")
+            return prod + bias[n0:n1]
+        ref = _reference(op, X, N, blocks(N, make), epi, False)
+        x, wq = X.to(torch.bfloat16), torch.cat([p[0] for p in parts], 0)
+        wsb = to_blocked(torch.cat([p[1] for p in parts], 0))
+        rsf, bpf, b = (rs.float() if rs is not None else None), bp.float(), bias.to(torch.bfloat16)
+        return Case(op, "nvfp4", M, N, K, N, None,
+                    lambda m: o.nvfp4_weight_linear(x[:m], rsf[:m] if rsf is not None else None, wq, wsb, bpf, b), ref=ref)
+    raise ValueError(op)

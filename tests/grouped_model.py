@@ -12,6 +12,15 @@ MAX_EXPERTS = 1024
 MIN_UNITS = 4
 
 
+def cumulative(rows):
+    """offs of torch._grouped_mm from the rows of each expert: the cumulative row ends."""
+    out, s = [], 0
+    for r in rows:
+        s += r
+        out.append(s)
+    return out
+
+
 def row_ends(offs, M):
     """end[e] = min(M, max(0, offs[0..e])): every offs[e] clamped into [end[e-1], M]."""
     ends, run = [], 0
