@@ -4,6 +4,7 @@
 //   mxfp8 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm block-scaled
 //   nvfp4 block-16 e4m3   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm fp4 + pts/bias kernels
 //   nvfp4 weight x bf16   (bf16 wgmma, weights dequantised exactly)      replaces F.linear on the dequantised weight
+//   mxfp4 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces F.linear on both dequantize()s
 // Reference call sites: int8/kernels.py:18-76,114-144 + int8_tensor.py:305-359;
 // float8/inference.py:86-123; mx_formats/mx_tensor.py:759-843; nvfp4_tensor.py:487-578.
 //
@@ -14,6 +15,9 @@
 // same products a block-scaled MMA sees, as long as the scaled element is exact in bf16:
 //   * e2m1 x e4m3 (at most 6 significant bits, >= 2^-10): exact for every finite non-negative scale byte, the
 //     subnormal and zero bytes included (nvfp4_fmt.cuh);
+//   * e2m1 x 2^(e-127) (at most 2 significant bits, every code a multiple of 2^-1): exact for every e8m0 byte
+//     0x00..0xFE, the smallest product 2^-128 being a bf16 subnormal; the products at or above 2^128 (|code| >= 4 at
+//     byte 253, |code| >= 2 at byte 254) are inf, as in the reference's fp32 dequantize, and byte 0xFF is NaN;
 //   * e4m3 x 2^(e-127) (4 significant bits, every code a multiple of 2^-9): exact for e8m0 bytes e >= 3.  For
 //     e = 0, 1, 2 the codes whose lowest set bit lies below 2^-(6+e) need bits under 2^-133, the smallest bf16
 //     subnormal, and round.
@@ -32,7 +36,7 @@
 namespace ao {
 namespace lowp {
 
-enum Kind { KIND_I8 = 0, KIND_F8 = 1, KIND_MXF8 = 2, KIND_NVF4 = 3 };
+enum Kind { KIND_I8 = 0, KIND_F8 = 1, KIND_MXF8 = 2, KIND_NVF4 = 3, KIND_MXF4 = 4 };
 
 using tsg::KCHUNK;
 using tsg::ROWS;
@@ -89,6 +93,15 @@ struct SsFmt {
   }
 };
 
+// the blocked e8m0 scales of block-32 weights W[N][K] as a 2-D tensor of 128 words x 512-byte tiles, one tile (4
+// scales x 128 rows = 128 k) per box
+static int e8m0_tile_map(const uint8_t* w_sf, int N, int K, CUtensorMap* tm_sf) {
+  const uint64_t dims[2] = {128, (uint64_t)ceil_div(N, ROWS) * (uint64_t)ceil_div(K / 32, 4)};
+  const uint64_t str[1] = {512};
+  const uint32_t box[2] = {128, 1};
+  return make_tmap(tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+}
+
 // 2^(e - 127) for an e8m0 byte (0xFF = NaN)
 __device__ __forceinline__ float e8m0_to_f32(uint32_t e) {
   return __uint_as_float(e == 0xFFu ? 0x7FC00000u : (e ? e << 23 : 0x00400000u));
@@ -109,10 +122,7 @@ struct Mxfp8Fmt {
   // the weights and the blocked scale tiles, one 512-byte tile per box
   static int make_maps(const uint8_t* wq, const uint8_t* w_sf, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
     if (int rc = kmajor_byte_map(wq, N, K, tm_w)) return rc;
-    const uint64_t dims[2] = {128, (uint64_t)ceil_div(N, ROWS) * (uint64_t)ceil_div(K / 32, 4)};
-    const uint64_t str[1] = {512};
-    const uint32_t box[2] = {128, 1};
-    return make_tmap(tm_sf, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, w_sf, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+    return e8m0_tile_map(w_sf, N, K, tm_sf);
   }
   __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES + AUX_BYTES; }
   __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap* tm_sf, const tsg::Params& p,
@@ -156,6 +166,88 @@ struct Mxfp8Fmt {
   }
 };
 
+// mxfp4 weights as the register-A operand: packed e2m1 pairs (the stored [N, K/2] qdata, even k in the low nibble,
+// loaded as nvf4w::Nvfp4Fmt loads them) x their block-32 e8m0 scale (one blocked tile per chunk, as Mxfp8Fmt) -> bf16.
+// A nibble placed at bf16 bits 15|8:6 is value * 2^-126 (Nvfp4Fmt::deq); one exact multiply by 2^126 gives the value and
+// a second one by the bf16 scale 2^(e-127) the element, exact for every byte (see the top of this file): the e8m0
+// range is the bf16 exponent range, 2^-127 a bf16 subnormal, and bf16 multiplies keep subnormals.  The scales are
+// decoded once per chunk; the thread keeps only the 16 code bytes of its two fragment rows that its steps read.
+struct Mxfp4Fmt {
+  static constexpr bool SS = false;
+  // at 80 registers (two CTAs per SM) the N_MMA = 32 decode tile keeps 8 bytes of stack, a spill and refill in every
+  // chunk: one CTA per SM, as mxfp8 and nvfp4 (DESIGN.md, mxfp4)
+  static constexpr bool DECODE_2CTA = false;
+  static constexpr bool PROMOTE = false;
+  static constexpr int X_ELEM_BYTES = 2;
+  static constexpr int W_BYTES = ROWS * KCHUNK / 2;   // 128 rows x 64 bytes, 64-byte swizzle
+  static constexpr int AUX_BYTES = 512;               // one blocked scale tile (4 scales = 128 k per row)
+  static constexpr int EPI = tsg::EPI_FLOAT;
+  static constexpr int ACC_EXP2 = 0;
+  static constexpr int MAX_N_MMA = 128;
+  static int make_maps(const uint8_t* wq, const uint8_t* w_sf, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
+    const uint64_t dims[2] = {(uint64_t)K / 2, (uint64_t)N};
+    const uint64_t str[1] = {(uint64_t)K / 2};
+    const uint32_t box[2] = {64, 128};
+    if (int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B))
+      return rc;
+    return e8m0_tile_map(w_sf, N, K, tm_sf);
+  }
+  __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES + AUX_BYTES; }
+  __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap* tm_sf, const tsg::Params& p,
+                                                 uint8_t* w_dst, uint8_t* aux_dst, uint64_t* bar, int n_tile, int kc,
+                                                 uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * 64, n_tile * ROWS, policy);
+    tma_load_2d(aux_dst, tm_sf, bar, 0, n_tile * p.aux_col_blocks + kc, policy);
+  }
+  // c[h][j]: row h's code bytes of k16 steps 2j, 2j + 1 (step kk reads byte t of bytes 8kk..8kk+3, the k pair
+  // 16kk + 2t, and byte t of 8kk+4..8kk+7, the pair 8 further), as bytes (2j lo, 2j hi, 2j+1 lo, 2j+1 hi);
+  // s[h][i]: bf16x2 of the scales of 32-k blocks 2i, 2i + 1
+  struct Raw {
+    uint32_t c[2][4];
+    uint32_t s[2][2];
+  };
+  __device__ static __forceinline__ void load(const tsg::Params&, uint32_t w_smem, uint32_t aux_smem, int row_lo, int lane,
+                                              Raw& raw) {
+    const uint32_t t = lane & 3;
+    const uint32_t sel = t | (t + 4) << 4 | t << 8 | (t + 4) << 12;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row_lo + 8 * h;
+      const uint32_t sc = tsg::lds32(aux_smem + (uint32_t)(r & 31) * 16u + (uint32_t)(r >> 5) * 4u);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const __nv_bfloat162 s2 = __floats2bfloat162_rn(e8m0_to_f32((sc >> (16 * i)) & 0xFFu),
+                                                        e8m0_to_f32((sc >> (16 * i + 8)) & 0xFFu));
+        raw.s[h][i] = *reinterpret_cast<const uint32_t*>(&s2);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t off = (uint32_t)r * 64u + j * 16;
+        const uint4 v = tsg::lds128(w_smem + (off ^ (((off >> 7) & 3) << 4)));   // undo the TMA 64B swizzle
+        raw.c[h][j] = __byte_perm(__byte_perm(v.x, v.y, sel), __byte_perm(v.z, v.w, sel), 0x5410);
+      }
+    }
+  }
+  __device__ static __forceinline__ uint32_t deq(uint32_t byte, __nv_bfloat162 s2) {
+    const uint32_t hh = (byte | (byte << 12)) & 0x000F000Fu;   // even k nibble at bits 3:0, odd k at 19:16
+    const uint32_t bits = (hh * 0x1040u) & 0x81C081C0u;         // sign | e1 e0 m at bf16 bits 15 | 8:6 = value * 2^-126
+    __nv_bfloat162 x = *reinterpret_cast<const __nv_bfloat162*>(&bits);
+    x = __hmul2(__hmul2(x, __nv_bfloat162(__ushort_as_bfloat16(0x7E80), __ushort_as_bfloat16(0x7E80))), s2);   // * 2^126
+    return *reinterpret_cast<uint32_t*>(&x);
+  }
+  __device__ static __forceinline__ void frag(const tsg::Params&, const Raw& raw, int kk, uint32_t (&a)[4]) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      // the scale of the 32-k block of step kk, in both halves
+      const uint32_t s_bits = __byte_perm(raw.s[h][kk >> 2], 0u, ((kk >> 1) & 1) ? 0x3232u : 0x1010u);
+      const __nv_bfloat162 s2 = *reinterpret_cast<const __nv_bfloat162*>(&s_bits);
+      const uint32_t cw = raw.c[h][kk >> 1] >> (16 * (kk & 1));
+      a[h] = deq(cw & 0xFFu, s2);
+      a[h + 2] = deq((cw >> 8) & 0xFFu, s2);
+    }
+  }
+};
+
 // Activation pre-pass of the block-scaled kinds: rows [m0, m0 + rows) of the quantised activations -> bf16 [rows][K],
 // every element times its block scale (exact in bf16).  One thread per 16 elements.
 template <int KIND>
@@ -172,9 +264,14 @@ __global__ void __launch_bounds__(256) dequant_act_kernel(const uint8_t* __restr
   const size_t tile = (size_t)(m / 128) * sf_col_blocks + kb / 4;
   const uint32_t sbyte = x_sf[tile * 512 + (m % 32) * 16 + ((m % 128) / 32) * 4 + kb % 4];
   __nv_bfloat16 o[16];
-  if (KIND == KIND_NVF4) {
-    const __half_raw sh = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)sbyte, __NV_E4M3);
-    const float s = __half2float(*reinterpret_cast<const __half*>(&sh));
+  if (KIND == KIND_NVF4 || KIND == KIND_MXF4) {
+    float s;
+    if (KIND == KIND_NVF4) {
+      const __half_raw sh = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)sbyte, __NV_E4M3);
+      s = __half2float(*reinterpret_cast<const __half*>(&sh));
+    } else {
+      s = e8m0_to_f32(sbyte);   // code x 2^(e-127) is exact in fp32 (subnormals kept) and then in bf16
+    }
     const uint2 v = *reinterpret_cast<const uint2*>(xq + (size_t)m * (K / 2) + k0 / 2);
     const float lut[8] = {0.f, 0.5f, 1.f, 1.5f, 2.f, 3.f, 4.f, 6.f};
 #pragma unroll
@@ -222,9 +319,10 @@ template <int KIND>
 static int block_scaled(const uint8_t* xq, const uint8_t* x_sf, const float* a_pts, int M, int K, const uint8_t* wq,
                         const uint8_t* w_sf, const float* b_pts, int N, const uint16_t* bias, uint16_t* y, void* ws,
                         size_t ws_bytes, void* stream) {
-  using Fmt = std::conditional_t<KIND == KIND_NVF4, nvf4w::Nvfp4Fmt, Mxfp8Fmt>;
+  using Fmt = std::conditional_t<KIND == KIND_NVF4, nvf4w::Nvfp4Fmt,
+                                 std::conditional_t<KIND == KIND_MXF4, Mxfp4Fmt, Mxfp8Fmt>>;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int sf_per_row = KIND == KIND_MXF8 ? K / 32 : K / 16;
+  const int sf_per_row = KIND == KIND_NVF4 ? K / 16 : K / 32;
   const int sf_col_blocks = ceil_div(sf_per_row, 4);
   CUtensorMap tm_w, tm_sf;
   if (int rc = Fmt::make_maps(wq, w_sf, N, K, &tm_w, &tm_sf)) return rc;
@@ -333,6 +431,19 @@ extern "C" int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked
   if (M == 0) return AO_OK;
   AO_REQUIRE(xq && x_scale_blocked && wq && w_scale_blocked && y, "mxfp8 linear: null pointer");
   return lowp::block_scaled<lowp::KIND_MXF8>(xq, x_scale_blocked, nullptr, M, K, wq, w_scale_blocked, nullptr, N, bias,
+                                             y, workspace, workspace_bytes, stream);
+}
+
+extern "C" int ao_mxfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,
+                               const uint8_t* wq, const uint8_t* w_scale_blocked, int N,
+                               const uint16_t* bias, uint16_t* y, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "mxfp4 linear: bad sizes M=%d K=%d N=%d", M, K, N);
+  // K / 2 bytes per weight row: a multiple of 16, the TMA row pitch; a K tail of the last chunk is zero-filled
+  AO_REQUIRE(K % 32 == 0, "mxfp4 linear: K=%d must be a multiple of 32 (mx_tensor.py:244-246)", K);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(xq && x_scale_blocked && wq && w_scale_blocked && y, "mxfp4 linear: null pointer");
+  return lowp::block_scaled<lowp::KIND_MXF4>(xq, x_scale_blocked, nullptr, M, K, wq, w_scale_blocked, nullptr, N, bias,
                                              y, workspace, workspace_bytes, stream);
 }
 

@@ -41,6 +41,13 @@ class MXDynamicActivationMXWeightConfig(AOBaseConfig):
 
     def __post_init__(self):
         assert self.activation_dtype == self.weight_dtype, "For now - we only support matching input/weight dtypes."
+        if self.weight_dtype not in (torch.float8_e4m3fn, torch.float4_e2m1fn_x2):
+            raise NotImplementedError(f"MX element dtype {self.weight_dtype}: only torch.float8_e4m3fn (mxfp8) and "
+                                      f"torch.float4_e2m1fn_x2 (mxfp4) are implemented")
+        if self.block_size != 32:
+            raise NotImplementedError(f"MX block_size={self.block_size}: only 32 is implemented")
+        if self.scaling_mode != ScaleCalculationMode.RCEIL:
+            raise NotImplementedError(f"MX scaling_mode={self.scaling_mode}: only ScaleCalculationMode.RCEIL is implemented")
 
 
 @register_quantize_module_handler(MXDynamicActivationMXWeightConfig)

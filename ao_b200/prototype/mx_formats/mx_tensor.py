@@ -1,10 +1,14 @@
-"""MXFP8 weight/activation tensor on Hopper wgmma (bf16, exactly dequantised operands).
+"""MXFP8 / MXFP4 weight/activation tensor on Hopper wgmma (bf16, exactly dequantised operands).
 
 Attribute names/order match torchao's MXTensor (torchao/prototype/mx_formats/mx_tensor.py:509-517):
 ``qdata, scale | elem_dtype, block_size, orig_dtype, kernel_preference, act_quant_kwargs,
 is_swizzled_scales``.  ``to_mx`` (e4m3, block 32, RCEIL) runs the fused CUDA quantizer
 (bit-exact with the reference's torch ops, tests/test_oracle_golden.py + test_lowp_gpu.py);
 the linear replaces ``mx_linear -> _addmm_mx_dispatch -> torch._scaled_mm`` (:759-882).
+
+With ``elem_dtype=torch.float4_e2m1fn_x2`` (mxfp4) ``qdata`` is uint8 ``[..., K/2]``, two e2m1 codes per byte with
+the even k in the low nibble, and the tensor's shape is the high-precision one (``K = 2 * qdata.shape[-1]``), as in
+the reference (:530-540).  ``to_mx`` runs ``mxfp4_quantize`` and the linear ``mxfp4_linear``.
 """
 from __future__ import annotations
 
@@ -52,7 +56,10 @@ class MXTensor(TorchAOBaseTensor):
 
     def __new__(cls, qdata, scale, elem_dtype, block_size, orig_dtype, kernel_preference, act_quant_kwargs,
                 is_swizzled_scales):
-        return torch.Tensor._make_wrapper_subclass(cls, qdata.shape, dtype=orig_dtype, device=qdata.device,
+        shape = qdata.shape
+        if elem_dtype == torch.float4_e2m1fn_x2:
+            shape = (*shape[:-1], shape[-1] * 2)   # two codes per byte: the high-precision shape
+        return torch.Tensor._make_wrapper_subclass(cls, shape, dtype=orig_dtype, device=qdata.device,
                                                    requires_grad=False)
 
     def __init__(self, qdata, scale, elem_dtype, block_size, orig_dtype, kernel_preference, act_quant_kwargs,
@@ -82,14 +89,19 @@ class MXTensor(TorchAOBaseTensor):
         # contiguous like the reference requires (mx_tensor.py:247), or a 2-D column slice (rows with a pitch): the
         # quantizer kernel takes the pitch, no copy
         assert data_hp.is_contiguous() or rows_for_kernel(data_hp) is data_hp, "unsupported"
-        if elem_dtype != torch.float8_e4m3fn or block_size != 32:
-            raise NotImplementedError("only mxfp8 (e4m3, block 32) is implemented (north-star formats)")
+        if elem_dtype not in (torch.float8_e4m3fn, torch.float4_e2m1fn_x2) or block_size != 32:
+            raise NotImplementedError(f"only mxfp8 and mxfp4 (float8_e4m3fn / float4_e2m1fn_x2, block 32) are "
+                                      f"implemented, got {elem_dtype} with block {block_size}")
         if scaling_mode != ScaleCalculationMode.RCEIL:
             raise NotImplementedError("only ScaleCalculationMode.RCEIL (the inference default) is implemented")
         lead, K = data_hp.shape[:-1], data_hp.shape[-1]
         x2 = data_hp.reshape(-1, K)
-        q, s = torch.ops.ao_b200.mxfp8_quantize(x2, is_swizzled_scales)
-        q = q.reshape(*lead, K)
+        if elem_dtype == torch.float4_e2m1fn_x2:
+            q, s = torch.ops.ao_b200.mxfp4_quantize(x2, is_swizzled_scales)
+            q = q.reshape(*lead, K // 2)
+        else:
+            q, s = torch.ops.ao_b200.mxfp8_quantize(x2, is_swizzled_scales)
+            q = q.reshape(*lead, K)
         s = s.view(torch.float8_e8m0fnu)
         if not is_swizzled_scales:
             s = s.reshape(*lead, K // block_size)
@@ -98,16 +110,26 @@ class MXTensor(TorchAOBaseTensor):
 
     def dequantize(self, output_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
         out = output_dtype or self.orig_dtype
-        K = self.qdata.shape[-1]
-        rows = self.qdata.numel() // K
+        K = self.shape[-1]
+        rows = self.qdata.numel() // self.qdata.shape[-1]
         s = self.scale.view(torch.uint8)
         if self.is_swizzled_scales:
             s = from_blocked(s.reshape(-1), rows, K // self.block_size)
         s = s.reshape(rows, K // self.block_size)
         e = torch.pow(2.0, s.to(torch.float32) - 127.0)
         e = torch.where(s == 255, torch.full_like(e, float("nan")), e)
-        v = self.qdata.reshape(rows, K).to(torch.float32) * e.repeat_interleave(self.block_size, dim=1)
-        return v.reshape(self.qdata.shape).to(out)
+        if self.elem_dtype == torch.float4_e2m1fn_x2:
+            q = self.qdata.view(torch.uint8).reshape(rows, K // 2)
+            c = torch.stack([q & 15, q >> 4], dim=-1).reshape(rows, K).to(torch.int32)   # even k in the low nibble
+            ce, cm = (c >> 1) & 3, (c & 1).to(torch.float32)
+            # e2m1 (s e1 e0 m): m / 2 for e = 0, else 2^(e-1) * (1 + m / 2); no host table, so it can be graph-captured
+            p2 = torch.bitwise_left_shift(torch.ones_like(ce), (ce - 1).clamp(min=0)).to(torch.float32)
+            v = torch.where(ce == 0, 0.5 * cm, p2 * (1.0 + 0.5 * cm))
+            v = torch.where((c & 8) != 0, -v, v)
+        else:
+            v = self.qdata.reshape(rows, K).to(torch.float32)
+        v = v * e.repeat_interleave(self.block_size, dim=1)
+        return v.reshape(self.shape).to(out)
 
 
 implements = MXTensor.implements
@@ -130,7 +152,8 @@ def _(func, types, args, kwargs):
         return x.new_empty(*orig_shape[:-1], N)
     xq = MXTensor.to_mx(rows_for_kernel(x2.to(torch.bfloat16)), k.elem_dtype, k.block_size, k.scaling_mode,
                         k.kernel_preference, None, True)
-    y = torch.ops.ao_b200.mxfp8_linear(xq.qdata, xq.scale.view(torch.uint8), w.qdata, w.scale.view(torch.uint8), bias)
+    mm = torch.ops.ao_b200.mxfp4_linear if w.elem_dtype == torch.float4_e2m1fn_x2 else torch.ops.ao_b200.mxfp8_linear
+    y = mm(xq.qdata, xq.scale.view(torch.uint8), w.qdata, w.scale.view(torch.uint8), bias)
     return y.reshape(*orig_shape[:-1], N).to(x.dtype)
 
 

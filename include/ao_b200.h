@@ -182,6 +182,23 @@ int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, in
                     const uint16_t* bias, uint16_t* y, void* workspace,
                     size_t workspace_bytes, void* stream);
 
+/* mxfp4 (e2m1 data, e8m0 block-32 scales) --------------------------------------- */
+/* Replaces MXTensor.to_mx(x, float4_e2m1fn_x2, 32, RCEIL, is_swizzled_scales) for activations
+ * (mx_tensor.py:228-409, :161-225): per 32-element block e8 = rceil(amax * f32(1/6)) (0xFF for inf / NaN),
+ * codes e2m1(x * 2^(127-e8)) rounded to nearest even and saturated at 6.  x bf16 [M,K] -> q uint8 [M,K/2]
+ * (even k in the LOW nibble), scales e8m0 bytes, plain [M][K/32] or (swizzled=1) blocked as for mxfp8 with the
+ * padding written as zero.  K % 32 == 0.                                                                     */
+int ao_mxfp4_quantize(const uint16_t* x, int M, int K, uint8_t* q, uint8_t* scale_e8m0,
+                      int swizzled, void* stream);
+/* y = bf16( sum_k xhat[m,k] * what[n,k] (fp32) + bias ), xhat / what = each operand's code x 2^(e8-127), the
+ * MXTensor.dequantize() of both (exact in bf16 for every scale byte: the products of the block-scaled fp4 MMA).
+ * xq uint8 [M,K/2], wq uint8 [N,K/2], both scale tensors in the blocked layout with zero padding.  K % 32 == 0
+ * (a K tail of the last 128-k chunk is zero-filled), any N.                                                  */
+int ao_mxfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,
+                    const uint8_t* wq, const uint8_t* w_scale_blocked, int N,
+                    const uint16_t* bias, uint16_t* y, void* workspace,
+                    size_t workspace_bytes, void* stream);
+
 /* nvfp4 (e2m1 data, e4m3 block-16 scales, f32 per-tensor scale) ------------------ */
 /* Replaces nvfp4_quantize + to_blocked for activations (nvfp4_tensor.py:772-854).
  * x bf16 [M,K] -> q uint8 [M,K/2] (even k in the LOW nibble), scales e4m3 bytes.
@@ -246,6 +263,8 @@ int ao_fp8_fakequant_rowwise(const uint16_t* x, int M, int K, uint16_t* xq_bf16,
 int ao_int8_quantize_rowwise_ld(const uint16_t* x, int ldx, int M, int K, int8_t* q, float* scale, void* stream);
 int ao_fp8_quantize_rowwise_ld(const uint16_t* x, int ldx, int M, int K, uint8_t* q, float* scale, void* stream);
 int ao_mxfp8_quantize_ld(const uint16_t* x, int ldx, int M, int K, uint8_t* q, uint8_t* scale_e8m0,
+                         int swizzled, void* stream);
+int ao_mxfp4_quantize_ld(const uint16_t* x, int ldx, int M, int K, uint8_t* q, uint8_t* scale_e8m0,
                          int swizzled, void* stream);
 int ao_nvfp4_quantize_ld(const uint16_t* x, int ldx, int M, int K, const float* per_tensor_scale,
                          uint8_t* q, uint8_t* scale_e4m3, int swizzled, void* stream);
