@@ -145,6 +145,9 @@ __global__ void __launch_bounds__(WARPS * 32) final_kernel(const __nv_bfloat16* 
   }
 }
 
+// Workspace layout: fp32 scale[G] and zero[G], then partial[nblocks] doubles at align16(8 G), then Ctrl.  The tests
+// read all of it back after a call (tests/test_hqq_exact_gpu.py, layout in tests/hqq_model.py workspace_layout), so a
+// change here needs the same change there.
 template <int EPL>
 static int run(const uint16_t* w, int N, int K, uint8_t* q, uint16_t* scale_out, uint16_t* zero_out, void* ws,
                cudaStream_t st) {
