@@ -5,6 +5,7 @@
 //   nvfp4 block-16 e4m3   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm fp4 + pts/bias kernels
 //   nvfp4 weight x bf16   (bf16 wgmma, weights dequantised exactly)      replaces F.linear on the dequantised weight
 //   mxfp4 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces F.linear on both dequantize()s
+//   int8 weight x bf16    (bf16 wgmma, weights converted exactly)        replaces torch.mm on qdata.to(bf16) + the scale
 // Reference call sites: int8/kernels.py:18-76,114-144 + int8_tensor.py:305-359;
 // float8/inference.py:86-123; mx_formats/mx_tensor.py:759-843; nvfp4_tensor.py:487-578.
 //
@@ -248,6 +249,70 @@ struct Mxfp4Fmt {
   }
 };
 
+// int8 weights x bf16 activations (Int8WeightOnlyConfig; reference int8_tensor.py:336-359, per-row and per-tensor
+// scales): the stored [N, K] qdata in the stage and map of SsFmt<KIND_I8>, each byte converted exactly to bf16 in the
+// register-A fragment.  The scale stays out of the K loop: bf16 x int8 products are exact in fp32, and the epilogue
+// (EPI_BF16_WSCALE) applies the reference's three roundings.
+// Conversion: a byte b of two's complement q gives bf16 0x4300 | (b & 0x7F) = 128 + (b & 0x7F) and
+// 0x4300 | (b & 0x80) = 128 (q >= 0) or 256 (q < 0); their difference is q, exact (|q| <= 128 has 8 significant bits).
+struct Int8WoFmt {
+  static constexpr bool SS = false;
+  // ptxas, sm_90a: no stack at 80 registers for the 16- and 32-token tiles (DESIGN.md §2c)
+  static constexpr bool DECODE_2CTA = true;
+  static constexpr bool PROMOTE = false;
+  static constexpr int X_ELEM_BYTES = 2;
+  static constexpr int W_BYTES = ROWS * KCHUNK;   // 128 rows x 128 bytes, 128-byte swizzle
+  static constexpr int AUX_BYTES = 0;
+  static constexpr int EPI = tsg::EPI_BF16_WSCALE;
+  static constexpr int ACC_EXP2 = 0;
+  static constexpr int MAX_N_MMA = 128;
+  // no aux operand: the weight map stands in for it (see SsFmt)
+  static int make_maps(const uint8_t* wq, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    return SsFmt<KIND_I8>::make_maps(wq, N, K, tm_w, tm_aux);
+  }
+  __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES; }
+  __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap*, const tsg::Params&,
+                                                 uint8_t* w_dst, uint8_t*, uint64_t* bar, int n_tile, int kc,
+                                                 uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
+  }
+  // the thread's two fragment rows: for k16 step kk the bytes of k 16kk + 2t + (0, 8, 1, 9), so that each bf16x2 lane
+  // finds its byte at its own bits 7:0 (k 2t, 2t + 1) or 15:8 (k 2t + 8, 2t + 9)
+  struct Raw {
+    uint32_t v[2][8];
+  };
+  __device__ static __forceinline__ void load(const tsg::Params&, uint32_t w_smem, uint32_t, int row_lo, int lane,
+                                              Raw& raw) {
+    const int t = lane & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row_lo + 8 * h;
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint32_t a = w_smem + (uint32_t)r * 128u + ((uint32_t)(kk ^ (r & 7)) << 4) + 2 * t;   // TMA 128B swizzle
+        raw.v[h][kk] = __byte_perm(tsg::lds16(a), tsg::lds16(a + 8), 0x5140);
+      }
+    }
+  }
+  // bf16x2 of the int8 at bits 7:0 of each 16-bit lane (the other bits are ignored)
+  __device__ static __forceinline__ uint32_t cvt(uint32_t w, uint32_t magic) {
+    uint32_t v, c;
+    asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(v) : "r"(w), "r"(0x007F007Fu), "r"(magic));   // (w & mask) | magic
+    asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(c) : "r"(w), "r"(0x00800080u), "r"(magic));
+    const __nv_bfloat162 d = __hsub2(*reinterpret_cast<const __nv_bfloat162*>(&v), *reinterpret_cast<const __nv_bfloat162*>(&c));
+    return *reinterpret_cast<const uint32_t*>(&d);
+  }
+  __device__ static __forceinline__ void frag(const tsg::Params&, const Raw& raw, int kk, uint32_t (&a)[4]) {
+    uint32_t magic = 0x43004300u;
+    asm volatile("" : "+r"(magic));   // keep it in a register
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      a[h] = cvt(raw.v[h][kk], magic);
+      a[h + 2] = cvt(raw.v[h][kk] >> 8, magic);
+    }
+  }
+};
+
 // Activation pre-pass of the block-scaled kinds: rows [m0, m0 + rows) of the quantised activations -> bf16 [rows][K],
 // every element times its block scale (exact in bf16).  One thread per 16 elements.
 template <int KIND>
@@ -379,6 +444,28 @@ extern "C" int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, 
   return lowp::rowwise<lowp::KIND_I8>(reinterpret_cast<const uint8_t*>(xq), nullptr, M, K,
                                       reinterpret_cast<const uint8_t*>(wq), nullptr, N, nullptr, nullptr, acc, workspace,
                                       workspace_bytes, stream);
+}
+
+// F.linear(x, Int8Tensor without act_quant_kwargs), per-row or per-tensor scale (int8_tensor.py:336-359):
+// y = bf16(bf16(bf16(x wq^T) * bf16(w_scale[n])) + bias[n]); one launch, no activation quantizer
+extern "C" int ao_int8_weight_linear(const uint16_t* x, int ldx, int M, int K, const int8_t* wq, const float* w_scale,
+                                     int N, const uint16_t* bias, uint16_t* y, void* workspace,
+                                     size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int8 weight linear: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(K % 16 == 0, "int8 weight linear: K=%d must be a multiple of 16 (TMA row pitch)", K);
+  AO_REQUIRE(ldx >= K && ldx % 8 == 0, "int8 weight linear: ldx=%d must be >= K=%d and a multiple of 8", ldx, K);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && wq && w_scale && y, "int8 weight linear: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "int8 weight linear: x must be 16-byte aligned");
+  CUtensorMap tm_w, tm_aux;
+  if (int rc = lowp::Int8WoFmt::make_maps(reinterpret_cast<const uint8_t*>(wq), N, K, &tm_w, &tm_aux)) return rc;
+  tsg::Params p{};
+  p.w_scale = w_scale;
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<lowp::Int8WoFmt>(p, tm_w, tm_aux, x, ldx, workspace, workspace_bytes, "int8 weight linear",
+                                   reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, int M, int K,

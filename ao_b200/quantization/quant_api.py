@@ -1,7 +1,8 @@
 """User API: ``quantize_`` + the stable configs + their module handlers.
 
 Same names, dataclass fields and defaults as torchao/quantization/quant_api.py
-(quantize_ :249-321, Int4WeightOnlyConfig :502-535, Int8DynamicActivationInt8WeightConfig :808-862,
+(quantize_ :249-321, Int4WeightOnlyConfig :502-535, Int8WeightOnlyConfig :703-780,
+Int8DynamicActivationInt8WeightConfig :808-862,
 Float8DynamicActivationFloat8WeightConfig :1112-1172, FqnToConfig :1514-1600; handlers :597-627,
 :885-915, :1299-1336).  Differences, all deliberate:
   * handlers do NOT touch global inductor flags (the reference calls
@@ -24,7 +25,7 @@ import torch.nn as nn
 from ao_b200._native import require_sm90
 from ao_b200.core.config import AOBaseConfig
 from ao_b200.float8.inference import FP8Granularity, Float8MMConfig, _normalize_granularity
-from ao_b200.quantization.granularity import Granularity, PerRow, PerTensor
+from ao_b200.quantization.granularity import Granularity, PerGroup, PerRow, PerTensor
 from ao_b200.quantization.quant_primitives import MappingType
 from ao_b200.quantization.quantize_.common.kernel_preference import KernelPreference
 from ao_b200.quantization.quantize_.workflows import (
@@ -35,7 +36,7 @@ from ao_b200.quantization.transform_module import _QUANTIZE_CONFIG_HANDLER, regi
 logger = logging.getLogger(__name__)
 
 __all__ = [
-    "quantize_", "Int4WeightOnlyConfig", "Int8DynamicActivationInt8WeightConfig",
+    "quantize_", "Int4WeightOnlyConfig", "Int8DynamicActivationInt8WeightConfig", "Int8WeightOnlyConfig",
     "Float8DynamicActivationFloat8WeightConfig", "FqnToConfig", "ModuleFqnToConfig", "fqn_matches_fqn_config",
     "_is_linear", "_replace_with_custom_fn_if_matches_filter",
 ]
@@ -222,6 +223,52 @@ def _int8_dynamic_activation_int8_weight_quantize_tensor(weight, config):
 def _int8_dynamic_activation_int8_weight_transform(module, config, *, parameter_name="weight"):
     assert hasattr(module, parameter_name), f"Expected module to have {parameter_name!r}"
     new_weight = _int8_dynamic_activation_int8_weight_quantize_tensor(getattr(module, parameter_name), config)
+    return _set_quantized_param(module, parameter_name, new_weight)
+
+
+# ---------------------------------------------------------------------------------------------
+# int8 weight only
+# ---------------------------------------------------------------------------------------------
+@dataclass
+class Int8WeightOnlyConfig(AOBaseConfig):
+    """int8 symmetric weight-only quantization, bf16 activations (reference :703-740).  ``PerRow()`` and
+    ``PerTensor()`` run on the sm_90a kernel; ``PerGroup`` is accepted here, as in the reference, and rejected by the
+    quantize handler."""
+
+    group_size: Optional[int] = None
+    granularity: Optional[Granularity] = PerRow()
+    set_inductor_config: bool = True
+    version: int = 2
+
+    def __post_init__(self):
+        if self.version == 1:
+            raise ValueError("version 1 of Int8WeightOnlyConfig has been removed, please use version 2")
+        assert self.group_size is None, (
+            f"Only support version 2 with group_size=None, got {self.group_size}. "
+            f"Use granularity=PerGroup({self.group_size}) instead.")
+        assert isinstance(self.granularity, (PerTensor, PerRow, PerGroup)), (
+            f"granularity must be PerTensor, PerRow, or PerGroup, but got {self.granularity}")
+
+
+def _int8_weight_only_quantize_tensor(weight, config):
+    if isinstance(config.granularity, PerGroup):
+        # the reference serves PerGroup by dequantize-then-mm (int8_tensor.py:338-345): another arithmetic, no kernel here
+        raise NotImplementedError(
+            f"Int8WeightOnlyConfig(granularity={config.granularity}): PerGroup int8 weights have no sm_90a kernel in "
+            f"this engine; use PerRow() or PerTensor()")
+    if weight.shape[-1] % 16 != 0:
+        # no fallback: the TMA row pitch of the int8 weights needs K % 16 == 0; leave the layer unquantized, with a log
+        # line, like the int8 dynamic flow does for its shape rule
+        logger.info(f"Skipping int8 weight only quantization: weight shape {tuple(weight.shape)} needs "
+                    f"in_features % 16 == 0 for the sm_90a kernel")
+        return weight
+    return Int8Tensor.from_hp(weight, granularity=config.granularity)
+
+
+@register_quantize_module_handler(Int8WeightOnlyConfig)
+def _int8_weight_only_transform(module, config, *, parameter_name="weight"):
+    assert hasattr(module, parameter_name), f"Expected module to have {parameter_name!r}"
+    new_weight = _int8_weight_only_quantize_tensor(getattr(module, parameter_name), config)
     return _set_quantized_param(module, parameter_name, new_weight)
 
 

@@ -5,6 +5,7 @@ Attribute names / order match torchao's Int8Tensor
 ``Int8Tensor.from_hp(x) -> _int_scaled_matmul -> aten._int_mm -> pointwise epilogue``
 (:266-359, int8/kernels.py:114-144) with two launches: a fused per-token quantizer and an int8 GEMM
 whose epilogue reproduces the reference's rounding order bf16(bf16(acc*s_x)*s_w + bias).
+Without ``act_quant_kwargs`` (Int8WeightOnlyConfig) the linear is one launch: bf16 activations on the int8 weights.
 """
 from __future__ import annotations
 
@@ -110,11 +111,9 @@ def _(func, types, args, kwargs):
     out_dtype = x.dtype
     if w.act_pre_scale is not None:
         x = x * w.act_pre_scale
-    if w.act_quant_kwargs is None:
-        raise NotImplementedError(
-            "int8 weight-only linear is outside this engine's scope (SURVEY §8); use "
-            "Int8DynamicActivationInt8WeightConfig")
     N, K = w.qdata.shape[-2], w.qdata.shape[-1]
+    if w.act_quant_kwargs is None:
+        return _weight_only_linear(x, w, bias, out_dtype)
     x2 = x.reshape(-1, K)
     out_shape = (*x.shape[:-1], N)
     if x2.shape[0] == 0:
@@ -141,6 +140,25 @@ def _(func, types, args, kwargs):
     y = (y - corr.to(out_dtype)) * ws
     if bias is not None:
         y = y + bias
+    return y.reshape(out_shape).to(out_dtype)
+
+
+def _weight_only_linear(x, w, bias, out_dtype):
+    """bf16 activations on per-row / per-tensor int8 weights (reference :336-359): one launch whose epilogue keeps the
+    reference's roundings bf16(bf16(bf16(acc) * bf16(s_w)) + bias).  Other activation dtypes are cast to bf16."""
+    N, K = w.qdata.shape[-2], w.qdata.shape[-1]
+    if w.qdata.dim() != 2 or list(w.block_size) not in ([1, K], [N, K]):
+        raise NotImplementedError(
+            f"int8 weight-only linear: block_size {list(w.block_size)} of a {tuple(w.qdata.shape)} weight is neither "
+            f"per-row nor per-tensor (PerGroup has no sm_90a kernel in this engine)")
+    out_shape = (*x.shape[:-1], N)
+    if x.numel() == 0:
+        return x.new_empty(out_shape)
+    x2 = rows_for_kernel(x.to(torch.bfloat16).reshape(-1, K))
+    ws = w.scale.reshape(-1).float()
+    if ws.numel() == 1:
+        ws = ws.expand(N)
+    y = torch.ops.ao_b200.int8_weight_linear(x2, w.qdata.contiguous(), ws.contiguous(), bias)
     return y.reshape(out_shape).to(out_dtype)
 
 

@@ -138,6 +138,13 @@ int ao_int8_dyn_linear(const int8_t* xq, const float* x_scale, int M, int K,
                        const int8_t* wq, const float* w_scale, int N,
                        const uint16_t* bias, uint16_t* y, void* workspace,
                        size_t workspace_bytes, void* stream);
+/* int8 weight-only: bf16 activations on the stored int8 weights, per-row scale (a per-tensor scale expanded to
+ * [N]).  Replaces torch.mm(x, qdata.t().to(bf16)) * scale.to(bf16) + bias (int8_tensor.py:336-359) with the same
+ * three roundings: y = bf16(bf16(bf16(acc_f32) * bf16(w_scale[n])) + bias[n]); no add without a bias.
+ * x bf16 [M][ldx] (ldx >= K, ldx % 8 == 0, 16-byte aligned), wq int8 [N,K], w_scale f32 [N]; K % 16 == 0, any N. */
+int ao_int8_weight_linear(const uint16_t* x, int ldx, int M, int K, const int8_t* wq, const float* w_scale,
+                          int N, const uint16_t* bias, uint16_t* y, void* workspace,
+                          size_t workspace_bytes, void* stream);
 /* int32 accumulator only (aten._int_mm equivalent; int8/kernels.py:18-76). */
 int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, int N, int32_t* acc,
                    void* workspace, size_t workspace_bytes, void* stream);
