@@ -6,6 +6,7 @@
 //   nvfp4 weight x bf16   (bf16 wgmma, weights dequantised exactly)      replaces F.linear on the dequantised weight
 //   mxfp4 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces F.linear on both dequantize()s
 //   int8 weight x bf16    (bf16 wgmma, weights converted exactly)        replaces torch.mm on qdata.to(bf16) + the scale
+//   e4m3 weight x bf16    (bf16 wgmma, weights dequantised per element)  replaces torch.matmul on the dequantised weight
 // Reference call sites: int8/kernels.py:18-76,114-144 + int8_tensor.py:305-359;
 // float8/inference.py:86-123; mx_formats/mx_tensor.py:759-843; nvfp4_tensor.py:487-578.
 //
@@ -137,6 +138,11 @@ struct Mxfp8Fmt {
     uint32_t v[2][8];
     uint32_t sc[2];
   };
+  // row r's e4m3 pairs of k16 step kk: k 16kk + 2t, + 1 at bits 15:0 and k 16kk + 2t + 8, + 9 at bits 31:16
+  __device__ static __forceinline__ uint32_t lds_pairs(uint32_t w_smem, int r, int kk, int t) {
+    const uint32_t a = w_smem + (uint32_t)r * 128u + ((uint32_t)(kk ^ (r & 7)) << 4) + 2 * t;   // TMA 128B swizzle
+    return tsg::lds16(a) | (tsg::lds16(a + 8) << 16);
+  }
   __device__ static __forceinline__ void load(const tsg::Params&, uint32_t w_smem, uint32_t aux_smem, int row_lo, int lane,
                                               Raw& raw) {
     const int t = lane & 3;
@@ -145,10 +151,7 @@ struct Mxfp8Fmt {
       const int r = row_lo + 8 * h;
       raw.sc[h] = tsg::lds32(aux_smem + (uint32_t)(r & 31) * 16u + (uint32_t)(r >> 5) * 4u);
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        const uint32_t a = w_smem + (uint32_t)r * 128u + ((uint32_t)(kk ^ (r & 7)) << 4) + 2 * t;   // TMA 128B swizzle
-        raw.v[h][kk] = tsg::lds16(a) | (tsg::lds16(a + 8) << 16);
-      }
+      for (int kk = 0; kk < 8; ++kk) raw.v[h][kk] = lds_pairs(w_smem, r, kk, t);
     }
   }
   __device__ static __forceinline__ uint32_t deq(uint32_t pair, float s) {
@@ -313,6 +316,64 @@ struct Int8WoFmt {
   }
 };
 
+// e4m3 weights x bf16 activations (Float8WeightOnlyConfig; reference float8_tensor.py:459-469, per-row and per-tensor
+// scales): the stored [N, K] qdata in the stage and map of Mxfp8Fmt, plus the tile's 128 fp32 row scales, one 512-byte
+// TMA box of w_scale [N] per chunk (rows past N zero-filled).  The reference dequantizes before the matmul,
+// w~ = bf16(fp32(e4m3(q) * s)): an e4m3 code has 4 significant bits and a bf16 scale 8, so the product rounds per
+// element and the scale cannot leave the K loop.  Each element is Mxfp8Fmt::deq with the row's fp32 scale in place of
+// the block's power of two (e4m3 -> half -> fp32 exactly, one fp32 multiply, one bf16 rounding; the build has no
+// flush-to-zero, so subnormal products stay), every bf16 x w~ product is exact in fp32, and the epilogue (EPI_BF16)
+// rounds the sum to bf16 and adds the bias in bf16, as torch.matmul and `+ bias` do.
+struct Fp8WoFmt {
+  static constexpr bool SS = false;
+  // ptxas, sm_90a: at 80 registers (two CTAs per SM) the N_MMA = 32 tile keeps 8 bytes of stack: one CTA per SM, as
+  // mxfp8 (DESIGN.md §2d)
+  static constexpr bool DECODE_2CTA = false;
+  static constexpr bool PROMOTE = false;
+  static constexpr int X_ELEM_BYTES = 2;
+  static constexpr int W_BYTES = ROWS * KCHUNK;   // 128 rows x 128 bytes, 128-byte swizzle
+  static constexpr int AUX_BYTES = ROWS * 4;      // the tile's fp32 row scales
+  static constexpr int EPI = tsg::EPI_BF16;
+  static constexpr int ACC_EXP2 = 0;
+  static constexpr int MAX_N_MMA = 128;
+  static int make_maps(const uint8_t* wq, const float* w_scale, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_s) {
+    if (int rc = kmajor_byte_map(wq, N, K, tm_w)) return rc;
+    const uint64_t dims[1] = {(uint64_t)N};
+    const uint32_t box[1] = {ROWS};
+    return make_tmap(tm_s, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 1, w_scale, dims, nullptr, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
+  __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES + AUX_BYTES; }
+  __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap* tm_s, const tsg::Params&,
+                                                 uint8_t* w_dst, uint8_t* aux_dst, uint64_t* bar, int n_tile, int kc,
+                                                 uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
+    tma_load_1d(aux_dst, tm_s, bar, n_tile * ROWS, policy);
+  }
+  // the pairs of Mxfp8Fmt::Raw and the scales of the thread's two fragment rows
+  struct Raw {
+    uint32_t v[2][8];
+    float s[2];
+  };
+  __device__ static __forceinline__ void load(const tsg::Params&, uint32_t w_smem, uint32_t aux_smem, int row_lo, int lane,
+                                              Raw& raw) {
+    const int t = lane & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row_lo + 8 * h;
+      raw.s[h] = __uint_as_float(tsg::lds32(aux_smem + (uint32_t)r * 4u));
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) raw.v[h][kk] = Mxfp8Fmt::lds_pairs(w_smem, r, kk, t);
+    }
+  }
+  __device__ static __forceinline__ void frag(const tsg::Params&, const Raw& raw, int kk, uint32_t (&a)[4]) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      a[h] = Mxfp8Fmt::deq(raw.v[h][kk] & 0xFFFFu, raw.s[h]);
+      a[h + 2] = Mxfp8Fmt::deq(raw.v[h][kk] >> 16, raw.s[h]);
+    }
+  }
+};
+
 // Activation pre-pass of the block-scaled kinds: rows [m0, m0 + rows) of the quantised activations -> bf16 [rows][K],
 // every element times its block scale (exact in bf16).  One thread per 16 elements.
 template <int KIND>
@@ -466,6 +527,29 @@ extern "C" int ao_int8_weight_linear(const uint16_t* x, int ldx, int M, int K, c
   p.M = M; p.N = N; p.N_out = N; p.K = K;
   return tsg::run<lowp::Int8WoFmt>(p, tm_w, tm_aux, x, ldx, workspace, workspace_bytes, "int8 weight linear",
                                    reinterpret_cast<cudaStream_t>(stream));
+}
+
+// F.linear(x, Float8Tensor without act_quant_kwargs), per-row or per-tensor scale (float8_tensor.py:459-469):
+// y = bf16(bf16(sum_k x[m,k] * bf16(fp32(e4m3(wq[n,k]) * w_scale[n]))) + bias[n]); one launch, no activation quantizer
+extern "C" int ao_fp8_weight_linear(const uint16_t* x, int ldx, int M, int K, const uint8_t* wq, const float* w_scale,
+                                    int N, const uint16_t* bias, uint16_t* y, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 weight linear: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(K % 16 == 0, "fp8 weight linear: K=%d must be a multiple of 16 (TMA row pitch)", K);
+  AO_REQUIRE(ldx >= K && ldx % 8 == 0, "fp8 weight linear: ldx=%d must be >= K=%d and a multiple of 8", ldx, K);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && wq && w_scale && y, "fp8 weight linear: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "fp8 weight linear: x must be 16-byte aligned");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(w_scale) & 15) == 0,
+             "fp8 weight linear: w_scale must be 16-byte aligned (it is loaded by TMA)");
+  CUtensorMap tm_w, tm_s;
+  if (int rc = lowp::Fp8WoFmt::make_maps(wq, w_scale, N, K, &tm_w, &tm_s)) return rc;
+  tsg::Params p{};
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<lowp::Fp8WoFmt>(p, tm_w, tm_s, x, ldx, workspace, workspace_bytes, "fp8 weight linear",
+                                  reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, int M, int K,

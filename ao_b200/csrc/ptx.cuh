@@ -68,6 +68,13 @@ __device__ __forceinline__ uint64_t policy_evict_last() {
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
+__device__ __forceinline__ void tma_load_1d(void* dst, const void* tmap, uint64_t* bar, int c0, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3}], [%2], %4;" ::"r"(smem_u32(dst)),
+      "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "l"(policy)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(void* dst, const void* tmap, uint64_t* bar, int c0,
                                             int c1, uint64_t policy) {
   asm volatile(

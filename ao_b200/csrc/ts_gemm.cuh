@@ -4,7 +4,7 @@
 //
 // Swap-AB: 128 weight rows of a tile are the wgmma M dimension (two consumer warpgroups of 64 rows each), the tokens
 // are the wgmma N dimension (N_MMA = 16..128).  A format policy (Fmt) decides how the weights reach the tensor core:
-//   * register-A (Fmt::SS == false): int4 tinygemm, nvfp4, mxfp8, mxfp4, int8 weight-only.  Each consumer thread loads the packed
+//   * register-A (Fmt::SS == false): int4 tinygemm, nvfp4, mxfp8, mxfp4, int8 and fp8 weight-only.  Each consumer thread loads the packed
 //     weights of its two fragment rows straight from the TMA-filled stage and dequantises them into the bf16 A
 //     fragment of wgmma.m64nNk16 (4 x bf16x2 per k16 step); the activations (bf16) are the shared-memory B operand
 //   * shared-memory A (Fmt::SS == true): int8 x int8 -> s32 and e4m3 x e4m3 -> f32 (wgmma k32), both operands are
@@ -61,7 +61,7 @@ constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA && !IsGroup
 constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
 
 // Epilogue arithmetic, per kind (Fmt::EPI; must stay what each format's reference computes, see Params)
-enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2, EPI_BF16_WSCALE = 3 };
+enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2, EPI_BF16_WSCALE = 3, EPI_BF16 = 4 };
 
 struct Params {
   const __nv_bfloat16* bias;
@@ -76,7 +76,8 @@ struct Params {
   };
   int out_scale_per_row;
   int grid_forced;          // Grouped<Fmt>: the host grid was forced (ao_b200_debug_set_streamk_ctas): no MIN_UNITS rule
-  const float* w_scale;     // EPI_I8 / EPI_F8 / EPI_BF16_WSCALE: per-output-feature weight scale [N]
+  const float* w_scale;     // EPI_I8 / EPI_F8 / EPI_BF16_WSCALE: per-output-feature weight scale [N] (EPI_BF16 never
+                            // reads it: its format applies the scale per weight, from the aux operand)
   __nv_bfloat16* y;         // [M, N_out]
   int32_t* i32_out;         // EPI_I8: raw int32 accumulators [M, N] instead of y
   float* ws_partial;        // [grid][N_MMA*128]   CTA b's CONTRIB partial (streamk.cuh)
@@ -462,7 +463,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
             if (p.out_scale2) osc *= *p.out_scale2;
           }
           osc *= __int_as_float((127 + Fmt::ACC_EXP2) << 23);
-        } else {
+        } else if constexpr (Fmt::EPI != EPI_BF16) {
           sw = w_scale ? w_scale[n] : 1.f;
         }
 #pragma unroll
@@ -490,6 +491,11 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
               // then a bf16 add of the bias (absent: no add).  The product of two bf16 is exact in fp32
               const float s = __bfloat162float(__float2bfloat16_rn(sw));
               __nv_bfloat16 o = __float2bfloat16_rn(__bfloat162float(__float2bfloat16_rn(__uint_as_float(raw))) * s);
+              if (p.bias) o = __float2bfloat16_rn(__bfloat162float(o) + bias);
+              *dst = o;
+            } else if constexpr (Fmt::EPI == EPI_BF16) {
+              // fp8 weight-only reference: torch.matmul returns bf16, then a bf16 add of the bias (absent: no add)
+              __nv_bfloat16 o = __float2bfloat16_rn(__uint_as_float(raw));
               if (p.bias) o = __float2bfloat16_rn(__bfloat162float(o) + bias);
               *dst = o;
             } else {

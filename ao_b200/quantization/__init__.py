@@ -6,7 +6,7 @@ from .quantize_.workflows import (  # noqa: F401
     Float8PackingFormat, Float8Tensor, Int4ChooseQParamsAlgorithm, Int4PackingFormat, Int4TilePackedTo4dTensor,
     Int8Tensor, QuantizeTensorToFloat8Kwargs, QuantizeTensorToInt8Kwargs)
 from .quant_api import (  # noqa: F401
-    Float8DynamicActivationFloat8WeightConfig, FqnToConfig, Int4WeightOnlyConfig,
+    Float8DynamicActivationFloat8WeightConfig, Float8WeightOnlyConfig, FqnToConfig, Int4WeightOnlyConfig,
     Int8DynamicActivationInt8WeightConfig, Int8WeightOnlyConfig, ModuleFqnToConfig, fqn_matches_fqn_config, quantize_)
 from .transform_module import register_quantize_module_handler  # noqa: F401
 from .utils import compute_error  # noqa: F401

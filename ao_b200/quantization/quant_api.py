@@ -3,7 +3,8 @@
 Same names, dataclass fields and defaults as torchao/quantization/quant_api.py
 (quantize_ :249-321, Int4WeightOnlyConfig :502-535, Int8WeightOnlyConfig :703-780,
 Int8DynamicActivationInt8WeightConfig :808-862,
-Float8DynamicActivationFloat8WeightConfig :1112-1172, FqnToConfig :1514-1600; handlers :597-627,
+Float8WeightOnlyConfig :1031-1109, Float8DynamicActivationFloat8WeightConfig :1112-1172, FqnToConfig :1514-1600;
+handlers :597-627,
 :885-915, :1299-1336).  Differences, all deliberate:
   * handlers do NOT touch global inductor flags (the reference calls
     recommended_inductor_config_setter(); this engine has no compiler in the hot path) --
@@ -37,8 +38,8 @@ logger = logging.getLogger(__name__)
 
 __all__ = [
     "quantize_", "Int4WeightOnlyConfig", "Int8DynamicActivationInt8WeightConfig", "Int8WeightOnlyConfig",
-    "Float8DynamicActivationFloat8WeightConfig", "FqnToConfig", "ModuleFqnToConfig", "fqn_matches_fqn_config",
-    "_is_linear", "_replace_with_custom_fn_if_matches_filter",
+    "Float8DynamicActivationFloat8WeightConfig", "Float8WeightOnlyConfig", "FqnToConfig", "ModuleFqnToConfig",
+    "fqn_matches_fqn_config", "_is_linear", "_replace_with_custom_fn_if_matches_filter",
 ]
 
 
@@ -331,6 +332,60 @@ def _float8_dynamic_activation_float8_weight_transform(module, config, *, parame
         require_sm90()
     assert hasattr(module, parameter_name), f"Expected module to have {parameter_name!r}"
     new_weight = _float8_dynamic_activation_float8_weight_quantize_tensor(getattr(module, parameter_name), config)
+    return _set_quantized_param(module, parameter_name, new_weight)
+
+
+# ---------------------------------------------------------------------------------------------
+# float8 weight only
+# ---------------------------------------------------------------------------------------------
+@dataclass
+class Float8WeightOnlyConfig(AOBaseConfig):
+    """float8 symmetric weight-only quantization, bf16 activations (reference :1031-1060).  e4m3 weights with
+    ``PerRow()`` (the default) or ``PerTensor()`` scales run on the sm_90a kernel; ``PerGroup`` is accepted here, as in
+    the reference, and rejected by the quantize handler, as is ``weight_dtype=torch.float8_e5m2``.  Weights that are
+    not bf16 are left unquantized: the reference computes their linear in their own dtype."""
+
+    weight_dtype: torch.dtype = e4m3_dtype
+    set_inductor_config: bool = True
+    version: int = 2
+    granularity: Granularity = None  # type: ignore[assignment]
+
+    def __post_init__(self):
+        if self.granularity is None:
+            self.granularity = PerRow()
+        assert isinstance(self.granularity, (PerTensor, PerRow, PerGroup)), (
+            f"granularity must be PerTensor, PerRow, or PerGroup, got {type(self.granularity)}")
+
+
+def _float8_weight_only_quantize_tensor(weight, config):
+    assert config.version == 2, f"Unexpected version: {config.version}"
+    if isinstance(config.granularity, PerGroup):
+        # [N, K / g] scales: the per-row box of one 128-k chunk is under TMA's 16-byte minimum for g = 64 and 128
+        raise NotImplementedError(
+            f"Float8WeightOnlyConfig(granularity={config.granularity}): PerGroup float8 weights have no sm_90a kernel "
+            f"in this engine; use PerRow() or PerTensor()")
+    if config.weight_dtype != e4m3_dtype:
+        raise NotImplementedError(
+            f"Float8WeightOnlyConfig(weight_dtype={config.weight_dtype}): only torch.float8_e4m3fn weights have an "
+            f"sm_90a kernel in this engine")
+    if weight.shape[-1] % 16 != 0:
+        # no fallback: the TMA row pitch of the e4m3 weights needs K % 16 == 0; leave the layer unquantized, with a log
+        # line, like the int8 weight-only flow does
+        logger.info(f"Skipping float8 weight only quantization: weight shape {tuple(weight.shape)} needs "
+                    f"in_features % 16 == 0 for the sm_90a kernel")
+        return weight
+    if weight.dtype != torch.bfloat16:
+        # the reference dequantizes into the weight's dtype and multiplies in it; the kernel computes in bf16 only
+        logger.info(f"Skipping float8 weight only quantization: weight dtype {weight.dtype} needs to be "
+                    f"torch.bfloat16 for the sm_90a kernel")
+        return weight
+    return Float8Tensor.from_hp(weight, float8_dtype=config.weight_dtype, granularity=config.granularity)
+
+
+@register_quantize_module_handler(Float8WeightOnlyConfig)
+def _float8_weight_only_transform(module, config, *, parameter_name="weight"):
+    assert hasattr(module, parameter_name), f"Expected module to have {parameter_name!r}"
+    new_weight = _float8_weight_only_quantize_tensor(getattr(module, parameter_name), config)
     return _set_quantized_param(module, parameter_name, new_weight)
 
 

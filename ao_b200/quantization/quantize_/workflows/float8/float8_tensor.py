@@ -5,6 +5,7 @@ Attribute names / order match torchao's Float8Tensor
 ``_float8_addmm_impl -> addmm_float8_unwrapped_inference -> torch._scaled_mm``
 (:338-469, float8/inference.py:86-123) with two launches: the per-token quantizer and the GEMM with
 a fused ``acc * s_x[m] * s_w[n] + bias -> bf16`` epilogue.
+Without ``act_quant_kwargs`` (Float8WeightOnlyConfig) the linear is one launch: bf16 activations on the e4m3 weights.
 """
 from __future__ import annotations
 
@@ -97,11 +98,8 @@ def _float8_linear_impl(input_tensor, weight_tensor: Float8Tensor, bias):
     N, K = weight_tensor.shape[-2], weight_tensor.shape[-1]
     out_shape = (*input_tensor.shape[:-1], N)
     if act_quant_kwargs is None:
-        # weight-only float8: outside the north-star path; semantics = matmul with dequantized weight
         assert not isinstance(input_tensor, TorchAOBaseTensor), "Expecting input_tensor to be unquantized"
-        raise NotImplementedError(
-            "Float8 weight-only linear is outside this engine's scope (SURVEY §8); use "
-            "Float8DynamicActivationFloat8WeightConfig")
+        return _weight_only_linear(input_tensor, weight_tensor, bias)
     assert not isinstance(input_tensor, TorchAOBaseTensor), "input tensor was already quantized"
     gran = act_quant_kwargs.granularity
     w_rowwise = _is_rowwise_scaled(weight_tensor.block_size, weight_tensor.shape)
@@ -124,6 +122,34 @@ def _float8_linear_impl(input_tensor, weight_tensor: Float8Tensor, bias):
     y = torch.ops.ao_b200.fp8_rowwise_linear(xq_t.qdata.contiguous(), x_scale.contiguous().float(),
                                              weight_tensor.qdata.contiguous(), w_scale.contiguous().float(), bias)
     return y.reshape(out_shape).to(input_tensor.dtype)
+
+
+def _weight_only_linear(x, w, bias):
+    """bf16 activations on per-row / per-tensor e4m3 weights (reference :459-469, torch.matmul on the dequantized
+    weight, then + bias): one launch that dequantizes each weight as the reference does, bf16(fp32(q) * s), and rounds
+    the sum and the bias add to bf16.  Other activation dtypes are cast to bf16.  The weight must come from a bf16
+    model: for an fp16 or fp32 one the reference dequantizes into that dtype and multiplies in it, which this kernel
+    does not compute."""
+    N, K = w.qdata.shape[-2], w.qdata.shape[-1]
+    if w.dtype != torch.bfloat16:
+        raise NotImplementedError(
+            f"float8 weight-only linear: the weight was quantized from {w.dtype}; the reference dequantizes it into "
+            f"{w.dtype} and runs the matmul in {w.dtype}, and the sm_90a kernel of this engine computes in "
+            f"torch.bfloat16 only")
+    if w.qdata.dim() != 2 or w.qdata.dtype != torch.float8_e4m3fn or list(w.block_size) not in ([1, K], [N, K]):
+        raise NotImplementedError(
+            f"float8 weight-only linear: a {tuple(w.qdata.shape)} {w.qdata.dtype} weight with block_size "
+            f"{list(w.block_size)} has no sm_90a kernel in this engine (2-D e4m3 weights with per-row or per-tensor "
+            f"scales only)")
+    out_shape = (*x.shape[:-1], N)
+    if x.numel() == 0:
+        return x.new_empty(out_shape)
+    x2 = rows_for_kernel(x.to(torch.bfloat16).reshape(-1, K))
+    ws = w.scale.reshape(-1).float()
+    if ws.numel() == 1:
+        ws = ws.expand(N)
+    y = torch.ops.ao_b200.fp8_weight_linear(x2, w.qdata.contiguous(), ws.contiguous(), bias)
+    return y.reshape(out_shape).to(x.dtype)
 
 
 @implements(aten.linear.default)

@@ -179,11 +179,12 @@ class TorchAOBaseTensor(torch.Tensor):
 
     def __setstate__(self, state):
         # checkpoints written before an optional attribute existed: fill with None (BC,
-        # reference utils.py:639-656)
+        # reference utils.py:639-656).  Names the class itself provides (Float8Tensor's `dtype` is the wrapper's own,
+        # read-only) are not instance state
         torch._utils._set_obj_state(self, state)
         for n in list(getattr(self, "optional_tensor_data_names", [])) + list(
                 getattr(self, "optional_tensor_attribute_names", [])):
-            if n not in self.__dict__:
+            if n not in self.__dict__ and not hasattr(type(self), n):
                 setattr(self, n, None)
 
     def __repr__(self):

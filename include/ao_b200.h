@@ -145,6 +145,14 @@ int ao_int8_dyn_linear(const int8_t* xq, const float* x_scale, int M, int K,
 int ao_int8_weight_linear(const uint16_t* x, int ldx, int M, int K, const int8_t* wq, const float* w_scale,
                           int N, const uint16_t* bias, uint16_t* y, void* workspace,
                           size_t workspace_bytes, void* stream);
+/* fp8 weight-only: bf16 activations on the stored e4m3 weights, per-row scale (a per-tensor scale expanded to [N]).
+ * Replaces torch.matmul(x, dequantize(W).t()) + bias (float8_tensor.py:459-469) with the same roundings: each weight
+ * w~ = bf16(fp32(e4m3(wq[n,k]) * w_scale[n])), y = bf16(bf16(sum_k x[m,k] * w~[n,k]) + bias[n]); no add without a bias.
+ * x bf16 [M][ldx] (ldx >= K, ldx % 8 == 0, 16-byte aligned), wq e4m3 [N,K], w_scale f32 [N] (16-byte aligned);
+ * K % 16 == 0, any N. */
+int ao_fp8_weight_linear(const uint16_t* x, int ldx, int M, int K, const uint8_t* wq, const float* w_scale,
+                         int N, const uint16_t* bias, uint16_t* y, void* workspace,
+                         size_t workspace_bytes, void* stream);
 /* int32 accumulator only (aten._int_mm equivalent; int8/kernels.py:18-76). */
 int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, int N, int32_t* acc,
                    void* workspace, size_t workspace_bytes, void* stream);
