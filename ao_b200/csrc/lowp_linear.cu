@@ -7,6 +7,7 @@
 //   mxfp4 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces F.linear on both dequantize()s
 //   int8 weight x bf16    (bf16 wgmma, weights converted exactly)        replaces torch.mm on qdata.to(bf16) + the scale
 //   e4m3 weight x bf16    (bf16 wgmma, weights dequantised per element)  replaces torch.matmul on the dequantised weight
+//                         and, per expert, torch._grouped_mm on the dequantised expert weights
 // Reference call sites: int8/kernels.py:18-76,114-144 + int8_tensor.py:305-359;
 // float8/inference.py:86-123; mx_formats/mx_tensor.py:759-843; nvfp4_tensor.py:487-578.
 //
@@ -349,6 +350,16 @@ struct Fp8WoFmt {
     tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
     tma_load_1d(aux_dst, tm_s, bar, n_tile * ROWS, policy);
   }
+  // grouped kernels: the 128 weight rows from `row` = e*N + 128t of the [E * N, K] map and their scales, the 512-byte
+  // box from element `row` of the 1-D map over w_scale [E * N] (N % 8 == 0: a box that started off a 16-byte boundary
+  // of w_scale faulted on the H100).  A tile past N reads the next expert's rows and scales, or the maps' zero fill
+  // after the last expert; each output row depends on its own weight row only, and the epilogue skips the features >= N
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, const CUtensorMap* tm_s,
+                                                      const tsg::Params&, uint8_t* w_dst, uint8_t* aux_dst,
+                                                      uint64_t* bar, int row, int kc, uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, row, policy);
+    tma_load_1d(aux_dst, tm_s, bar, row, policy);
+  }
   // the pairs of Mxfp8Fmt::Raw and the scales of the thread's two fragment rows
   struct Raw {
     uint32_t v[2][8];
@@ -591,6 +602,38 @@ extern "C" int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale
   p.M = M; p.N = N; p.N_out = N; p.K = K;
   return tsg::run<Fmt>(p, tm_w, tm_aux, xq, K, workspace, workspace_bytes, "fp8 grouped mm",
                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+// torch._grouped_mm(x, W.transpose(-2, -1), offs) on weight-only e4m3 expert weights (float8_tensor.py:1085-1122,
+// weight-only branch: torch._grouped_mm on W.dequantize()), 2-D x 3-D: expert e's rows [offs[e-1], offs[e]) of the
+// bf16 x against wq[e] (the stored [E, N, K] qdata), each weight dequantized as the dense fp8 weight-only linear does
+// with w_scale[e, n], y = bf16(sum).  No bias.  offs stays on the device (grouped schedule, ts_gemm.cuh).
+extern "C" int ao_fp8_weight_grouped_mm(const uint16_t* x, int M, int K, const uint8_t* wq, const float* w_scale, int E,
+                                        int N, const int32_t* offs, uint16_t* y, void* workspace,
+                                        size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 weight grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "fp8 weight grouped mm: E=%d experts must be in [1, %d]", E,
+             tsg::MAX_EXPERTS);
+  AO_REQUIRE(K % 16 == 0, "fp8 weight grouped mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
+  // every scale box (element e*N + 128t of w_scale) starts on 32 bytes and every weight box on a row multiple of 8
+  AO_REQUIRE(N % 8 == 0, "fp8 weight grouped mm: N=%d must be a multiple of 8", N);
+  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "fp8 weight grouped mm: E*N=%lld weight rows exceed the int32 range",
+             (long long)E * N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && wq && w_scale && offs && y && workspace, "fp8 weight grouped mm: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "fp8 weight grouped mm: x must be 16-byte aligned");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(w_scale) & 15) == 0,
+             "fp8 weight grouped mm: w_scale must be 16-byte aligned (it is loaded by TMA)");
+  using Fmt = tsg::Grouped<lowp::Fp8WoFmt>;
+  CUtensorMap tm_w, tm_s;
+  if (int rc = Fmt::make_maps(wq, w_scale, E * N, K, &tm_w, &tm_s)) return rc;
+  tsg::Params p{};
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.offs = offs;
+  p.E = E;
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<Fmt>(p, tm_w, tm_s, x, K, workspace, workspace_bytes, "fp8 weight grouped mm",
+                       reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,

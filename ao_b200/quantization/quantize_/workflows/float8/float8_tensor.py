@@ -173,6 +173,20 @@ def _(func, types, args, kwargs):
     return Float8Tensor(qd, sc, bs, self.mm_config, self.act_quant_kwargs, self.kernel_preference, self.dtype)
 
 
+@implements(aten.select.int)
+def _(func, types, args, kwargs):
+    """Expert `index` of a 3-D weight as a 2-D tensor (reference :936-955): qdata[index], scale[index] and
+    block_size[1:], which the dense linear serves: the MoE expert loop's `F.linear(x, w[e])`.  A per-tensor scale
+    [1, 1, 1] is shared by every expert: each gets scale[0] (the reference's scale[index] fails for index > 0)."""
+    self, dim, index = args
+    assert dim == 0, f"Float8Tensor aten.select.int with {dim=} is not yet supported"
+    assert self.qdata.dim() == self.scale.dim() == len(self.block_size), "unsupported"
+    sc = self.scale[index] if self.scale.shape[0] == self.qdata.shape[0] else self.scale[0]
+    new = Float8Tensor(self.qdata[index], sc, list(self.block_size[1:]), self.mm_config,
+                       self.act_quant_kwargs, self.kernel_preference, self.dtype)
+    return return_and_correct_aliasing(func, args, kwargs, new)
+
+
 @implements(aten.transpose.int)
 def _(func, types, args, kwargs):
     """A view with qdata, scale and block_size swapped (float8_tensor.py:842-860): how a 3-D expert weight [E, N, K]
@@ -187,9 +201,10 @@ def _(func, types, args, kwargs):
 
 @implements(aten._grouped_mm.default)
 def _(func, types, args, kwargs):
-    """torch._grouped_mm(x, W.transpose(-2, -1), offs=offs) with a rowwise Float8Tensor expert weight W [E, N, K]
-    (the reference's handler, float8_tensor.py:1085-1122): the routed tokens are quantized per row and the grouped
-    GEMM runs on the stored qdata with w_scale[e, n].  Only the 2-D x 3-D form with PerRow activations."""
+    """torch._grouped_mm(x, W.transpose(-2, -1), offs=offs) with a Float8Tensor expert weight W [E, N, K] (the
+    reference's handler, float8_tensor.py:1085-1122).  Dynamic (rowwise) activations: the routed tokens are quantized
+    per row and the grouped GEMM runs on the stored qdata with w_scale[e, n].  Only the 2-D x 3-D form with PerRow
+    activations.  Weight-only: _weight_only_grouped_mm."""
     mat_a, mat_b = args[0], args[1]
     offs = args[2] if len(args) > 2 else kwargs.get("offs", None)
     assert isinstance(mat_b, Float8Tensor)
@@ -197,8 +212,7 @@ def _(func, types, args, kwargs):
     assert mat_b.qdata.stride(-2) < mat_b.qdata.stride(-1), "mat_b must be the transposed [E, N, K] weight"
     act_quant_kwargs = mat_b.act_quant_kwargs
     if act_quant_kwargs is None:
-        raise NotImplementedError("Float8 weight-only _grouped_mm is outside this engine's scope; use "
-                                  "Float8DynamicActivationFloat8WeightConfig")
+        return _weight_only_grouped_mm(mat_a, mat_b, offs, args, kwargs)
     if not isinstance(act_quant_kwargs.granularity, PerRow):
         raise NotImplementedError(f"_grouped_mm only supports PerRow granularity, got {act_quant_kwargs.granularity}")
     if mat_a.dim() != 2 or mat_b.dim() != 3:
@@ -215,6 +229,48 @@ def _(func, types, args, kwargs):
                                                  wq.contiguous(), mat_b.scale.reshape(E, N).float().contiguous(),
                                                  offs.to(torch.int32))
     return y.to(mat_a.dtype)
+
+
+def _weight_only_grouped_mm(mat_a, mat_b, offs, args, kwargs):
+    """The weight-only branch (reference :1099-1100, torch._grouped_mm on mat_b.dequantize()): expert e's rows
+    [offs[e-1], offs[e]) of the bf16 mat_a times its weights, each dequantized as the reference does,
+    bf16(fp32(q) * s), inside one grouped wgmma kernel; the sum is rounded once to bf16.  Rows from offs[-1] on are
+    left unwritten, as torch leaves them.  Only the 2-D x 3-D form of a bf16 model, no bias, a bf16 output, and
+    N % 8 == 0."""
+    bias = args[3] if len(args) > 3 else kwargs.get("bias", None)
+    out_dtype = args[4] if len(args) > 4 else kwargs.get("out_dtype", None)
+    if mat_b.dtype != torch.bfloat16:
+        raise NotImplementedError(
+            f"Float8Tensor weight-only _grouped_mm: the weight was quantized from {mat_b.dtype}; the reference "
+            f"dequantizes it into {mat_b.dtype} and multiplies in {mat_b.dtype}, and the sm_90a kernel of this engine "
+            f"computes in torch.bfloat16 only")
+    if isinstance(mat_a, TorchAOBaseTensor) or mat_a.dtype != torch.bfloat16 or out_dtype not in (None, torch.bfloat16):
+        raise NotImplementedError(f"Float8Tensor weight-only _grouped_mm: bf16 mat_a and output only, got "
+                                  f"{mat_a.dtype} -> {out_dtype}")
+    if bias is not None:
+        raise NotImplementedError("Float8Tensor weight-only _grouped_mm: bias is not supported")
+    if mat_a.dim() != 2 or mat_b.dim() != 3:
+        raise NotImplementedError(f"Float8Tensor weight-only _grouped_mm: only 2-D mat_a x 3-D mat_b, got "
+                                  f"{mat_a.dim()}-D x {mat_b.dim()}-D")
+    E, K, N = mat_b.shape
+    if mat_b.qdata.dtype != torch.float8_e4m3fn or list(mat_b.block_size) not in ([1, K, 1], [E, K, N]):
+        raise NotImplementedError(
+            f"Float8Tensor weight-only _grouped_mm: a {mat_b.qdata.dtype} weight with block_size "
+            f"{list(mat_b.block_size)} has no sm_90a kernel in this engine (e4m3 expert weights with per-row or "
+            f"per-tensor scales only)")
+    if N % 8 != 0:
+        raise NotImplementedError(f"Float8Tensor weight-only _grouped_mm: N={N} output features per expert; the sm_90a "
+                                  f"kernel of this engine needs N % 8 == 0 (each expert's scales start on 32 bytes)")
+    if mat_a.shape[-1] != K:
+        raise ValueError(f"_grouped_mm: mat_a has K={mat_a.shape[-1]}, mat_b K={K}")
+    wq = mat_b.qdata.transpose(-2, -1)   # back to the stored [E, N, K]
+    ws = mat_b.scale.float()
+    ws = ws.reshape(E, N) if ws.numel() == E * N else ws.reshape(1, 1).expand(E, N)
+    # the kernel takes contiguous, 16-byte aligned rows (alignment from the storage offset: traceable with fake tensors)
+    x = mat_a.contiguous()
+    if x.storage_offset() % 8 != 0:
+        x = x.clone()
+    return torch.ops.ao_b200.fp8_weight_grouped_mm(x, wq.contiguous(), ws.contiguous(), offs.to(torch.int32))
 
 
 Float8Tensor.__module__ = "ao_b200.quantization"

@@ -153,6 +153,18 @@ int ao_int8_weight_linear(const uint16_t* x, int ldx, int M, int K, const int8_t
 int ao_fp8_weight_linear(const uint16_t* x, int ldx, int M, int K, const uint8_t* wq, const float* w_scale,
                          int N, const uint16_t* bias, uint16_t* y, void* workspace,
                          size_t workspace_bytes, void* stream);
+/* torch._grouped_mm(x, W.transpose(-2, -1), offs) for a 3-D weight-only Float8Tensor expert weight W [E, N, K],
+ * 2-D x 3-D form (float8_tensor.py:1085-1122, weight-only branch: torch._grouped_mm on W.dequantize()): for
+ * offs[e-1] <= m < offs[e] (offs[-1] = 0)
+ *   y[m, n] = bf16( sum_k x[m,k] * bf16(fp32(e4m3(wq[e][n,k]) * w_scale[e][n])) ),  f32 accumulate,
+ * each weight dequantized as ao_fp8_weight_linear does.  x bf16 [M,K] (tokens sorted by expert, rows contiguous,
+ * 16-byte aligned); wq e4m3 [E][N][K] (the stored qdata); w_scale f32 [E][N] (16-byte aligned); offs int32 [E] on the
+ * device, cumulative row ends.  The host never reads offs (no sync, CUDA-graph capturable); the kernel clamps each
+ * offs[e] into [offs[e-1], M].  Rows from offs[E-1] on are not written.
+ * 1 <= E <= 1024, K % 16 == 0, N % 8 == 0, no bias.                                                              */
+int ao_fp8_weight_grouped_mm(const uint16_t* x, int M, int K, const uint8_t* wq, const float* w_scale, int E, int N,
+                             const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes,
+                             void* stream);
 /* int32 accumulator only (aten._int_mm equivalent; int8/kernels.py:18-76). */
 int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, int N, int32_t* acc,
                    void* workspace, size_t workspace_bytes, void* stream);

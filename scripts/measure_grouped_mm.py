@@ -4,7 +4,7 @@ F.scaled_grouped_mm on identical operands, for MoE expert shapes; with --fmt nvf
 per-expert activation quantizer nvfp4_fakequant_grouped plus nvfp4_grouped_mm) against the fp8 path with its
 quantizer (fp8_quantize_rowwise plus fp8_rowwise_grouped_mm) and bf16 torch._grouped_mm on the unquantized weights.
 
-  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4] [--group-size 32] [--replays 20] [--out FILE]
+  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4|fp8wo] [--group-size 32] [--replays 20] [--out FILE]
 
   * shapes: Mixtral-8x7B experts (E=8, 4096 -> 14336 and 14336 -> 4096, top-2) and Qwen3-30B-A3B experts (E=128,
     2048 -> 768 and 768 -> 2048, top-8);
@@ -23,7 +23,11 @@ roofline, 989 TFLOP/s, is never the bound at these shapes up to 128 tokens).  --
 int4 expert GEMM (int4_tilepacked_grouped_mm on 3-D Int4TilePackedTo4dTensor weights) against the dense int4 linear of
 each active expert (the select loop, captured with the routing fixed, without its host syncs), the fp8 path with its
 quantizer and bf16 torch._grouped_mm; bytes are the int4 path's (0.5 + 4 / g bytes per weight of the active experts,
-K and N as padded, the bf16 activations read once, the outputs).
+K and N as padded, the bf16 activations read once, the outputs).  --fmt fp8wo: the weight-only e4m3 expert GEMM
+(torch._grouped_mm on 3-D Float8Tensor weights of Float8WeightOnlyConfig) against the reference's recipe (torch._grouped_mm
+on W.dequantize(), all E experts dequantized on every call), bf16 torch._grouped_mm and the fp8 dynamic path with its
+quantizer; bytes are the weight-only path's (1 byte per weight and 4 per row scale of the active experts, the bf16
+activations read once, the outputs, offs) and its roofline term the HBM time of those bytes.
 """
 from __future__ import annotations
 
@@ -62,7 +66,7 @@ def routing(T, E, topk, skewed, seed):
     return torch.bincount(picks.reshape(-1), minlength=E).tolist()
 
 
-def time_graph(fn_of_copy, copies, replays):
+def time_graph(fn_of_copy, copies, replays, rounds=None):
     """µs per call of fn_of_copy(c) from a CUDA graph that calls it once for every weight copy c, several rounds."""
     import torch
 
@@ -72,7 +76,7 @@ def time_graph(fn_of_copy, copies, replays):
         for c in range(copies):   # warm-up outside the capture (workspaces, module loads)
             fn_of_copy(c)
     torch.cuda.synchronize()
-    rounds = max(1, 64 // copies)
+    rounds = rounds or max(1, 64 // copies)
     g = torch.cuda.CUDAGraph()
     with torch.cuda.graph(g, stream=st):
         for _ in range(rounds):
@@ -230,9 +234,73 @@ def measure_int4(a, ops, dev, lines):
         torch.cuda.empty_cache()
 
 
+def measure_fp8wo(a, ops, dev, lines):
+    """The weight-only e4m3 expert GEMM (torch._grouped_mm on a 3-D Float8Tensor without act_quant_kwargs) against
+    the reference's recipe (torch._grouped_mm on W.dequantize(), every expert dequantized in eager torch on each call),
+    bf16 torch._grouped_mm and the fp8 dynamic path with its quantizer."""
+    import torch
+
+    from ao_b200.quantization import Float8Tensor, PerRow
+
+    for name, E, N, K, topk in SHAPES:
+        g = torch.Generator(device=dev).manual_seed(E * N + K)
+        copies = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * (N * K + N * 4))) + 1)
+        copies_bf16 = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * N * K * 2)) + 1)
+        wo, w8, s8, wb = [], [], [], []
+        for c in range(max(copies, copies_bf16)):
+            w = (torch.randn(E, N, K, device=dev, generator=g) * 0.05).to(torch.bfloat16)
+            if c < copies:
+                t = Float8Tensor.from_hp(w, torch.float8_e4m3fn, PerRow())
+                wo.append(t)
+                w8.append(t.qdata)
+                s8.append(t.scale.reshape(E, N))
+            if c < copies_bf16:
+                wb.append(w)
+            del w
+        for T in TOKENS:
+            for skewed in (False, True):
+                rows = routing(T, E, topk, skewed, seed=T * 131 + E + skewed)
+                M = sum(rows)
+                offs = torch.tensor(rows, dtype=torch.int64).cumsum(0).to(torch.int32).to(dev)
+                x = torch.randn(M, K, device=dev, generator=g).to(torch.bfloat16)
+                active = sum(1 for r in rows if r)
+                need = active * (N * K + N * 4) + M * K * 2 + M * N * 2 + E * 4
+                rec = dict(fmt="fp8wo", shape=name, E=E, N=N, K=K, topk=topk, tokens=T,
+                           routing="skewed" if skewed else "balanced", rows=M, active_experts=active, bytes=need,
+                           weight_copies=copies, roofline_us=round(need / HBM_BPS * 1e6, 2))
+
+                def ours(c):
+                    return torch._grouped_mm(x, wo[c].transpose(-2, -1), offs=offs)
+
+                def recipe(c):
+                    return torch._grouped_mm(x, wo[c].dequantize().transpose(-2, -1), offs=offs)
+
+                def bf16(c):
+                    return torch._grouped_mm(x, wb[c].transpose(-2, -1), offs=offs)
+
+                def fp8(c):
+                    xq, sx = ops.fp8_quantize_rowwise(x)
+                    return ops.fp8_rowwise_grouped_mm(xq, sx.reshape(-1), w8[c], s8[c], offs)
+
+                n = int(offs[-1])
+                y = ours(0)[:n]
+                rec["sqnr_vs_recipe_db"] = sqnr_db(recipe(0)[:n], y)
+                rec["sqnr_vs_bf16_db"] = sqnr_db(bf16(0)[:n], y)
+                # the recipe allocates a bf16 copy of all E experts per call: one round of copies per replay
+                for key, fn, cp, rounds in (("ours", ours, copies, None), ("recipe", recipe, copies, 1),
+                                            ("bf16", bf16, copies_bf16, None), ("fp8", fp8, copies, None)):
+                    us = time_graph(fn, cp, a.replays, rounds)
+                    rec[f"{key}_us"] = round(us, 2)
+                    rec[f"{key}_GBps"] = round(need / us * 1e-3, 1)
+                print(json.dumps(rec), flush=True)
+                lines.append(rec)
+        del wo, w8, s8, wb
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4"], default="fp8")
+    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4", "fp8wo"], default="fp8")
     ap.add_argument("--group-size", type=int, choices=[32, 64, 128, 256], default=32)
     ap.add_argument("--replays", type=int, default=20)
     ap.add_argument("--out", default=None)
@@ -301,6 +369,8 @@ def main():
         measure_nvfp4(a, ops, dev, lines)
     if a.fmt == "int4":
         measure_int4(a, ops, dev, lines)
+    if a.fmt == "fp8wo":
+        measure_fp8wo(a, ops, dev, lines)
     info = dict(card=card(), torch=torch.__version__)
     print(json.dumps(info), flush=True)
     if a.out:
