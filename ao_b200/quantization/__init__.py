@@ -7,7 +7,8 @@ from .quantize_.workflows import (  # noqa: F401
     Int8Tensor, QuantizeTensorToFloat8Kwargs, QuantizeTensorToInt8Kwargs)
 from .quant_api import (  # noqa: F401
     Float8DynamicActivationFloat8WeightConfig, Float8WeightOnlyConfig, FqnToConfig, Int4WeightOnlyConfig,
-    Int8DynamicActivationInt8WeightConfig, Int8WeightOnlyConfig, ModuleFqnToConfig, fqn_matches_fqn_config, quantize_)
+    Int8DynamicActivationInt8WeightConfig, Int8StaticActivationInt8WeightConfig, Int8WeightOnlyConfig, ModuleFqnToConfig,
+    fqn_matches_fqn_config, quantize_)
 from .transform_module import register_quantize_module_handler  # noqa: F401
 from .utils import compute_error  # noqa: F401
 from ao_b200.float8.inference import Float8MMConfig  # noqa: F401

@@ -2,10 +2,10 @@
 
 Same names, dataclass fields and defaults as torchao/quantization/quant_api.py
 (quantize_ :249-321, Int4WeightOnlyConfig :502-535, Int8WeightOnlyConfig :703-780,
-Int8DynamicActivationInt8WeightConfig :808-862,
+Int8DynamicActivationInt8WeightConfig :808-862, Int8StaticActivationInt8WeightConfig :918-978,
 Float8WeightOnlyConfig :1031-1109, Float8DynamicActivationFloat8WeightConfig :1112-1172, FqnToConfig :1514-1600;
 handlers :597-627,
-:885-915, :1299-1336).  Differences, all deliberate:
+:885-915, :981-1028, :1299-1336).  Differences, all deliberate:
   * handlers do NOT touch global inductor flags (the reference calls
     recommended_inductor_config_setter(); this engine has no compiler in the hot path) --
     ``set_inductor_config`` is kept as an accepted, ignored field;
@@ -37,7 +37,8 @@ from ao_b200.quantization.transform_module import _QUANTIZE_CONFIG_HANDLER, regi
 logger = logging.getLogger(__name__)
 
 __all__ = [
-    "quantize_", "Int4WeightOnlyConfig", "Int8DynamicActivationInt8WeightConfig", "Int8WeightOnlyConfig",
+    "quantize_", "Int4WeightOnlyConfig", "Int8DynamicActivationInt8WeightConfig", "Int8StaticActivationInt8WeightConfig",
+    "Int8WeightOnlyConfig",
     "Float8DynamicActivationFloat8WeightConfig", "Float8WeightOnlyConfig", "FqnToConfig", "ModuleFqnToConfig",
     "fqn_matches_fqn_config", "_is_linear", "_replace_with_custom_fn_if_matches_filter",
 ]
@@ -224,6 +225,64 @@ def _int8_dynamic_activation_int8_weight_quantize_tensor(weight, config):
 def _int8_dynamic_activation_int8_weight_transform(module, config, *, parameter_name="weight"):
     assert hasattr(module, parameter_name), f"Expected module to have {parameter_name!r}"
     new_weight = _int8_dynamic_activation_int8_weight_quantize_tensor(getattr(module, parameter_name), config)
+    return _set_quantized_param(module, parameter_name, new_weight)
+
+
+# ---------------------------------------------------------------------------------------------
+# int8 static activation x int8 weight
+# ---------------------------------------------------------------------------------------------
+@dataclass
+class Int8StaticActivationInt8WeightConfig(AOBaseConfig):
+    """int8 weights with int8 activations quantized by a calibrated (static) scale, e.g. from SmoothQuant (reference
+    :918-978).  ``act_quant_scale`` is f32 ``[1, 1]`` (PerTensor) or ``[M, 1]`` (PerRow, one calibration batch);
+    ``act_quant_zero_point`` is int8 of the same shape, for ASYMMETRIC activations.  The linear quantizes the
+    activations with one kernel (``torch.ops.ao_b200.int8_quantize_static``), fusing the weight's ``act_pre_scale``."""
+
+    act_quant_scale: Optional[torch.Tensor] = None
+    act_quant_zero_point: Optional[torch.Tensor] = None
+    granularity: Optional[Union[Granularity, List[Granularity]]] = PerRow()
+    act_mapping_type: Optional[MappingType] = MappingType.SYMMETRIC
+    set_inductor_config: bool = True
+    version: int = 1
+    reduce_range: Optional[bool] = False
+
+    def __post_init__(self):
+        a, w = Int8Tensor._normalize_granularity(self.granularity)
+        _validate_granularity_int8(a, w)
+        assert self.act_mapping_type in (MappingType.SYMMETRIC, MappingType.ASYMMETRIC), (
+            "Int8StaticActivationInt8WeightConfig requires `act_mapping_type` in (MappingType.SYMMETRIC, "
+            "MappingType.ASYMMETRIC).")
+
+    def get_act_quant_kwargs(self) -> QuantizeTensorToInt8Kwargs:
+        """The activation quantization kwargs the quantized weight carries (reference :964-978)."""
+        a, _ = Int8Tensor._normalize_granularity(self.granularity)
+        return QuantizeTensorToInt8Kwargs(granularity=a, mapping_type=self.act_mapping_type,
+                                          reduce_range=self.reduce_range)
+
+
+def _int8_static_activation_int8_weight_quantize_tensor(weight, config):
+    if config.act_quant_scale is None:
+        # the reference fails on `None.detach()` (:1010)
+        raise ValueError("Int8StaticActivationInt8WeightConfig needs act_quant_scale (a calibrated activation scale)")
+    _, w = Int8Tensor._normalize_granularity(config.granularity)
+    if weight.shape[-1] % 16 != 0 or weight.shape[-2] % 8 != 0:
+        logger.info(f"Skipping int8 static quantization: weight shape {tuple(weight.shape)} needs in_features % 16 == 0 "
+                    f"and out_features % 8 == 0 for the sm_90a kernel")
+        return weight
+    # the calibrated tensors move to the weight's device here, so the forward (and a CUDA graph capturing it) never
+    # copies them from the host
+    zp = config.act_quant_zero_point
+    return Int8Tensor.from_hp(
+        weight, granularity=w, act_quant_kwargs=config.get_act_quant_kwargs(),
+        act_quant_scale=config.act_quant_scale.detach().to(weight.device),
+        act_quant_zero_point=None if zp is None else zp.detach().to(weight.device),
+        reduce_range=config.reduce_range)
+
+
+@register_quantize_module_handler(Int8StaticActivationInt8WeightConfig)
+def _int8_static_activation_int8_weight_transform(module, config, *, parameter_name="weight"):
+    assert hasattr(module, parameter_name), f"Expected module to have attribute `{parameter_name}` but not found"
+    new_weight = _int8_static_activation_int8_weight_quantize_tensor(getattr(module, parameter_name), config)
     return _set_quantized_param(module, parameter_name, new_weight)
 
 

@@ -6,6 +6,8 @@ Attribute names / order match torchao's Int8Tensor
 (:266-359, int8/kernels.py:114-144) with two launches: a fused per-token quantizer and an int8 GEMM
 whose epilogue reproduces the reference's rounding order bf16(bf16(acc*s_x)*s_w + bias).
 Without ``act_quant_kwargs`` (Int8WeightOnlyConfig) the linear is one launch: bf16 activations on the int8 weights.
+With a calibrated ``act_quant_scale`` (Int8StaticActivationInt8WeightConfig) one kernel applies ``act_pre_scale`` and the
+static scale and zero point, then the same GEMM runs.
 """
 from __future__ import annotations
 
@@ -109,9 +111,11 @@ def _(func, types, args, kwargs):
     x, w, bias = args[0], args[1], args[2] if len(args) > 2 else None
     assert isinstance(w, Int8Tensor), f"Expected weight to be Int8Tensor, got {type(w)}"
     out_dtype = x.dtype
+    N, K = w.qdata.shape[-2], w.qdata.shape[-1]
+    if w.act_quant_kwargs is not None and _static_quantizer_serves(x, w):
+        return _static_linear(x, w, bias, out_dtype)
     if w.act_pre_scale is not None:
         x = x * w.act_pre_scale
-    N, K = w.qdata.shape[-2], w.qdata.shape[-1]
     if w.act_quant_kwargs is None:
         return _weight_only_linear(x, w, bias, out_dtype)
     x2 = x.reshape(-1, K)
@@ -125,17 +129,50 @@ def _(func, types, args, kwargs):
     xs = xt.scale.reshape(-1).float()
     if xs.numel() == 1:
         xs = xs.expand(M)
+    return _int8_activation_linear(xt.qdata, xs.contiguous(), xt.zero_point, w, bias, out_shape, out_dtype)
+
+
+def _static_quantizer_serves(x, w):
+    """The calibrated-scale path: bf16 activations and an fp32 ``act_quant_scale`` on x's device, the dtypes
+    calibration produces.  A bf16 scale would make torch take the reciprocal and the product in bf16, and other
+    activation dtypes promote differently: those keep the torch route below."""
+    s, zp, p = w.act_quant_scale, w.act_quant_zero_point, w.act_pre_scale
+    return (s is not None and x.dtype == torch.bfloat16 and x.is_cuda and s.dtype == torch.float32
+            and s.device == x.device and (zp is None or (zp.dtype == torch.int8 and zp.device == x.device))
+            and (p is None or (p.dtype in (torch.bfloat16, torch.float32) and p.numel() == x.shape[-1]
+                               and p.device == x.device)))
+
+
+def _static_linear(x, w, bias, out_dtype):
+    """Two launches for a symmetric mapping: int8_quantize_static (the pre-scale product, the calibrated scale and zero
+    point, the clamp) and int8_dyn_linear.  The scales are read on the device, so a CUDA graph replays whatever
+    ``act_quant_scale`` holds.  Unlike the reference, a ``[1, 1]`` scale also serves a 3-D input: x is flattened to
+    [M, K] first."""
+    N, K = w.qdata.shape[-2], w.qdata.shape[-1]
+    out_shape = (*x.shape[:-1], N)
+    x2 = x.reshape(-1, K)
+    if x2.shape[0] == 0:
+        return x.new_empty(out_shape, dtype=out_dtype)
+    qmin, qmax = (-64, 63) if w.act_quant_kwargs.reduce_range else (-128, 127)
+    xq, xs, xzp = torch.ops.ao_b200.int8_quantize_static(rows_for_kernel(x2), w.act_quant_scale, w.act_quant_zero_point,
+                                                         w.act_pre_scale, qmin, qmax)
+    return _int8_activation_linear(xq, xs, xzp, w, bias, out_shape, out_dtype)
+
+
+def _int8_activation_linear(xq, xs, xzp, w, bias, out_shape, out_dtype):
+    """int8 activations xq [M, K] with f32 scales xs [M] (zero points xzp for an asymmetric mapping) on the weight."""
+    N = w.qdata.shape[-2]
     ws = w.scale.reshape(-1).float()
     if ws.numel() == 1:
         ws = ws.expand(N)
     wq = w.qdata.contiguous()
-    if kw.mapping_type == MappingType.SYMMETRIC:
-        y = torch.ops.ao_b200.int8_dyn_linear(xt.qdata.contiguous(), xs.contiguous(), wq, ws.contiguous(), bias)
+    if w.act_quant_kwargs.mapping_type == MappingType.SYMMETRIC:
+        y = torch.ops.ao_b200.int8_dyn_linear(xq.contiguous(), xs, wq, ws.contiguous(), bias)
         return y.reshape(out_shape).to(out_dtype)
     # asymmetric activations (int8_tensor.py:322-330): Y = (Xq Wq^T) s_x s_w - zp_x s_x rowsum(Wq) s_w
-    acc = torch.ops.ao_b200.int8_mm_i32(xt.qdata.contiguous(), wq)
+    acc = torch.ops.ao_b200.int8_mm_i32(xq.contiguous(), wq)
     y = (acc * xs.reshape(-1, 1)).to(out_dtype)
-    zp = xt.zero_point.reshape(-1, 1).float()
+    zp = xzp.reshape(-1, 1).float()
     corr = (zp * xs.reshape(-1, 1)) * w.qdata.sum(dim=-1).float()
     y = (y - corr.to(out_dtype)) * ws
     if bias is not None:
@@ -189,7 +226,9 @@ def _(func, types, args, kwargs):
     if zp is not None and zp.dim() == self.qdata.dim() and zp.shape[0] == self.qdata.shape[0]:
         zp = zp[index]
     return Int8Tensor(self.qdata[index], sc, list(self.block_size[1:]), self.dtype, zero_point=zp,
-                      act_quant_kwargs=self.act_quant_kwargs, reduce_range=self.reduce_range)
+                      act_quant_scale=self.act_quant_scale, act_quant_zero_point=self.act_quant_zero_point,
+                      act_pre_scale=self.act_pre_scale, act_quant_kwargs=self.act_quant_kwargs,
+                      reduce_range=self.reduce_range)
 
 
 Int8Tensor.__module__ = "ao_b200.quantization"

@@ -131,6 +131,19 @@ int ao_int4_tilepacked_grouped_mm(const uint16_t* x, int M, int K, const int32_t
  * quantize_tensor_kwargs.py:36-71).  x bf16 [M,K] -> q int8 [M,K], scale f32 [M].  */
 int ao_int8_quantize_rowwise(const uint16_t* x, int M, int K, int8_t* q, float* scale,
                              void* stream);
+/* Static (calibrated) int8 quantisation of activations, one launch: replaces x * act_pre_scale followed by
+ * Int8Tensor.from_hp(x, g, mapping, scale=act_quant_scale, zero_point=act_quant_zero_point) (int8_tensor.py:212-230,
+ * :280-294) on CUDA tensors:
+ *   q[m,k] = int8(clamp(rne(xp[m,k] * (1 / scale[m])) + zp[m], qmin, qmax)),
+ * xp = x * pre_scale[k] in fp32, rounded to bf16 when pre_scale_dtype = 1 (bf16 [K]), kept in fp32 when it is 2 (f32
+ * [K]); xp = x when it is 0 (pre_scale NULL).  1 / scale is the IEEE reciprocal, rne rounds half to even, a NaN gives 0.
+ * scale f32 and zero_point int8 (NULL: zeros) are device memory, one value or (*_per_row != 0) one per row [M]; they
+ * are never read on the host.  Outputs: q int8 [M,K] (dense), x_scale f32 [M] (the per-row scale ao_int8_dyn_linear
+ * takes), x_zero_point int8 [M] (NULL: not written).  x bf16 [M][ldx] (ldx >= K, ldx % 8 == 0, 16-byte aligned),
+ * pre_scale 16-byte aligned, K % 8 == 0, -128 <= qmin <= qmax <= 127.                                                */
+int ao_int8_quantize_static(const uint16_t* x, int ldx, int M, int K, const void* pre_scale, int pre_scale_dtype,
+                            const float* scale, int scale_per_row, const int8_t* zero_point, int zp_per_row, int qmin,
+                            int qmax, int8_t* q, float* x_scale, int8_t* x_zero_point, void* stream);
 /* Replaces _int_scaled_matmul + the epilogue (int8/kernels.py:114-144,
  * int8_tensor.py:305-359): y = bf16(bf16(acc_i32 * x_scale[m]) * w_scale[n] + bias[n]).
  * xq int8 [M,K], wq int8 [N,K] (K-major, i.e. the stored qdata), scales f32.         */
