@@ -75,6 +75,17 @@ __device__ __forceinline__ void tma_load_1d(void* dst, const void* tmap, uint64_
       "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "l"(policy)
       : "memory");
 }
+// plain bulk copy (no tensor map): `bytes` (a multiple of 16, both addresses 16-byte aligned) from global memory
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+// orders this thread's earlier global accesses (and what it acquired) before its later async-proxy ones (bulk_load)
+__device__ __forceinline__ void fence_proxy_async_global() {
+  asm volatile("fence.proxy.async.global;" ::: "memory");
+}
 __device__ __forceinline__ void tma_load_2d(void* dst, const void* tmap, uint64_t* bar, int c0,
                                             int c1, uint64_t policy) {
   asm volatile(

@@ -19,9 +19,15 @@
 // (which finishes that tile last) looks for it; only when the tile is split so finely that its contributors
 // have no other work do publish and gather run back to back.
 //
+// Staged gather (ts_gemm.cuh, where a partial fits a ring stage: Cfg::STAGE_PARTIALS).  Once the producer warp of an
+// owner has issued its last chunk, lane k of it waits for ring stage nunits + k to come back, acquires contributor
+// b+1+k's flag, and bulk-copies (cp.async.bulk, after fence.proxy.async) that partial's valid token columns into
+// the stage, for k < n_staged = min(b_last - b, STAGES).  These copies run while the consumers finish the owner's
+// last chunks.  The consumers add the staged partials from shared memory, then the rest from L2, in CTA order.
+//
 // Workspace (caller-owned, zero-initialised once): flags uint32[grid] at +0 (0 = empty, 1 = published; the owner
 // resets the flags it consumed, so the flags are all-zero again when the kernel ends), partial slots [grid][N_MMA * 128] 32-bit words at +64 KiB (slot b = CTA b's CONTRIB partial,
-// column-major: word (j, r) at j * 128 + r).
+// column-major: token j's 128 rows at j * 128, in the row order of part_word below).
 //
 // Forward progress: an owner spins on flags of CTAs with HIGHER block indices, of its own grid only.  The launchers
 // keep the grid at or below the SM count.  Decode kernels fit two CTAs per SM, so grid j+1 (PDL) shares the SMs with
@@ -33,6 +39,10 @@
 //     (the weights must be complete before grid j starts: a weight quantized by this library is separated from its
 //     first linear by ao_b200_pdl_fence, which quantize_ launches);
 //   * CTAs of j+1 that did not find room become resident as CTAs of j exit, which they do without waiting on j+1.
+// The staged gather adds no wait on another grid: its flags are the same flags of the same grid, polled by the
+// producer warp after its griddepcontrol.wait.  Inside the CTA, the stages it waits for are released by consumers
+// that wait on nothing but the ring before their last segment's epilogue, so the gatherer and the consumers cannot
+// wait on each other.
 //
 // Device-side grid (grouped GEMM, ts_gemm.cuh Grouped<Fmt>).  The units per expert come from offs, which only the
 // device reads, so the host launches a grid sized for an upper bound of U.  With more CTAs than units, unit_begin
@@ -86,6 +96,12 @@ struct Walk {
     return (s == 0 && (u0 % KT) != 0) ? SEG_CONTRIB : SEG_OWNER;
   }
 };
+
+// Word (token j, row r) of a partial slot.  STAGED (kernels that stage partials in shared memory): the rows of a token
+// column are XOR-permuted in blocks of 8 by bits 1..2 of j, so the four columns 2t + c (t = 0..3) of one fragment
+// access land on distinct shared-memory banks when the owner reads a slot copied verbatim into a ring stage
+template <bool STAGED>
+__device__ __forceinline__ int part_word(int j, int r) { return j * ROWS + (STAGED ? r ^ (((j >> 1) & 3) << 3) : r); }
 
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
   unsigned v;

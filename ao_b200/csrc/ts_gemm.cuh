@@ -173,6 +173,9 @@ struct Cfg {
   static constexpr int BAR_BYTES = 3 * STAGES * 8;   // wfull, xfull, sempty per stage
   static constexpr size_t SMEM_BYTES = (size_t)BAR_OFF + BAR_BYTES + 1024;   // + the 1024-byte alignment of the base
   static_assert(CTAS * (SMEM_BYTES + SMEM_RESERVED_PER_CTA) <= SMEM_PER_SM, "CTAs per SM do not fit");
+  // the owner's gather stages up to STAGES contributors' partials in the ring (see the producer) when one fits a stage;
+  // not for PROMOTE (e4m3 x e4m3): its bs=32 decode stack measured 5 % slower with it (DESIGN §4)
+  static constexpr bool STAGE_PARTIALS = !Fmt::PROMOTE && N_MMA * ROWS * 4 <= STAGE_BYTES;
 };
 
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
@@ -332,6 +335,35 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       }
       __syncwarp();
     }
+    if constexpr (C::STAGE_PARTIALS) {
+      // The gatherer: the partial of contributor b+1+k goes into ring position nunits + k (after the last chunk) as
+      // soon as that stage comes back and the flag is up, while the consumers still run the last chunks.  The
+      // consumers add them from shared memory in CTA order (epilogue, OWNER); contributors past the ring take the
+      // register path there.  Only the owner's valid token columns are copied
+      if (last_is_owner) {
+        const int tile = walk.seg_tile(seg_last);
+        const int b_last = streamk::cta_of_unit((long long)tile * p.KT + p.KT - 1, U, G);
+        const int n_staged = b_last - b < S ? b_last - b : S;
+        int m0 = (tile / p.n_tiles) * N_MMA, m_end = p.M;
+        if constexpr (GROUPED) {
+          const GroupTile gt = group_tile<N_MMA>(g_end, g_mbp, p.E, tile / p.n_tiles);
+          m0 = gt.row0;
+          m_end = gt.row_end;
+        }
+        const int cols = m_end - m0 < N_MMA ? m_end - m0 : N_MMA;
+        // one lane per contributor: the flags are polled at once, not one round trip after another
+        static_assert(S <= 32, "one gatherer lane per staged partial");
+        if (lane < n_staged) {
+          const int i = nunits + lane, s = i % S;
+          mbar_wait(&sempty[s], ((i / S) & 1) ^ 1);
+          while (streamk::ld_acquire_u32(p.ws_flag + b + 1 + lane) == 0u) __nanosleep(64);
+          fence_proxy_async_global();   // the contributor's st.cg stores, acquired above, before the bulk reads
+          mbar_expect_tx(&wfull[s], cols * ROWS * 4);
+          bulk_load(stage(s), p.ws_partial + (size_t)(b + 1 + lane) * (N_MMA * ROWS), cols * ROWS * 4, &wfull[s]);
+        }
+        __syncwarp();
+      }
+    }
   } else {
     // ------------------------------------------------------------ consumers: warpgroup wg owns rows 64wg .. 64wg+63
     if constexpr (C::CTAS > 1) setmaxnreg_inc<CONSUMER_REGS>();
@@ -366,7 +398,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         out_scale += gt.e;
       }
       if (kind == streamk::SEG_CONTRIB) {
-        // publish the partial (column-major slot: word (token j, row r) at j * 128 + r), then one gpu-scope release
+        // publish the partial (column-major slot, streamk::part_word), then one gpu-scope release
         uint32_t* slot = reinterpret_cast<uint32_t*>(p.ws_partial) + (size_t)b * (N_MMA * ROWS);
 #pragma unroll
         for (int q = 0; q < NACC / 4; ++q)
@@ -375,24 +407,45 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
 #pragma unroll
             for (int c = 0; c < 2; ++c) {
               const int col = 8 * q + 2 * t + c, r = row_lo + 8 * h;
-              if (m0 + col < m_end) __stcg(&slot[col * ROWS + r], v[4 * q + 2 * h + c]);
+              if (m0 + col < m_end) __stcg(&slot[streamk::part_word<C::STAGE_PARTIALS>(col, r)], v[4 * q + 2 * h + c]);
             }
         asm volatile("bar.sync 1, 256;" ::: "memory");   // all 128 rows stored (cta-scope order) ...
         if (warp == 4 && lane == 0) streamk::st_release_u32(p.ws_flag + b, 1u);   // ... then one gpu-scope release
         return;
       }
       if (kind == streamk::SEG_OWNER) {
-        // own partial + the partials of CTAs b+1 .. b_last in that order (fixed: bit-reproducible run to run)
-        // One warp polls the flags, on distinct lanes at once (one L2 round trip when they are up, not one per
-        // contributor), and the consumer barrier passes its acquire on; narrow tiles then load the partials of GB
-        // contributors before adding any of them
+        // own partial + the partials of CTAs b+1 .. b_last in that order (fixed: bit-reproducible run to run).
+        // The first n_staged arrive in ring stages (the producer's gatherer): each is added once its stage is full.
+        // For the rest, one warp polls the flags, on distinct lanes at once (one L2 round trip when they are up, not
+        // one per contributor), and the consumer barrier passes its acquire on; narrow tiles then load the partials of
+        // GB contributors before adding any of them
         const int b_last = streamk::cta_of_unit((long long)tile * p.KT + p.KT - 1, U, G);
-        if (warp == 4) streamk::wait_flags(p.ws_flag + b + 1, b_last - b, lane);
+        const int n_staged = !C::STAGE_PARTIALS ? 0 : (b_last - b < S ? b_last - b : S);
+        if (warp == 4) streamk::wait_flags(p.ws_flag + b + 1 + n_staged, b_last - b - n_staged, lane);
         asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll 1
+        for (int k = 0; k < n_staged; ++k) {
+          const int i = nunits + k, s = i % S;
+          mbar_wait(&wfull[s], (i / S) & 1);
+          const uint32_t part = smem_u32(stage(s));
+#pragma unroll
+          for (int q = 0; q < NACC / 4; ++q)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int cc = 0; cc < 2; ++cc) {
+                const int col = 8 * q + 2 * t + cc, r = row_lo + 8 * h, j = 4 * q + 2 * h + cc;
+                if (m0 + col < m_end) {
+                  const uint32_t o = lds32(part + streamk::part_word<C::STAGE_PARTIALS>(col, r) * 4);
+                  if constexpr (Fmt::EPI == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o);
+                  else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o));
+                }
+              }
+        }
         // registers: GB x NACC words of partials (restated by tests/streamk_model.py::group_width)
         constexpr int GB = NACC <= 8 ? 4 : (NACC <= 16 ? 2 : 1);
 #pragma unroll 1
-        for (int c = b + 1; c <= b_last && GB == 1; ++c) {
+        for (int c = b + 1 + n_staged; c <= b_last && GB == 1; ++c) {
           const uint32_t* slot = reinterpret_cast<const uint32_t*>(p.ws_partial) + (size_t)c * (N_MMA * ROWS);
 #pragma unroll
           for (int q = 0; q < NACC / 4; ++q) {
@@ -405,7 +458,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
               for (int cc = 0; cc < 2; ++cc) {
                 const int col = 8 * q + 2 * t + cc, r = row_lo + 8 * h, j = 4 * q + 2 * h + cc;
                 if (m0 + col < m_end) {
-                  const uint32_t o = __ldcg(slot + col * ROWS + r);
+                  const uint32_t o = __ldcg(slot + streamk::part_word<C::STAGE_PARTIALS>(col, r));
                   if constexpr (Fmt::EPI == EPI_I8) v[j] = (uint32_t)((int32_t)v[j] + (int32_t)o);
                   else v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(o));
                 }
@@ -413,7 +466,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           }
         }
 #pragma unroll 1
-        for (int c0 = b + 1; c0 <= b_last && GB > 1; c0 += GB) {
+        for (int c0 = b + 1 + n_staged; c0 <= b_last && GB > 1; c0 += GB) {
           uint32_t o[GB][NACC];
 #pragma unroll
           for (int gi = 0; gi < GB; ++gi) {
@@ -426,7 +479,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
 #pragma unroll
                 for (int cc = 0; cc < 2; ++cc) {
                   const int col = 8 * q + 2 * t + cc, r = row_lo + 8 * h, j = 4 * q + 2 * h + cc;
-                  o[gi][j] = m0 + col < m_end ? __ldcg(slot + col * ROWS + r) : 0u;
+                  o[gi][j] = m0 + col < m_end ? __ldcg(slot + streamk::part_word<C::STAGE_PARTIALS>(col, r)) : 0u;
                 }
           }
 #pragma unroll
