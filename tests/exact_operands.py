@@ -6,6 +6,9 @@ accumulates exactly in any order and under any stream-K split; the epilogue's sc
 well.  The kernel's bf16 output must then equal the fp64 reference rounded to bf16, bit for bit, in every element.
 Each builder asserts that premise before anything is compared.  Scales have mantissa bits set (int4 s, the e4m3
 block scales of nvfp4, the fp8 row scales), so the scale arithmetic is checked too, not only powers of two.
+
+The weight-only int8 and fp8 linears and mxfp4 round where their recipes round, so their references are not the fp64
+sum rounded once: the sum is exact in fp32 and the reference applies the recipe's own roundings to it (recipe()).
 """
 import torch
 
@@ -75,6 +78,28 @@ def premise(X, W, bias_acc=None, chunk=False):
         top_c = float(torch.einsum("mkc,nkc->mnk", Xp, Wp).max())
         assert top_c < 2.0**13 * u, f"premise: a 128-k chunk reaches {top_c / u:.0f} u >= 2^13 u"
     return u
+
+
+def recipe(op, acc, scale=None, bias=None):
+    """The bf16 output of a linear whose epilogue rounds as its reference does, from the exact sums acc (fp64 [M, n]):
+    int8wo bf16(bf16(bf16(acc) * bf16(scale)) + bias) (torch.mm in bf16, then the bf16 scale and bias);
+    fp8wo bf16(bf16(acc) + bias) (the weights are already bf16(e4m3 * scale)); mxfp4 bf16(fp32(acc) + bias)."""
+    fp32_exact(acc, f"{op}: the sums")
+    a = acc.float()
+    if op == "int8wo":
+        y = a.to(torch.bfloat16) * scale.to(torch.bfloat16)
+    elif op == "fp8wo":
+        y = a.to(torch.bfloat16)
+    elif op == "mxfp4":
+        return (a + bias.float()).to(torch.bfloat16) if bias is not None else a.to(torch.bfloat16)
+    else:
+        raise ValueError(op)
+    return y if bias is None else y + bias
+
+
+def mxfp4_value(codes, scale_bytes):
+    """fp64 e2m1 codes [R, K] times e8m0 bytes [R, K/32] (every byte here is a normal power of two)."""
+    return e2m1_value(codes) * pow2(scale_bytes.long() - 127).repeat_interleave(32, 1)[:, : codes.shape[1]]
 
 
 def bias_for(n, q, g):
@@ -150,7 +175,8 @@ def int4_weights(n, K, group_size, g):
 
 
 def build(op, M, N, K, seed=0, n_out=None, w_bytes=None, group_size=64):
-    """op: int4 | int8_dyn | int8_mm_i32 | fp8 | mxfp8 | nvfp4 | nvfp4w | nvfp4w_xs | nvfp4w_rowpts.
+    """op: int4 | int8_dyn | int8_mm_i32 | fp8 | mxfp8 | nvfp4 | nvfp4w | nvfp4w_xs | nvfp4w_rowpts | int8wo | fp8wo |
+    mxfp4.
     n_out: int4 output features (<= N).  w_bytes: nvfp4 weight scale bytes [N, K/16] (default: a window of normal
     bytes with mantissa bits set).  group_size: int4 (32, 64, 128 or 256).  The value windows are fixed and the
     premise is checked on the drawn values: for the test shapes (K <= 16384, M x N small); served() picks the windows
@@ -270,6 +296,52 @@ def build(op, M, N, K, seed=0, n_out=None, w_bytes=None, group_size=64):
         bpf = bp.float()
         return Case(op, "nvfp4", M, N, K, N, prod + bias,
                     lambda m: o.nvfp4_weight_linear(x[:m], rsf[:m] if rsf is not None else None, wq, wsb, bpf, b))
+    if op == "int8wo":
+        # any int8 weight; scales with 12 significant bits over 13 binades, so bf16(scale) rounds
+        X = randint(-8, 8, (M, K), g).double() * 2.0**-3
+        wq = randint(-128, 127, (N, K), g).to(torch.int8)
+        premise(X, wq.double())
+        s = (randint(2048, 4095, (N,), g).double() * 2.0**-20 * pow2(randint(-6, 6, (N,), g))).float()
+        assert not torch.equal(s.to(torch.bfloat16).float(), s), "premise: bf16(scale) rounds"
+        b = (torch.randn(N, device=DEV, generator=g) * 4.0).to(torch.bfloat16)
+        x = X.to(torch.bfloat16)
+        return Case(op, "int8wo", M, N, K, N, None, lambda m: o.int8_weight_linear(x[:m], wq, s, b),
+                    ref=recipe(op, X @ wq.double().t(), s, b))
+    if op == "fp8wo":
+        # codes c/8, row scales odd * 2^p over nine binades: bf16(e4m3 * s) = c * s exactly, and each output
+        # feature's products are multiples of its own quantum 2^(p-6)
+        X = randint(-8, 8, (M, K), g).double() * 2.0**-3
+        c = randint(-7, 7, (N, K), g).double() * 2.0**-3
+        p = randint(-12, -4, (N,), g)
+        s = (pick([3, 5, 7], (N,), g) * pow2(p)).float()
+        wq = c.to(torch.float8_e4m3fn)
+        W = (wq.float() * s[:, None]).to(torch.bfloat16).double()   # the reference's dequantize
+        assert torch.equal(W, c * s.double()[:, None]), "premise: e4m3 * scale exact in bf16"
+        assert bool(((X.abs() @ W.abs().t()) < 2.0**24 * 2.0**-6 * pow2(p)[None, :]).all()), "premise: sums < 2^24 quanta"
+        b = (torch.randn(N, device=DEV, generator=g) * 4.0).to(torch.bfloat16)
+        x = X.to(torch.bfloat16)
+        return Case(op, "fp8wo", M, N, K, N, None, lambda m: o.fp8_weight_linear(x[:m], wq, s, b),
+                    ref=recipe(op, X @ W.t(), bias=b))
+    if op == "mxfp4":
+        # every e2m1 code; e8m0 bytes from 80..171 per row (x) or feature (w), +1 in some blocks: each (m, n) sums
+        # multiples of its own quantum 2^-2 2^(x byte + w byte - 254) of the lowest bytes
+        nb = -(-K // 32)
+        xc, wc = randint(0, 15, (M, K), g), randint(0, 15, (N, K), g)
+        xs = randint(80, 170, (M, 1), g) + randint(0, 1, (M, nb), g)
+        ws = randint(80, 170, (N, 1), g) + randint(0, 1, (N, nb), g)
+        X, W = mxfp4_value(xc, xs), mxfp4_value(wc, ws)
+        u = 0.25 * pow2(xs.min(1).values[:, None] + ws.min(1).values[None, :] - 254)
+        assert bool(((X.abs() @ W.abs().t()) < 2.0**24 * u).all()), "premise: sums < 2^24 quanta"
+        b = (torch.randn(N, device=DEV, generator=g) * 2.0**20).to(torch.bfloat16)
+        xq, wq = pack_e2m1(xc), pack_e2m1(wc)
+        xs8, wsb = xs.to(torch.uint8), to_blocked(ws.to(torch.uint8))
+        cache = {}
+
+        def run(m):
+            if m not in cache:
+                cache[m] = to_blocked(xs8[:m])
+            return o.mxfp4_linear(xq[:m], cache[m], wq, wsb, b)
+        return Case(op, "mxfp4", M, N, K, N, None, run, ref=recipe(op, X @ W.t(), bias=b))
     raise ValueError(op)
 
 
@@ -353,6 +425,12 @@ def served_candidates(op):
         return [dict(xr=3, wb=list(range(0x30, 0x34)), odd=[3, 5, 7], bp=1.25),
                 dict(xr=1, wb=[0x30, 0x34], odd=[3, 5, 7], bp=1.25),
                 dict(xr=1, wb=[0x30, 0x34], odd=[3], bp=0.75)]
+    if op == "int8wo":
+        return [dict(xr=r) for r in (8, 4, 2, 1)]
+    if op == "fp8wo":
+        return [dict(xr=a, wr=b) for a, b in ((8, 7), (4, 7), (2, 3), (1, 1))]
+    if op == "mxfp4":
+        return [dict(xc=list(range(16)), d=1), dict(xc=list(range(16)), d=0), dict(xc=E2M1_UPTO1, d=0)]
     raise ValueError(op)
 
 
@@ -376,6 +454,13 @@ def factors(op, win):
         epi = [] if op == "nvfp4w" else [span([o * 2.0**-6 for o in win["odd"]])]
         epi.append(span([o * 2.0**-4 for o in win["odd"]]) if op == "nvfp4w_rowpts" else span([win["bp"]]))
         return [span(_codes(win["xr"], 0.5))], [span(E2M1), span([_e4m3(b) for b in win["wb"]])], epi
+    if op == "int8wo":
+        return [span(_codes(win["xr"], 2.0**-3))], [span(list(range(-128, 128)))], []
+    if op == "fp8wo":   # bf16(e4m3 * scale) = (c / 8) * odd * 2^-8, odd in {3, 5, 7}
+        return [span(_codes(win["xr"], 2.0**-3))], [span(_codes(win["wr"], 2.0**-3)), span([3.0, 5.0, 7.0])], []
+    if op == "mxfp4":
+        pw = span([2.0**j for j in range(win["d"] + 1)])
+        return [span([E2M1[c] for c in win["xc"]]), pw], [span(E2M1), pw], []
     raise ValueError(op)
 
 
@@ -384,8 +469,8 @@ def bound(op, K, win):
     and 128 max|X| max|W| for the e4m3 chunk.  Exact when the first is < 2^24 and the second < 2^13."""
     xf, wf, ef = factors(op, win)
     xw = units(xf) * units(wf)
-    if op in ("int8_dyn", "int8_mm_i32"):
-        return K * xw, None   # the int32 sum converts to fp32 exactly; the epilogue rounds as the reference does
+    if op in ("int8_dyn", "int8_mm_i32", "int8wo", "fp8wo", "mxfp4"):
+        return K * xw, None   # the sum is exact in fp32; the epilogue rounds as the reference does (recipe())
     return K * xw * units(ef) + BIAS_UNITS, (128 * xw if op == "fp8" else None)
 
 
@@ -589,4 +674,50 @@ def served(op, M, N, K, seed=0, group_size=32, n_out=None, x_seed=None):
         rsf, bpf, b = (rs.float() if rs is not None else None), bp.float(), bias.to(torch.bfloat16)
         return Case(op, "nvfp4", M, N, K, N, None,
                     lambda m: o.nvfp4_weight_linear(x[:m], rsf[:m] if rsf is not None else None, wq, wsb, bpf, b), ref=ref)
+    if op == "int8wo":
+        X = randint(-win["xr"], win["xr"], (M, K), gx).double() * 2.0**-3
+        s = (randint(2048, 4095, (N,), gw).double() * 2.0**-20 * pow2(randint(-6, 6, (N,), gw))).float()
+        b = (randint(-127, 127, (N,), gx).double() * 2.0**-4).to(torch.bfloat16)
+
+        def make(nb):
+            wq = randint(-128, 127, (nb, K), gw).to(torch.int8)
+            return wq.double(), wq
+        ref = _reference(op, X, N, blocks(N, make), lambda acc, n0, n1: recipe(op, acc, s[n0:n1], b[n0:n1]).double(), False)
+        x, wq = X.to(torch.bfloat16), torch.cat(parts, 0)
+        c = Case(op, "int8wo", M, N, K, N, None, lambda m: o.int8_weight_linear(x[:m], wq, s, b), ref=ref)
+        c.inputs = [x, b]
+        return c
+    if op == "fp8wo":
+        X = randint(-win["xr"], win["xr"], (M, K), gx).double() * 2.0**-3
+        s = (pick([3, 5, 7], (N,), gw) * 2.0**-8).float()
+        b = (randint(-127, 127, (N,), gx).double() * 2.0**-4).to(torch.bfloat16)
+
+        def make(nb):
+            wq = (randint(-win["wr"], win["wr"], (nb, K), gw).double() * 2.0**-3).to(torch.float8_e4m3fn)
+            return (wq.float() * s[len(parts) * W_BLOCK:][:nb, None]).to(torch.bfloat16).double(), wq
+        ref = _reference(op, X, N, blocks(N, make), lambda acc, n0, n1: recipe(op, acc, bias=b[n0:n1]).double(), False)
+        x, wq = X.to(torch.bfloat16), torch.cat(parts, 0)
+        c = Case(op, "fp8wo", M, N, K, N, None, lambda m: o.fp8_weight_linear(x[:m], wq, s, b), ref=ref)
+        c.inputs = [x, b]
+        return c
+    if op == "mxfp4":
+        xc = pick(win["xc"], (M, K), gx).long()
+        xs = 126 + randint(0, win["d"], (M, K // 32), gx)
+        X = mxfp4_value(xc, xs)
+        b = (randint(-127, 127, (N,), gx).double() * 2.0**-4).to(torch.bfloat16)
+
+        def make(nb):
+            wc = randint(0, 15, (nb, K), gw)
+            ws = 125 + randint(0, win["d"], (nb, K // 32), gw)
+            return mxfp4_value(wc, ws), (pack_e2m1(wc), ws.to(torch.uint8))
+        ref = _reference(op, X, N, blocks(N, make), lambda acc, n0, n1: recipe(op, acc, bias=b[n0:n1]).double(), False)
+        xq, wq = pack_e2m1(xc), torch.cat([p[0] for p in parts], 0)
+        xs8, wsb = xs.to(torch.uint8), to_blocked(torch.cat([p[1] for p in parts], 0))
+        cache = {}
+
+        def run(m):
+            if m not in cache:
+                cache[m] = to_blocked(xs8[:m])
+            return o.mxfp4_linear(xq[:m], cache[m], wq, wsb, b)
+        return Case(op, "mxfp4", M, N, K, N, None, run, ref=ref)
     raise ValueError(op)

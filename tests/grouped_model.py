@@ -1,4 +1,4 @@
-"""A CPU restatement of the grouped schedule of ts_gemm_kernel<SsFmt<F8>, N_MMA, GROUPED> (torch._grouped_mm), for tests.
+"""A CPU restatement of the grouped schedule of ts_gemm_kernel<Grouped<Fmt>, N_MMA> (torch._grouped_mm), for tests.
 
 It mirrors `grouped_schedule`, `group_tile` and `grouped_grid` of ao_b200/csrc/ts_gemm.cuh and the upper-bound grid of
 `launch_gemm<..., GROUPED>`; the walk of each CTA is streamk_model.walk.  Keep the two in step: a change to the grouped
@@ -81,6 +81,7 @@ class GroupedPlan:
     U_bound: int
     G_host: int
     G: int
+    fmt: str = "fp8"
     ctas: list = field(default_factory=list)     # ctas[b] = list of streamk_model.Seg (b < G)
     owners: dict = field(default_factory=dict)   # split tile -> (owner CTA, [contributor CTAs])
 
@@ -89,19 +90,30 @@ class GroupedPlan:
         e, row0, row_end = group_tile(self.ends, self.mbp, t // self.n_tiles, self.width)
         return e, row0, row_end, t % self.n_tiles
 
+    def contributor_counts(self):
+        return [len(c) for _, c in self.owners.values()]
 
-def plan(offs, M, N, K, grid=None, sm=132):
-    """The grouped split for one launch: grid None = the heuristic, else the forced CTA count."""
+    def gather_split(self, c):
+        return sk.gather_split(self.fmt, self.width, True, c)
+
+    def owner_cols(self, t):
+        """Valid token columns of tile t: the rows of its expert from its first row on, at most the width."""
+        _, row0, row_end, _ = self.tile(t)
+        return min(row_end - row0, self.width)
+
+
+def plan(offs, M, N, K, grid=None, sm=132, fmt="fp8"):
+    """The grouped split of one launch of Grouped<fmt>: grid None = the heuristic, else the forced CTA count."""
     E = len(offs)
-    width = sk.n_mma("fp8", M)
-    KT = sk.k_chunks("fp8", K)
+    width = sk.n_mma(fmt, M)
+    KT = sk.k_chunks(fmt, K)
     n_tiles = -(-N // sk.ROWS)
     ends = row_ends(offs, M)
     mbp = mblock_prefix(ends, width)
     U = n_tiles * mbp[-1] * KT
     U_bound, G_host = host_grid(M, E, n_tiles, KT, width, grid or 0, sm)
     G = grouped_grid(G_host, U, bool(grid))
-    p = GroupedPlan(M, N, K, E, width, n_tiles, KT, ends, mbp, U, U_bound, G_host, G)
+    p = GroupedPlan(M, N, K, E, width, n_tiles, KT, ends, mbp, U, U_bound, G_host, G, fmt)
     for b in range(G):
         u0, u1 = sk.unit_begin(b, U, G), sk.unit_begin(b + 1, U, G)
         p.ctas.append(sk.walk(u0, u1 - u0, KT) if u1 > u0 else [])

@@ -1,9 +1,10 @@
 """A CPU restatement of the stream-K work split of the quantized GEMM kernel, for tests.
 
-It mirrors `unit_begin`, `cta_of_unit` and `Walk` of ao_b200/csrc/streamk.cuh, the grid choice and the partial
-group width `GB` of ao_b200/csrc/ts_gemm.cuh, and the token-tile width and K-chunk count each launcher picks.  Keep
-the two in step: a change to the walk there needs the same change here, or test_streamk_plan.py and the messages of
-test_exact_gemm_gpu.py describe a split the kernel does not run.
+It mirrors `unit_begin`, `cta_of_unit` and `Walk` of ao_b200/csrc/streamk.cuh, the grid choice, the ring (`Cfg`,
+`ctas_per_sm`) and the partial group width `GB` of ao_b200/csrc/ts_gemm.cuh, and the token-tile width and K-chunk
+count each launcher picks.  Keep the two in step: a change to the walk or to a format's stage layout there needs the
+same change here, or test_streamk_plan.py and the messages of test_exact_gemm_gpu.py describe a split the kernel does
+not run.
 """
 from dataclasses import dataclass, field
 
@@ -14,7 +15,48 @@ KIND_NAMES = {FULL: "FULL", CONTRIB: "CONTRIB", OWNER: "OWNER"}
 
 # token-tile widths each format's launcher can pick (fp8 keeps a second accumulator per chunk: 64 at most)
 WIDTHS = {"int4": (16, 32, 64, 128), "int8": (16, 32, 64, 128), "fp8": (16, 32, 64), "mxfp8": (16, 32, 64, 128),
-          "nvfp4": (16, 32, 64, 128)}
+          "nvfp4": (16, 32, 64, 128), "mxfp4": (16, 32, 64, 128), "int8wo": (16, 32, 64, 128),
+          "fp8wo": (16, 32, 64, 128)}
+
+# Each format policy's stage layout, from its Fmt struct: (W_BYTES, AUX_BYTES, X_ELEM_BYTES, DECODE_2CTA, PROMOTE,
+# MAX_N_MMA).  int8 is SsFmt<KIND_I8>, fp8 SsFmt<KIND_F8> (e4m3 x e4m3), int8wo Int8WoFmt, fp8wo Fp8WoFmt.
+POLICIES = {
+    "int4": (8192, 2048, 2, True, False, 128),
+    "int8": (16384, 0, 1, True, False, 128),
+    "fp8": (16384, 0, 1, False, True, 64),
+    "mxfp8": (16384, 512, 2, False, False, 128),
+    "mxfp4": (8192, 512, 2, False, False, 128),
+    "nvfp4": (8192, 1024, 2, False, False, 128),
+    "int8wo": (16384, 0, 2, True, False, 128),
+    "fp8wo": (16384, 512, 2, False, False, 128),
+}
+SMEM_PER_SM, RESERVED_PER_CTA, MAX_STAGES = 228 * 1024, 1024, 12
+
+
+def ring(fmt, width, grouped=False):
+    """(STAGE_BYTES, CTAS, STAGES, STAGE_PARTIALS) of ts_gemm.cuh Cfg<Fmt, width> (Grouped<Fmt> when grouped): two CTAs
+    per SM for decode tiles of a DECODE_2CTA format (ctas_per_sm), and an owner stages up to STAGES partials in the
+    ring when one (width x 128 fp32) fits a stage, except under PROMOTE."""
+    w, aux, xe, two, promote, max_n = POLICIES[fmt]
+    assert width in WIDTHS[fmt] and width <= max_n, (fmt, width)
+    stage = w + ((aux + 1023) & ~1023) + width * KCHUNK * xe
+    ctas = 2 if width <= 32 and two and not grouped else 1
+    fit = 200 * 1024 // stage if ctas == 1 else (SMEM_PER_SM // 2 - RESERVED_PER_CTA - 1024) // (stage + 24)
+    return stage, ctas, min(fit, MAX_STAGES), not promote and width * ROWS * 4 <= stage
+
+
+def ring_smem(fmt, width, grouped=False):
+    """Cfg::SMEM_BYTES: the ring, its barriers (3 x 8 bytes per stage) and the 1024-byte alignment of the base."""
+    stage, _, stages, _ = ring(fmt, width, grouped)
+    return stages * stage + 3 * stages * 8 + 1024
+
+
+def gather_split(fmt, width, grouped, c):
+    """(staged, through registers) of an owner with c contributors: the first min(c, STAGES) arrive in ring stages
+    when the kernel stages partials, the rest are read from L2 in groups of GB."""
+    _, _, stages, staging = ring(fmt, width, grouped)
+    n = min(c, stages) if staging else 0
+    return n, c - n
 
 
 def n_mma(fmt, M):
@@ -103,6 +145,13 @@ class Plan:
 
     def contributor_counts(self):
         return [len(c) for _, c in self.owners.values()]
+
+    def gather_split(self, c):
+        return gather_split(self.fmt, self.width, False, c)
+
+    def owner_cols(self, t):
+        """Valid token columns of tile t (the columns an owner's gather copies)."""
+        return min(self.M - (t // self.n_tiles) * self.width, self.width)
 
     def tile_of(self, m, n):
         return (m // self.width) * self.n_tiles + n // ROWS

@@ -2,7 +2,8 @@
 
 The decode instantiations of ts_gemm_kernel (N_MMA 16 and 32) of the formats with Fmt::DECODE_2CTA must launch with
 at most 80 registers per thread (65536 / (2 x 384), rounded down to the allocation granule of 8), and their shared
-memory (ts_gemm.cuh Cfg::SMEM_BYTES, restated here) plus the 1 KB reserved per CTA must fit twice into the SM's 228 KB.
+memory (ts_gemm.cuh Cfg::SMEM_BYTES, restated by streamk_model.ring) plus the 1 KB reserved per CTA must fit twice
+into the SM's 228 KB.
 """
 import os
 import re
@@ -11,21 +12,20 @@ import subprocess
 
 import pytest
 
+from streamk_model import MAX_STAGES, RESERVED_PER_CTA, SMEM_PER_SM, ring, ring_smem  # noqa: F401 (re-exported)
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "ao_b200", "lib", "libao_b200.so")
 
-SMEM_PER_SM, RESERVED_PER_CTA, MAX_STAGES = 228 * 1024, 1024, 12
-# Fmt with DECODE_2CTA: (W_BYTES, AUX_BYTES, X_ELEM_BYTES) of one 128-k chunk, from the format policies
-FORMATS = {"Int4Fmt": (8192, 2048, 2), "SsFmt<0>": (16384, 0, 1)}
+# Fmt with DECODE_2CTA whose decode tiles this file checks: the kernel's name -> streamk_model's format
+FORMATS = {"Int4Fmt": "int4", "SsFmt<0>": "int8"}
 
 
 def cfg(fmt, n_mma):
     """(stages, SMEM_BYTES) as ts_gemm.cuh Cfg<Fmt, N_MMA> computes them."""
-    w, aux, xe = FORMATS[fmt]
-    stage = w + ((aux + 1023) & ~1023) + n_mma * 128 * xe
-    fit = 200 * 1024 // stage if n_mma > 32 else (SMEM_PER_SM // 2 - RESERVED_PER_CTA - 1024) // (stage + 24)
-    stages = min(fit, MAX_STAGES)
-    return stages, stages * stage + 3 * stages * 8 + 1024
+    _, ctas, stages, _ = ring(FORMATS[fmt], n_mma)
+    assert ctas == 2
+    return stages, ring_smem(FORMATS[fmt], n_mma)
 
 
 def resource_usage():

@@ -13,7 +13,8 @@ import pytest
 import torch
 import torch.nn as nn
 
-from test_decode_residency import MAX_STAGES, SMEM_PER_SM, RESERVED_PER_CTA, resource_usage
+import streamk_model as sk
+from test_decode_residency import SMEM_PER_SM, RESERVED_PER_CTA, resource_usage
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
@@ -386,9 +387,8 @@ def test_tiles_registers_stack_and_shared_memory(n_mma):
     reg, stack = usage[("Fp8WoFmt", n_mma)]
     assert reg <= (80 if two else 168), (reg, two)
     assert stack == 0, f"ts_gemm_kernel<Fp8WoFmt, {n_mma}>: {stack} bytes of stack"
-    stage = 128 * 128 + 1024 + n_mma * 128 * 2   # ts_gemm.cuh Cfg: the e4m3 chunk, the scale slot, the bf16 tile
-    fit = (SMEM_PER_SM // 2 - RESERVED_PER_CTA - 1024) // (stage + 24) if two else 200 * 1024 // stage
-    stages = min(fit, MAX_STAGES)
-    smem = stages * stage + 3 * stages * 8 + 1024
+    _, ctas, stages, _ = sk.ring("fp8wo", n_mma)
+    smem = sk.ring_smem("fp8wo", n_mma)
+    assert ctas == (2 if two else 1)
     assert stages >= 2
     assert (2 if two else 1) * (smem + RESERVED_PER_CTA) <= SMEM_PER_SM

@@ -63,7 +63,7 @@ def gm_offs(rows):
 
 def grids_of(case_rows, N, K, tail, grids, sm):
     M = sum(case_rows) + tail
-    p = gnm.plan(gm_offs(case_rows), M, N, K, grid=1, sm=sm)
+    p = gnm.plan(gm_offs(case_rows), M, N, K, grid=1, sm=sm, fmt="fp8wo")
     top = min(p.U_bound, sm)
     return list(range(1, top + 1)) if grids is None else [G for G in grids if G <= top]
 
@@ -137,7 +137,7 @@ def _sweep(ops, set_ctas, case, grids, what):
     wrong = [(G, b, r) for G, b, r in zip(grids, bad, raised) if b or r]
     if wrong:
         G, nb, nr = wrong[0]
-        p = gnm.plan(case.offs.tolist(), case.M, case.N, case.K, grid=G, sm=ex.sm_count())
+        p = gnm.plan(case.offs.tolist(), case.M, case.N, case.K, grid=G, sm=ex.sm_count(), fmt="fp8wo")
         pytest.fail(f"{what} M={case.M} N={case.N} K={case.K} E={case.E} grid={G or 'default'}: {nb} wrong elements, "
                     f"{nr} flags left raised (U={p.U}, width {p.width}, device grid {p.G} of {p.G_host}); "
                     f"{len(wrong)} of {len(grids)} launches wrong")

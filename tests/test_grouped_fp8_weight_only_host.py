@@ -25,7 +25,7 @@ import torch.nn.functional as F
 
 import grouped_nvfp4_model as gnm
 import streamk_model as sk
-from test_decode_residency import LIB, MAX_STAGES, RESERVED_PER_CTA, SMEM_PER_SM
+from test_decode_residency import LIB, RESERVED_PER_CTA, SMEM_PER_SM
 from test_float8_weight_only_host import bf16_round, dequantize_ref, f32, same_bits_or_both_nan, same_codes
 from test_float8_weight_only_host import within_one_step_of_the_sum
 from test_grouped_schedule import _cum, _offs_cases
@@ -88,7 +88,7 @@ def plan(offs, M, N, K, grid=None, sm=132):
     """The grouped split of one launch: the nvfp4 plan, whose token tiles (16 .. 128) are this format's too, with the
     K tail of the 8-bit kinds (ceil(K / 128) chunks, zero-filled)."""
     assert sk.WIDTHS["mxfp8"] == sk.WIDTHS["nvfp4"] and sk.k_chunks("mxfp8", K) == -(-K // 128)
-    return gnm.plan(offs, M, N, K, grid=grid, sm=sm)
+    return gnm.plan(offs, M, N, K, grid=grid, sm=sm, fmt="fp8wo")
 
 
 def _check(offs, M, N, K, grid, sm=132):
@@ -202,17 +202,14 @@ def test_issue_w_rows_loads_each_experts_rows_and_scales(E, N, K):
 
 
 # ------------------------------------------------------------------------------------------------ residency
-STAGE = (16384, 512, 2)   # Fp8WoFmt: W_BYTES, AUX_BYTES, X_ELEM_BYTES of one 128-k chunk
 TABLE_BYTES = 4 * (1024 + 1025)   # s_end[MAX_EXPERTS] + s_mbp[MAX_EXPERTS + 1]
 
 
 def test_grouped_tables_fit_beside_the_ring_one_cta_per_sm():
     for n_mma in (16, 32, 64, 128):
-        w, aux, xe = STAGE
-        stage = w + ((aux + 1023) & ~1023) + n_mma * 128 * xe
-        stages = min(200 * 1024 // stage, MAX_STAGES)
-        smem = stages * stage + 3 * stages * 8 + 1024
-        assert stages >= 2
+        _, ctas, stages, _ = sk.ring("fp8wo", n_mma, grouped=True)
+        smem = sk.ring_smem("fp8wo", n_mma, grouped=True)
+        assert ctas == 1 and stages >= 2
         assert smem + TABLE_BYTES <= 227 * 1024 and smem + TABLE_BYTES + RESERVED_PER_CTA <= SMEM_PER_SM, n_mma
 
 

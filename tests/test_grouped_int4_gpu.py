@@ -56,7 +56,7 @@ def gm_offs(rows):
 
 def grids_of(case_rows, N_out, K, tail, grids, sm):
     M = sum(case_rows) + tail
-    p = gnm.plan(gm_offs(case_rows), M, N_out, K, grid=1, sm=sm)
+    p = gnm.plan(gm_offs(case_rows), M, N_out, K, grid=1, sm=sm, fmt="int4")
     top = min(p.U_bound, sm)
     return list(range(1, top + 1)) if grids is None else [G for G in grids if G <= top]
 
@@ -137,7 +137,7 @@ def _sweep(ops, set_ctas, case, grids, what):
     wrong = [(G, b, r) for G, b, r in zip(grids, bad, raised) if b or r]
     if wrong:
         G, nb, nr = wrong[0]
-        p = gnm.plan(case.offs.tolist(), case.M, case.N_out, case.K, grid=G, sm=ex.sm_count())
+        p = gnm.plan(case.offs.tolist(), case.M, case.N_out, case.K, grid=G, sm=ex.sm_count(), fmt="int4")
         pytest.fail(f"{what} M={case.M} N_out={case.N_out} K={case.K} g={case.g} E={case.E} grid={G or 'default'}: "
                     f"{nb} wrong elements, {nr} flags left raised (U={p.U}, width {p.width}, device grid {p.G} of "
                     f"{p.G_host}); {len(wrong)} of {len(grids)} launches wrong")

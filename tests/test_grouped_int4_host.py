@@ -23,7 +23,7 @@ import torch
 
 import grouped_nvfp4_model as gnm
 import streamk_model as sk
-from test_decode_residency import LIB, MAX_STAGES, RESERVED_PER_CTA, SMEM_PER_SM
+from test_decode_residency import LIB, RESERVED_PER_CTA, SMEM_PER_SM
 from test_grouped_schedule import _cum, _offs_cases
 
 
@@ -84,7 +84,7 @@ def plan(offs, M, N_out, K, grid=None, sm=132):
     """The grouped split of one int4 launch: the nvfp4 plan, whose token tiles (16 .. 128) and whole 128-k chunks are
     int4's too; the tiles cover the N_out output features."""
     assert sk.WIDTHS["int4"] == sk.WIDTHS["nvfp4"] and sk.k_chunks("int4", K) == sk.k_chunks("nvfp4", K)
-    return gnm.plan(offs, M, N_out, K, grid=grid, sm=sm)
+    return gnm.plan(offs, M, N_out, K, grid=grid, sm=sm, fmt="int4")
 
 
 # (N padded, N_out, K): N tails inside the last tile, N a multiple of 128, several n-tiles
@@ -191,20 +191,17 @@ def test_issue_w_rows_addresses_each_experts_block(E, N, K):
 
 
 # ------------------------------------------------------------------------------------------------ residency
-INT4 = (8192, 2048, 2)   # Int4Fmt: W_BYTES, AUX_BYTES, X_ELEM_BYTES of one 128-k chunk
 TABLE_BYTES = 4 * (1024 + 1025)   # s_end[MAX_EXPERTS] + s_mbp[MAX_EXPERTS + 1]
 
 
 def test_grouped_tables_fit_beside_the_ring_one_cta_per_sm():
     for n_mma in (16, 32, 64, 128):
-        w, aux, xe = INT4
-        stage = w + ((aux + 1023) & ~1023) + n_mma * 128 * xe
-        stages = min(200 * 1024 // stage, MAX_STAGES)
-        smem = stages * stage + 3 * stages * 8 + 1024
+        _, ctas, _, _ = sk.ring("int4", n_mma, grouped=True)
+        smem = sk.ring_smem("int4", n_mma, grouped=True)
+        assert ctas == 1
         assert smem + TABLE_BYTES <= 227 * 1024 and smem + TABLE_BYTES + RESERVED_PER_CTA <= SMEM_PER_SM, n_mma
         # two CTAs with the dense decode ring (6 stages of a 32-wide tile) and the tables would not fit
-    stage32 = w + aux + 32 * 128 * xe
-    assert 2 * (6 * stage32 + 3 * 6 * 8 + 1024 + TABLE_BYTES + RESERVED_PER_CTA) > SMEM_PER_SM
+    assert 2 * (sk.ring_smem("int4", 32) + TABLE_BYTES + RESERVED_PER_CTA) > SMEM_PER_SM
 
 
 def test_grouped_int4_kernels_have_no_stack():

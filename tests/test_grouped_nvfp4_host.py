@@ -19,7 +19,7 @@ import torch
 import grouped_model as gm
 import grouped_nvfp4_model as gnm
 import streamk_model as sk
-from test_decode_residency import LIB, MAX_STAGES, RESERVED_PER_CTA, SMEM_PER_SM
+from test_decode_residency import LIB, RESERVED_PER_CTA, SMEM_PER_SM
 from test_grouped_schedule import _cum, _offs_cases
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -190,16 +190,14 @@ def test_stacked_blocked_scales_are_the_reference_layout():
 
 
 # ------------------------------------------------------------------------------------------------ residency
-NVFP4 = (8192, 1024, 2)   # Nvfp4Fmt: W_BYTES, AUX_BYTES, X_ELEM_BYTES of one 128-k chunk
 TABLE_BYTES = 4 * (1024 + 1025)   # s_end[MAX_EXPERTS] + s_mbp[MAX_EXPERTS + 1]
 
 
 def test_grouped_tables_fit_beside_the_ring():
     for n_mma in (16, 32, 64, 128):
-        w, aux, xe = NVFP4
-        stage = w + ((aux + 1023) & ~1023) + n_mma * 128 * xe
-        stages = min(200 * 1024 // stage, MAX_STAGES)
-        smem = stages * stage + 3 * stages * 8 + 1024
+        _, ctas, _, _ = sk.ring("nvfp4", n_mma, grouped=True)
+        smem = sk.ring_smem("nvfp4", n_mma, grouped=True)
+        assert ctas == 1
         assert smem + TABLE_BYTES <= 227 * 1024 and smem + TABLE_BYTES + RESERVED_PER_CTA <= SMEM_PER_SM, n_mma
 
 
