@@ -1,11 +1,13 @@
 // Swap-AB streaming GEMMs for 8-bit / 4-bit operands on Hopper wgmma (sm_90a), all on the kernel of ts_gemm.cuh:
 //   int8 x int8 -> int32  (wgmma s8, both operands TMA tiles)      replaces aten._int_mm + the scale epilogue
+//                         and, per expert, aten._int_mm on select()ed int8 expert weights
 //   e4m3 x e4m3 -> f32    (wgmma e4m3, both operands TMA tiles)    replaces torch._scaled_mm rowwise
 //   mxfp8 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm block-scaled
 //   nvfp4 block-16 e4m3   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm fp4 + pts/bias kernels
 //   nvfp4 weight x bf16   (bf16 wgmma, weights dequantised exactly)      replaces F.linear on the dequantised weight
 //   mxfp4 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces F.linear on both dequantize()s
 //   int8 weight x bf16    (bf16 wgmma, weights converted exactly)        replaces torch.mm on qdata.to(bf16) + the scale
+//                         and, per expert, the same on select()ed int8 expert weights
 //   e4m3 weight x bf16    (bf16 wgmma, weights dequantised per element)  replaces torch.matmul on the dequantised weight
 //                         and, per expert, torch._grouped_mm on the dequantised expert weights
 // Reference call sites: int8/kernels.py:18-76,114-144 + int8_tensor.py:305-359;
@@ -279,6 +281,15 @@ struct Int8WoFmt {
                                                  uint8_t* w_dst, uint8_t*, uint64_t* bar, int n_tile, int kc,
                                                  uint64_t policy) {
     tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
+  }
+  // grouped kernels: 128 rows from `row` = e*N + 128t of the [E * N, K] map of all experts' weights.  No aux box: the
+  // EPI_BF16_WSCALE epilogue reads w_scale[e*N + n] itself, so N needs no alignment.  A tile past N reads the next
+  // expert's rows (or the map's zero fill); each output row depends on its own weight row only, and the epilogue skips
+  // the features >= N
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, const CUtensorMap*, const tsg::Params&,
+                                                      uint8_t* w_dst, uint8_t*, uint64_t* bar, int row, int kc,
+                                                      uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, row, policy);
   }
   // the thread's two fragment rows: for k16 step kk the bytes of k 16kk + 2t + (0, 8, 1, 9), so that each bf16x2 lane
   // finds its byte at its own bits 7:0 (k 2t, 2t + 1) or 15:8 (k 2t + 8, 2t + 9)
@@ -633,6 +644,66 @@ extern "C" int ao_fp8_weight_grouped_mm(const uint16_t* x, int M, int K, const u
   p.E = E;
   p.M = M; p.N = N; p.N_out = N; p.K = K;
   return tsg::run<Fmt>(p, tm_w, tm_s, x, K, workspace, workspace_bytes, "fp8 weight grouped mm",
+                       reinterpret_cast<cudaStream_t>(stream));
+}
+
+// torch._grouped_mm(x, W.transpose(-2, -1), offs) on weight-only int8 expert weights, 2-D x 3-D: expert e's rows
+// [offs[e-1], offs[e]) of the bf16 x against wq[e] (the stored [E, N, K] qdata), the dense int8 weight-only epilogue
+// with w_scale[e, n] and no bias, y = bf16(bf16(bf16(x wq[e]^T) * bf16(w_scale[e, n]))), which is what select + the
+// dense linear computes per expert.  offs stays on the device (grouped schedule, ts_gemm.cuh).
+extern "C" int ao_int8_weight_grouped_mm(const uint16_t* x, int M, int K, const int8_t* wq, const float* w_scale, int E,
+                                         int N, const int32_t* offs, uint16_t* y, void* workspace,
+                                         size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int8 weight grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "int8 weight grouped mm: E=%d experts must be in [1, %d]", E,
+             tsg::MAX_EXPERTS);
+  AO_REQUIRE(K % 16 == 0, "int8 weight grouped mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
+  // no N rule: weight boxes may start on any row of the [E * N, K] map, and the scales are read by the epilogue
+  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "int8 weight grouped mm: E*N=%lld weight rows exceed the int32 range",
+             (long long)E * N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && wq && w_scale && offs && y && workspace, "int8 weight grouped mm: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "int8 weight grouped mm: x must be 16-byte aligned");
+  using Fmt = tsg::Grouped<lowp::Int8WoFmt>;
+  CUtensorMap tm_w, tm_aux;
+  if (int rc = Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), E * N, K, &tm_w, &tm_aux)) return rc;
+  tsg::Params p{};
+  p.w_scale = w_scale;
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.offs = offs;
+  p.E = E;
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<Fmt>(p, tm_w, tm_aux, x, K, workspace, workspace_bytes, "int8 weight grouped mm",
+                       reinterpret_cast<cudaStream_t>(stream));
+}
+
+// torch._grouped_mm(x, W.transpose(-2, -1), offs) on int8 expert weights with per-token int8 activations: expert e's
+// rows [offs[e-1], offs[e]) of xq (x_scale [M] per row) against wq[e], s32 sums, the dense int8 epilogue
+// y = bf16(bf16(acc * x_scale[m]) * w_scale[e, n]) without bias.  offs stays on the device (grouped schedule,
+// ts_gemm.cuh).
+extern "C" int ao_int8_dyn_grouped_mm(const int8_t* xq, const float* x_scale, int M, int K, const int8_t* wq,
+                                      const float* w_scale, int E, int N, const int32_t* offs, uint16_t* y,
+                                      void* workspace, size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int8 grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "int8 grouped mm: E=%d experts must be in [1, %d]", E, tsg::MAX_EXPERTS);
+  AO_REQUIRE(K % 16 == 0, "int8 grouped mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
+  AO_REQUIRE(N % 8 == 0, "int8 grouped mm: N=%d must be a multiple of 8 (reference: int8/kernels.py:48-58)", N);
+  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "int8 grouped mm: E*N=%lld weight rows exceed the int32 range",
+             (long long)E * N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(xq && x_scale && wq && w_scale && offs && y && workspace, "int8 grouped mm: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(xq) & 15) == 0, "int8 grouped mm: xq must be 16-byte aligned");
+  using Fmt = tsg::Grouped<lowp::SsFmt<lowp::KIND_I8>>;
+  CUtensorMap tm_w, tm_aux;
+  if (int rc = Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), E * N, K, &tm_w, &tm_aux)) return rc;
+  tsg::Params p{};
+  p.row_scale = x_scale;
+  p.w_scale = w_scale;
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.offs = offs;
+  p.E = E;
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<Fmt>(p, tm_w, tm_aux, xq, K, workspace, workspace_bytes, "int8 grouped mm",
                        reinterpret_cast<cudaStream_t>(stream));
 }
 

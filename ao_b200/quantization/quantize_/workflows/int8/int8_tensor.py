@@ -15,6 +15,7 @@ from dataclasses import dataclass
 from typing import List, Optional
 
 import torch
+from torch.utils._python_dispatch import return_and_correct_aliasing
 
 from ao_b200.quantization.granularity import Granularity, PerRow, PerTensor
 from ao_b200.quantization.quant_primitives import (
@@ -229,6 +230,114 @@ def _(func, types, args, kwargs):
                       act_quant_scale=self.act_quant_scale, act_quant_zero_point=self.act_quant_zero_point,
                       act_pre_scale=self.act_pre_scale, act_quant_kwargs=self.act_quant_kwargs,
                       reduce_range=self.reduce_range)
+
+
+@implements(aten.transpose.int)
+def _(func, types, args, kwargs):
+    """A view with qdata, scale, zero_point and block_size swapped: how a 3-D expert weight [E, N, K] reaches
+    torch._grouped_mm as mat_b [E, K, N].  Transposing twice gives back the stored form."""
+    self, dim0, dim1 = args
+    bs = list(self.block_size)
+    bs[dim0], bs[dim1] = bs[dim1], bs[dim0]
+
+    def swap(t):
+        return t.transpose(dim0, dim1) if t is not None and t.dim() == self.qdata.dim() else t
+
+    new = Int8Tensor(self.qdata.transpose(dim0, dim1), swap(self.scale), bs, self.dtype,
+                     zero_point=swap(self.zero_point), act_quant_scale=self.act_quant_scale,
+                     act_quant_zero_point=self.act_quant_zero_point, act_pre_scale=self.act_pre_scale,
+                     act_quant_kwargs=self.act_quant_kwargs, reduce_range=self.reduce_range)
+    return return_and_correct_aliasing(func, args, kwargs, new)
+
+
+@implements(aten._grouped_mm.default)
+def _(func, types, args, kwargs):
+    """torch._grouped_mm(x, W.transpose(-2, -1), offs=offs) with an Int8Tensor expert weight W [E, N, K], 2-D x 3-D:
+    expert e's rows [offs[e-1], offs[e]) of x times W[e] in one launch, computing what the per-expert recipe
+    F.linear(x[rows_e], W[e]) (select, then the dense linear) computes:
+
+    * weight-only (no ``act_quant_kwargs``): bf16(bf16(bf16(x W[e]^T) * bf16(s_w[e]))), on bf16 x (after
+      ``act_pre_scale``), ``int8_weight_grouped_mm``;
+    * dynamic, symmetric PerRow activations: every routed row quantized as the dense linear quantizes it (a row's
+      scale depends on that row only, so all M rows at once equal each expert's rows), then ``int8_dyn_grouped_mm``;
+    * static, symmetric PerTensor activations with a [1, 1] ``act_quant_scale``: one scale for every row, the fused
+      ``int8_quantize_static`` (``act_pre_scale`` included), then ``int8_dyn_grouped_mm``.
+
+    Rows from offs[-1] on are left unwritten, as torch leaves them.  Other forms raise NotImplementedError."""
+    mat_a, mat_b = args[0], args[1]
+    offs = args[2] if len(args) > 2 else kwargs.get("offs", None)
+    bias = args[3] if len(args) > 3 else kwargs.get("bias", None)
+    out_dtype = args[4] if len(args) > 4 else kwargs.get("out_dtype", None)
+    assert isinstance(mat_b, Int8Tensor)
+    assert offs is not None, "offs is required for _grouped_mm"
+    what = "Int8Tensor _grouped_mm"
+    if mat_a.dim() != 2 or mat_b.dim() != 3:
+        raise NotImplementedError(f"{what}: only 2-D mat_a x 3-D mat_b, got {mat_a.dim()}-D x {mat_b.dim()}-D")
+    if mat_b.qdata.stride(-2) >= mat_b.qdata.stride(-1):
+        raise NotImplementedError(f"{what}: mat_b must be the transposed [E, N, K] expert weight, "
+                                  f"W.transpose(-2, -1)")
+    if bias is not None:
+        raise NotImplementedError(f"{what}: bias is not supported")
+    if isinstance(mat_a, TorchAOBaseTensor) or mat_a.dtype != torch.bfloat16 or out_dtype not in (None, torch.bfloat16):
+        raise NotImplementedError(f"{what}: bf16 mat_a and output only, got {mat_a.dtype} -> {out_dtype}")
+    E, K, N = mat_b.shape
+    if list(mat_b.block_size) not in ([1, K, 1], [E, K, N]):
+        raise NotImplementedError(
+            f"{what}: block_size {list(mat_b.block_size)} of a {tuple(mat_b.shape)} weight is neither per-row nor "
+            f"per-tensor (PerGroup has no sm_90a kernel in this engine)")
+    if mat_a.shape[-1] != K:
+        raise ValueError(f"_grouped_mm: mat_a has K={mat_a.shape[-1]}, mat_b K={K}")
+    if mat_a.shape[0] == 0:
+        return mat_a.new_empty((0, N))
+    wq = mat_b.qdata.transpose(-2, -1).contiguous()   # back to the stored [E, N, K]
+    ws = mat_b.scale.float()
+    # a per-tensor scale is expanded to one value per (expert, feature), a torch copy
+    ws = (ws.reshape(E, N) if ws.numel() == E * N else ws.reshape(1, 1).expand(E, N)).contiguous()
+    offs = offs.to(torch.int32)
+    kw = mat_b.act_quant_kwargs
+    x = mat_a
+    if kw is None:
+        if mat_b.act_pre_scale is not None:
+            x = x * mat_b.act_pre_scale
+        # the kernel takes contiguous, 16-byte aligned rows (alignment from the storage offset: traceable with fake
+        # tensors)
+        x = x.to(torch.bfloat16).contiguous()
+        if x.storage_offset() % 8 != 0:
+            x = x.clone()
+        return torch.ops.ao_b200.int8_weight_grouped_mm(x, wq, ws, offs)
+    if kw.mapping_type != MappingType.SYMMETRIC or mat_b.act_quant_zero_point is not None:
+        raise NotImplementedError(
+            f"{what}: asymmetric int8 activations (or a static act_quant_zero_point) need each expert's rowsum(Wq) "
+            f"correction, which the grouped kernel does not apply")
+    if N % 8 != 0:
+        raise NotImplementedError(f"{what}: N={N} output features per expert; the int8 x int8 kernel needs N % 8 == 0 "
+                                  f"(the dense int8 rule)")
+    s = mat_b.act_quant_scale
+    if s is None:
+        if not isinstance(kw.granularity, PerRow):
+            raise NotImplementedError(
+                f"{what}: dynamic {kw.granularity} activations; the per-expert recipe computes one scale over each "
+                f"expert's own rows, not over all M, so only PerRow activations are served")
+        if mat_b.act_pre_scale is not None:
+            x = x * mat_b.act_pre_scale
+        xt = Int8Tensor.from_hp(x, kw.granularity, mapping_type=kw.mapping_type, reduce_range=kw.reduce_range)
+        xq, xs = xt.qdata, xt.scale.reshape(-1).float()
+    else:
+        if not isinstance(kw.granularity, PerTensor) or s.numel() != 1:
+            raise NotImplementedError(
+                f"{what}: a static {kw.granularity} act_quant_scale of shape {tuple(s.shape)}; it is tied to the rows "
+                f"of one calibration batch and does not fit an expert's rows.  Only PerTensor with a [1, 1] scale")
+        if _static_quantizer_serves(x, mat_b):
+            qmin, qmax = (-64, 63) if kw.reduce_range else (-128, 127)
+            xq, xs, _ = torch.ops.ao_b200.int8_quantize_static(rows_for_kernel(x), s, None, mat_b.act_pre_scale,
+                                                               qmin, qmax)
+        else:
+            if mat_b.act_pre_scale is not None:
+                x = x * mat_b.act_pre_scale
+            xt = Int8Tensor.from_hp(x, kw.granularity, mapping_type=kw.mapping_type, scale=s,
+                                    reduce_range=kw.reduce_range)
+            xq, xs = xt.qdata, xt.scale.reshape(-1).float().expand(x.shape[0])
+    return torch.ops.ao_b200.int8_dyn_grouped_mm(xq.contiguous(), xs.contiguous(), wq, ws, offs)
 
 
 Int8Tensor.__module__ = "ao_b200.quantization"

@@ -178,6 +178,26 @@ int ao_fp8_weight_linear(const uint16_t* x, int ldx, int M, int K, const uint8_t
 int ao_fp8_weight_grouped_mm(const uint16_t* x, int M, int K, const uint8_t* wq, const float* w_scale, int E, int N,
                              const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes,
                              void* stream);
+/* torch._grouped_mm(x, W.transpose(-2, -1), offs) for a 3-D weight-only Int8Tensor expert weight W [E, N, K], 2-D x 3-D
+ * form, as the per-expert recipe select + ao_int8_weight_linear computes it: for offs[e-1] <= m < offs[e]
+ * (offs[-1] = 0)
+ *   y[m, n] = bf16( bf16(bf16(sum_k x[m,k] * wq[e][n,k]) * bf16(w_scale[e][n])) ),  f32 accumulate (exact products).
+ * x bf16 [M,K] (tokens sorted by expert, rows contiguous, 16-byte aligned); wq int8 [E][N][K] (the stored qdata);
+ * w_scale f32 [E][N] (a per-tensor scale expanded); offs int32 [E] on the device, cumulative row ends.  The host never
+ * reads offs (no sync, CUDA-graph capturable); the kernel clamps each offs[e] into [offs[e-1], M].  Rows from
+ * offs[E-1] on are not written.  1 <= E <= 1024, K % 16 == 0, any N, no bias.                                       */
+int ao_int8_weight_grouped_mm(const uint16_t* x, int M, int K, const int8_t* wq, const float* w_scale, int E, int N,
+                              const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes,
+                              void* stream);
+/* torch._grouped_mm(x, W.transpose(-2, -1), offs) for a 3-D Int8Tensor expert weight W [E, N, K] with symmetric
+ * per-token int8 activations (dynamic PerRow, or static PerTensor after ao_int8_quantize_static), as the per-expert
+ * recipe select + ao_int8_dyn_linear computes it: for offs[e-1] <= m < offs[e]
+ *   y[m, n] = bf16( bf16(acc_i32[m, n] * x_scale[m]) * w_scale[e][n] ),  acc_i32 = sum_k xq[m,k] * wq[e][n,k].
+ * xq int8 [M,K] (16-byte aligned), x_scale f32 [M], wq int8 [E][N][K], w_scale f32 [E][N], offs as above.
+ * 1 <= E <= 1024, K % 16 == 0, N % 8 == 0, no bias.                                                                 */
+int ao_int8_dyn_grouped_mm(const int8_t* xq, const float* x_scale, int M, int K, const int8_t* wq,
+                           const float* w_scale, int E, int N, const int32_t* offs, uint16_t* y, void* workspace,
+                           size_t workspace_bytes, void* stream);
 /* int32 accumulator only (aten._int_mm equivalent; int8/kernels.py:18-76). */
 int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, int N, int32_t* acc,
                    void* workspace, size_t workspace_bytes, void* stream);

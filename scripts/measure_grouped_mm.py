@@ -4,7 +4,8 @@ F.scaled_grouped_mm on identical operands, for MoE expert shapes; with --fmt nvf
 per-expert activation quantizer nvfp4_fakequant_grouped plus nvfp4_grouped_mm) against the fp8 path with its
 quantizer (fp8_quantize_rowwise plus fp8_rowwise_grouped_mm) and bf16 torch._grouped_mm on the unquantized weights.
 
-  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4|fp8wo] [--group-size 32] [--replays 20] [--out FILE]
+  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4|fp8wo|int8wo|int8] [--group-size 32] [--replays 20]
+                                       [--out FILE]
 
   * shapes: Mixtral-8x7B experts (E=8, 4096 -> 14336 and 14336 -> 4096, top-2) and Qwen3-30B-A3B experts (E=128,
     2048 -> 768 and 768 -> 2048, top-8);
@@ -27,7 +28,14 @@ K and N as padded, the bf16 activations read once, the outputs).  --fmt fp8wo: t
 (torch._grouped_mm on 3-D Float8Tensor weights of Float8WeightOnlyConfig) against the reference's recipe (torch._grouped_mm
 on W.dequantize(), all E experts dequantized on every call), bf16 torch._grouped_mm and the fp8 dynamic path with its
 quantizer; bytes are the weight-only path's (1 byte per weight and 4 per row scale of the active experts, the bf16
-activations read once, the outputs, offs) and its roofline term the HBM time of those bytes.
+activations read once, the outputs, offs) and its roofline term the HBM time of those bytes.  --fmt int8wo / int8:
+the int8 expert GEMM (torch._grouped_mm on 3-D Int8Tensor weights; int8: dynamic PerRow activations, quantizer
+included) against this engine's dense int8 op per active expert (the select loop, captured with the routing fixed),
+the reference's per-expert recipe restated in torch (int8wo: torch.mm on qdata.to(bf16) times the bf16 scale; int8:
+per-row quantization, torch._int_mm and the pointwise epilogue), bf16 torch._grouped_mm and the fp8 counterpart (fp8
+weight-only, or fp8 rowwise with its quantizer); bytes are the int8 path's (1 byte per weight and 4 per row scale of
+the active experts, the activations as the GEMM reads them, the outputs, offs), its roofline term their HBM time, and
+vs_select_linear compares the output with select + F.linear on every active expert.
 """
 from __future__ import annotations
 
@@ -298,9 +306,108 @@ def measure_fp8wo(a, ops, dev, lines):
         torch.cuda.empty_cache()
 
 
+def measure_int8(a, ops, dev, lines):
+    """The int8 expert GEMM (torch._grouped_mm on a 3-D Int8Tensor; --fmt int8wo weight-only, --fmt int8 dynamic PerRow
+    activations with their quantizer) against this engine's dense int8 op on each active expert (the select loop,
+    captured with the routing fixed, without its host syncs), the reference's per-expert recipe restated in torch,
+    bf16 torch._grouped_mm, and this engine's fp8 counterpart (fp8 weight-only, or fp8 rowwise with its quantizer)."""
+    import torch
+
+    from ao_b200.quantization import Float8Tensor, Int8Tensor, PerRow, QuantizeTensorToInt8Kwargs
+
+    dyn = a.fmt == "int8"
+    for name, E, N, K, topk in SHAPES:
+        g = torch.Generator(device=dev).manual_seed(E * N + K)
+        copies = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * (N * K + N * 4))) + 1)
+        copies_bf16 = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * N * K * 2)) + 1)
+        w8, f8, wb = [], [], []
+        kw = dict(act_quant_kwargs=QuantizeTensorToInt8Kwargs(granularity=PerRow())) if dyn else {}
+        for c in range(max(copies, copies_bf16)):
+            w = (torch.randn(E, N, K, device=dev, generator=g) * 0.05).to(torch.bfloat16)
+            if c < copies:
+                w8.append(Int8Tensor.from_hp(w, PerRow(), **kw))
+                f8.append(Float8Tensor.from_hp(w, torch.float8_e4m3fn, PerRow()))
+            if c < copies_bf16:
+                wb.append(w)
+            del w
+        for T in TOKENS:
+            for skewed in (False, True):
+                rows = routing(T, E, topk, skewed, seed=T * 131 + E + skewed)
+                M = sum(rows)
+                offs = torch.tensor(rows, dtype=torch.int64).cumsum(0).to(torch.int32).to(dev)
+                x = torch.randn(M, K, device=dev, generator=g).to(torch.bfloat16)
+                active = sum(1 for r in rows if r)
+                act_bytes = M * K + M * 4 if dyn else M * K * 2
+                need = active * (N * K + N * 4) + act_bytes + M * N * 2 + E * 4
+                rec = dict(fmt=a.fmt, shape=name, E=E, N=N, K=K, topk=topk, tokens=T,
+                           routing="skewed" if skewed else "balanced", rows=M, active_experts=active, bytes=need,
+                           weight_copies=copies, roofline_us=round(need / HBM_BPS * 1e6, 2))
+                spans, start = [], 0
+                for e, r in enumerate(rows):
+                    if r:
+                        spans.append((e, start, start + r))
+                    start += r
+                ws = [t.scale.reshape(E, N).float() for t in w8]
+
+                def ours(c):
+                    return torch._grouped_mm(x, w8[c].transpose(-2, -1), offs=offs)
+
+                def loop(c):
+                    w = w8[c]
+                    if dyn:
+                        xq, sx = ops.int8_quantize_rowwise(x)
+                        for e, s0, s1 in spans:
+                            ops.int8_dyn_linear(xq[s0:s1], sx.reshape(-1)[s0:s1], w.qdata[e], ws[c][e], None)
+                    else:
+                        for e, s0, s1 in spans:
+                            ops.int8_weight_linear(x[s0:s1], w.qdata[e], ws[c][e], None)
+
+                def recipe(c):
+                    # per expert, in torch: weight-only torch.mm on qdata.to(bf16) times the bf16 scale; dynamic
+                    # per-row quantization, torch._int_mm (rows padded to 17, its minimum on CUDA) and the epilogue
+                    w = w8[c]
+                    for e, s0, s1 in spans:
+                        xe = x[s0:s1]
+                        if dyn:
+                            sx = (xe.float().abs().amax(dim=1, keepdim=True) / 127).clamp(min=torch.finfo(torch.float32).eps)
+                            xq = torch.clamp(torch.round(xe.float() / sx), -128, 127).to(torch.int8)
+                            xq = torch.nn.functional.pad(xq, (0, 0, 0, max(0, 17 - xq.shape[0])))
+                            acc = torch._int_mm(xq, w.qdata[e].t())[: s1 - s0]
+                            (acc * sx).to(torch.bfloat16) * ws[c][e]
+                        else:
+                            torch.mm(xe, w.qdata[e].to(torch.bfloat16).t()) * ws[c][e].to(torch.bfloat16)
+
+                def bf16(c):
+                    return torch._grouped_mm(x, wb[c].transpose(-2, -1), offs=offs)
+
+                if dyn:
+                    def fp8(c):
+                        xq, sx = ops.fp8_quantize_rowwise(x)
+                        return ops.fp8_rowwise_grouped_mm(xq, sx.reshape(-1), f8[c].qdata, f8[c].scale.reshape(E, N), offs)
+                else:
+                    def fp8(c):
+                        return torch._grouped_mm(x, f8[c].transpose(-2, -1), offs=offs)
+
+                n = int(offs[-1])
+                y = ours(0)[:n]
+                y_loop = torch.cat([torch.nn.functional.linear(x[s0:s1], w8[0][e]) for e, s0, s1 in spans])
+                rec["vs_select_linear"] = "identical" if torch.equal(y.view(torch.int16), y_loop.view(torch.int16)) \
+                    else sqnr_db(y_loop, y)
+                rec["sqnr_vs_bf16_db"] = sqnr_db(bf16(0)[:n], y)
+                for key, fn, cp in (("ours", ours, copies), ("expert_loop", loop, copies), ("recipe", recipe, copies),
+                                    ("bf16", bf16, copies_bf16), ("fp8" if dyn else "fp8wo", fp8, copies)):
+                    us = time_graph(fn, cp, a.replays)
+                    rec[f"{key}_us"] = round(us, 2)
+                    rec[f"{key}_GBps"] = round(need / us * 1e-3, 1)
+                print(json.dumps(rec), flush=True)
+                lines.append(rec)
+        del w8, f8, wb
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4", "fp8wo"], default="fp8")
+    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4", "fp8wo", "int8wo", "int8"], default="fp8")
     ap.add_argument("--group-size", type=int, choices=[32, 64, 128, 256], default=32)
     ap.add_argument("--replays", type=int, default=20)
     ap.add_argument("--out", default=None)
@@ -371,6 +478,8 @@ def main():
         measure_int4(a, ops, dev, lines)
     if a.fmt == "fp8wo":
         measure_fp8wo(a, ops, dev, lines)
+    if a.fmt in ("int8wo", "int8"):
+        measure_int8(a, ops, dev, lines)
     info = dict(card=card(), torch=torch.__version__)
     print(json.dumps(info), flush=True)
     if a.out:
