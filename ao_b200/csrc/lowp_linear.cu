@@ -2,6 +2,7 @@
 //   int8 x int8 -> int32  (wgmma s8, both operands TMA tiles)      replaces aten._int_mm + the scale epilogue
 //                         and, per expert, aten._int_mm on select()ed int8 expert weights
 //   e4m3 x e4m3 -> f32    (wgmma e4m3, both operands TMA tiles)    replaces torch._scaled_mm rowwise
+//                         and, 1x128 x 128x128 block scales, the reference's blockwise Triton GEMM
 //   mxfp8 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm block-scaled
 //   nvfp4 block-16 e4m3   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm fp4 + pts/bias kernels
 //   nvfp4 weight x bf16   (bf16 wgmma, weights dequantised exactly)      replaces F.linear on the dequantised weight
@@ -94,6 +95,78 @@ struct SsFmt {
       const uint64_t bd = wgmma_desc_k_sw128(x_s + kk * 32);
       if (KIND == KIND_I8) Wgmma<N_MMA>::ss_s8(acc, ad, bd, kk == 0 ? scale_d : 1u);
       else Wgmma<N_MMA>::ss_e4m3(acc, ad, bd, kk == 0 ? scale_d : 1u);
+    }
+  }
+  // PROMOTE (e4m3): the rowwise scales stay in the epilogue, each chunk's partial is added as it is
+  struct NoScales {};
+  template <int N_MMA>
+  __device__ static __forceinline__ NoScales chunk_scales(const tsg::Params&, uint32_t, int, int, int) { return {}; }
+  template <int N_MMA>
+  __device__ static __forceinline__ void promote(uint32_t (&acc)[N_MMA / 2], const uint32_t (&part)[N_MMA / 2],
+                                                 uint32_t accumulate, NoScales) {
+#pragma unroll
+    for (int j = 0; j < N_MMA / 2; ++j)
+      acc[j] = accumulate ? __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(part[j])) : part[j];
+  }
+};
+
+// Blockwise e4m3 (Float8DynamicActivationFloat8WeightConfig with PerBlock([1, 128]) activations and PerBlock([128,
+// 128]) weights; reference float8_tensor.py:431-447 and its Triton loop, kernels.py:86-97): the operands, wgmmas and
+// per-chunk promotion of SsFmt<KIND_F8>.  A tile is 128 weight rows and a chunk 128 k, i.e. exactly one weight block
+// and one activation block per token, so each chunk's partial is scaled as it is promoted, in the loop's order:
+//   acc = fma(part * a_s[m][kc], w_s[n_tile][kc], acc)      (acc = 0 before a segment's first chunk)
+// The multiply-add is fused (what Triton's default fp-fusion contracts `acc += dot * a_s * w_s` to).  The epilogue is
+// EPI_BF16: bf16(acc), then a bf16 add of the bias.  Stream-K partials are such scaled sums and are gathered in the
+// fixed CTA order as for every format.
+// Scales: w_s from w_scale [N/128][K/128] (Params::w_scale), one value per chunk read by every thread; a_s from the
+// transposed activation scales [K/128][ldm] (ldm = M rounded up to 4, ao_fp8_quantize_1x128): one 256-byte TMA box of
+// 64 tokens per chunk, requested with the activation tile into the stage's aux slot (the 64-token box serves every
+// token tile: tokens past the tile or past M are never stored).
+struct BlockwiseF8Fmt : SsFmt<KIND_F8> {
+  static constexpr int X_AUX_BYTES = MAX_N_MMA * 4;
+  static constexpr int AUX_BYTES = X_AUX_BYTES;
+  static constexpr int EPI = tsg::EPI_BF16;
+  static int make_maps(const uint8_t* wq, const float* x_scale_t, int M, int N, int K, CUtensorMap* tm_w,
+                       CUtensorMap* tm_xs) {
+    if (int rc = kmajor_byte_map(wq, N, K, tm_w)) return rc;
+    const uint64_t ldm = ((uint64_t)M + 3) & ~3ull;
+    const uint64_t dims[2] = {ldm, (uint64_t)K / KCHUNK};
+    const uint64_t str[1] = {ldm * 4};
+    const uint32_t box[2] = {MAX_N_MMA, 1};
+    return make_tmap(tm_xs, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, x_scale_t, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
+  __device__ static __forceinline__ void issue_x_aux(const CUtensorMap* tm_xs, uint8_t* aux_dst, uint64_t* bar, int m0,
+                                                     int kc, uint64_t policy) {
+    tma_load_2d(aux_dst, tm_xs, bar, m0, kc, policy);
+  }
+  // the weight block's scale and the activation scales of the thread's tokens 8q + 2t, + 1 (accumulator value
+  // 4q + 2h + c is token 8q + 2t + c)
+  template <int N_MMA>
+  struct Scales {
+    float w;
+    float2 a[N_MMA / 8];
+  };
+  template <int N_MMA>
+  __device__ static __forceinline__ Scales<N_MMA> chunk_scales(const tsg::Params& p, uint32_t aux_s, int n_tile, int kc,
+                                                               int lane) {
+    Scales<N_MMA> cs;
+    cs.w = p.w_scale[(size_t)n_tile * p.KT + kc];
+    const uint32_t t = lane & 3;
+#pragma unroll
+    for (int q = 0; q < N_MMA / 8; ++q) {
+      const uint2 v = tsg::lds64(aux_s + (8 * q + 2 * t) * 4);
+      cs.a[q] = make_float2(__uint_as_float(v.x), __uint_as_float(v.y));
+    }
+    return cs;
+  }
+  template <int N_MMA>
+  __device__ static __forceinline__ void promote(uint32_t (&acc)[N_MMA / 2], const uint32_t (&part)[N_MMA / 2],
+                                                 uint32_t accumulate, const Scales<N_MMA>& cs) {
+#pragma unroll
+    for (int j = 0; j < N_MMA / 2; ++j) {
+      const float a = (j & 1) ? cs.a[j / 4].y : cs.a[j / 4].x;
+      const float prev = accumulate ? __uint_as_float(acc[j]) : 0.f;
+      acc[j] = __float_as_uint(__fmaf_rn(__fmul_rn(__uint_as_float(part[j]), a), cs.w, prev));
     }
   }
 };
@@ -585,6 +658,31 @@ extern "C" int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, in
   AO_REQUIRE(xq && x_scale && wq && w_scale && y, "fp8 linear: null pointer");
   return lowp::rowwise<lowp::KIND_F8>(xq, x_scale, M, K, wq, w_scale, N, bias, y, nullptr, workspace, workspace_bytes,
                                       stream);
+}
+
+// F.linear(x, Float8Tensor with 128x128 weight blocks and 1x128 activation blocks) (float8_tensor.py:431-447):
+// y = bf16(bf16(acc) + bias[n]), acc summed chunk by chunk as BlockwiseF8Fmt states.  x_scale_t: the transposed
+// activation scales [K/128][round_up(M, 4)] of ao_fp8_quantize_1x128; w_scale [N/128][K/128].
+extern "C" int ao_fp8_blockwise_linear(const uint8_t* xq, const float* x_scale_t, int M, int K, const uint8_t* wq,
+                                       const float* w_scale, int N, const uint16_t* bias, uint16_t* y, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 blockwise linear: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(K % 128 == 0, "fp8 blockwise linear: K=%d must be a multiple of 128 (one scale per 128 k)", K);
+  AO_REQUIRE(N % 128 == 0, "fp8 blockwise linear: N=%d must be a multiple of 128 (one scale per 128 rows)", N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(xq && x_scale_t && wq && w_scale && y, "fp8 blockwise linear: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(xq) & 15) == 0, "fp8 blockwise linear: xq must be 16-byte aligned");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x_scale_t) & 15) == 0,
+             "fp8 blockwise linear: x_scale must be 16-byte aligned (it is loaded by TMA)");
+  CUtensorMap tm_w, tm_xs;
+  if (int rc = lowp::BlockwiseF8Fmt::make_maps(wq, x_scale_t, M, N, K, &tm_w, &tm_xs)) return rc;
+  tsg::Params p{};
+  p.w_scale = w_scale;
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<lowp::BlockwiseF8Fmt>(p, tm_w, tm_xs, xq, K, workspace, workspace_bytes, "fp8 blockwise linear",
+                                        reinterpret_cast<cudaStream_t>(stream));
 }
 
 // torch._grouped_mm(x, W.transpose(-2, -1), offs) on rowwise e4m3 operands: expert e's rows [offs[e-1], offs[e]) of

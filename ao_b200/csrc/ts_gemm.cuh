@@ -20,6 +20,8 @@
 #pragma once
 #include <cuda_bf16.h>
 
+#include <type_traits>
+
 #include "common.h"
 #include "ptx.cuh"
 #include "streamk.cuh"
@@ -56,6 +58,17 @@ struct IsGrouped<Grouped<F>> {
   static constexpr bool value = true;
 };
 
+// Fmt::X_AUX_BYTES (optional, default 0): bytes of the stage's aux slot that arrive with the activation tile (xfull,
+// after griddepcontrol.wait: per-token values the previous kernel wrote), requested by Fmt::issue_x_aux
+template <class F, class = void>
+struct XAux {
+  static constexpr int BYTES = 0;
+};
+template <class F>
+struct XAux<F, std::void_t<decltype(F::X_AUX_BYTES)>> {
+  static constexpr int BYTES = F::X_AUX_BYTES;
+};
+
 template <class Fmt, int N_MMA>
 constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA && !IsGrouped<Fmt>::value ? 2 : 1; }
 constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
@@ -77,7 +90,8 @@ struct Params {
   int out_scale_per_row;
   int grid_forced;          // Grouped<Fmt>: the host grid was forced (ao_b200_debug_set_streamk_ctas): no MIN_UNITS rule
   const float* w_scale;     // EPI_I8 / EPI_F8 / EPI_BF16_WSCALE: per-output-feature weight scale [N] (EPI_BF16 never
-                            // reads it: its format applies the scale per weight, from the aux operand)
+                            // reads it: its format applies the scale per weight, from the aux operand, or, blockwise
+                            // e4m3, per 128x128 block [N/128][KT] in its promotion)
   __nv_bfloat16* y;         // [M, N_out]
   int32_t* i32_out;         // EPI_I8: raw int32 accumulators [M, N] instead of y
   float* ws_partial;        // [grid][N_MMA*128]   CTA b's CONTRIB partial (streamk.cuh)
@@ -212,6 +226,8 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 //                                                                  [E * N, K] map of all experts, and their aux tiles
 //   EXPERT_SCALE (grouped EPI_FLOAT only): the epilogue multiplies by out_scale[e] (nvfp4: yes, int4: no scale at all)
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
+//   PROMOTE: cs = chunk_scales<N_MMA>(p, aux smem, n_tile, kc, lane)  the chunk's scales (before its wgmmas)
+//            static void promote<N_MMA>(acc, part, accumulate, cs)   acc (+)= the chunk's partial sums, scaled by cs
 //   RA:  struct Raw; static void load(p, w smem, aux smem, row_lo, lane, Raw&)   rows row_lo and row_lo + 8
 //        static void frag(p, raw, kk, a[4])                        bf16 A fragment of k16 step kk (0..7)
 // Grouped<Fmt>: the grouped schedule above; the dense kernels compile without any of it.
@@ -312,10 +328,11 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       int m0 = (tile_of(i) / p.n_tiles) * N_MMA;
       // grouped: from the expert's rows on (rows of the next expert in the box are loaded but never stored)
       if constexpr (GROUPED) m0 = group_tile<N_MMA>(g_end, g_mbp, p.E, tile_of(i) / p.n_tiles).row0;
-      mbar_expect_tx(&xfull[s], C::X_BYTES);
+      mbar_expect_tx(&xfull[s], C::X_BYTES + XAux<Fmt>::BYTES);
 #pragma unroll
       for (int a = 0; a < C::X_ATOMS; ++a)
         tma_load_2d(xs + a * (N_MMA * 128), &tm_x, &xfull[s], kc_of(i) * KCHUNK + a * (KCHUNK / C::X_ATOMS), m0, pol_x);
+      if constexpr (XAux<Fmt>::BYTES > 0) Fmt::issue_x_aux(&tm_aux, stage(s) + Fmt::W_BYTES, &xfull[s], m0, kc_of(i), pol_x);
     };
     const int pre = nunits < S ? nunits : S;
     for (int i = 0; i < pre; ++i) {
@@ -570,8 +587,11 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         mbar_wait(&wfull[s], ph);
         if constexpr (Fmt::PROMOTE) {
           // e4m3: a chain of wgmmas accumulates in the tensor core's reduced-precision adder; each chunk's four k32
-          // wgmmas go to a fresh accumulator that is added to the fp32 registers here (fp32 accuracy across K)
+          // wgmmas go to a fresh accumulator that is added to the fp32 registers here (fp32 accuracy across K).  The
+          // format's chunk scales (none for rowwise) are read before the wgmmas, so their loads overlap them, and
+          // before the stage goes back
           mbar_wait(&xfull[s], ph);
+          const auto cs = Fmt::template chunk_scales<N_MMA>(p, aux_s, tile_of(i) % p.n_tiles, kc_of(i), lane);
           uint32_t part[NACC];
           wgmma_fence();
           Fmt::template mma<N_MMA>(part, w_s, x_s, wg, 0u);
@@ -579,9 +599,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           wgmma_wait<0>();
           wgmma_fence_operand(part);
           release(s);
-#pragma unroll
-          for (int j = 0; j < NACC; ++j)
-            acc[j] = scale_d ? __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(part[j])) : part[j];
+          Fmt::template promote<N_MMA>(acc, part, scale_d, cs);
           continue;
         } else if constexpr (Fmt::SS) {
           mbar_wait(&xfull[s], ph);

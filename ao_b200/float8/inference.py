@@ -1,4 +1,5 @@
 """fp8 inference helpers (reference: torchao/float8/inference.py:26-39, :177-265)."""
+import math
 from typing import List, NamedTuple, Optional, Tuple, Union
 
 import torch
@@ -26,6 +27,22 @@ def _is_tensorwise_scaled(block_size, shape) -> bool:
     return all(int(b) in (-1, int(s)) for b, s in zip(block_size, shape))
 
 
+def _is_1_128_scaled(block_size) -> bool:
+    """1x128 blocks along the last dim (the blockwise recipe's activations; reference :197-204)."""
+    return len(block_size) >= 2 and math.prod(block_size[:-1]) == 1 and block_size[-1] == 128
+
+
+def _is_128_128_scaled(block_size) -> bool:
+    """128x128 blocks of a 2-D weight (the blockwise recipe's weights; reference :207-214)."""
+    return len(block_size) == 2 and block_size[0] == 128 and block_size[1] == 128
+
+
+def _granularity_is_a_1_128_w_128_128(g) -> bool:
+    """The blockwise pair, by the dataclasses' equality as the reference compares it (reference :217-228): the block
+    sizes are compared as given, so PerBlock([1, 128]) matches and PerBlock((1, 128)) does not."""
+    return len(g) == 2 and g[0] == PerBlock([1, 128]) and g[1] == PerBlock([128, 128])
+
+
 def _normalize_granularity(granularity) -> Tuple[FP8Granularity, FP8Granularity]:
     if granularity is None:
         return PerTensor(), PerTensor()
@@ -33,8 +50,10 @@ def _normalize_granularity(granularity) -> Tuple[FP8Granularity, FP8Granularity]
         return granularity, granularity
     if isinstance(granularity, (tuple, list)) and len(granularity) == 2:
         a, w = granularity
-        ok = (isinstance(a, PerTensor) and isinstance(w, PerTensor)) or (isinstance(a, PerRow) and isinstance(w, PerRow))
+        ok = ((isinstance(a, PerTensor) and isinstance(w, PerTensor)) or (isinstance(a, PerRow) and isinstance(w, PerRow))
+              or _granularity_is_a_1_128_w_128_128(granularity))
         if not ok:
-            raise ValueError(f"Unsupported granularity types: {granularity}, only PerTensor or PerRow pairs are supported.")
+            raise ValueError(f"Unsupported granularity types: {granularity}, only PerTensor or PerRow pairs and "
+                             f"[PerBlock([1, 128]), PerBlock([128, 128])] are supported.")
         return a, w
     raise ValueError(f"Invalid granularity specification: {granularity}")

@@ -46,7 +46,8 @@ def _same(a, b) -> bool:
 
 def cat_out_features(ws: Sequence[torch.Tensor]) -> Optional[torch.Tensor]:
     """Concatenate packed weights of one class along the out-feature dimension; None when they cannot be merged
-    (different class / K / quantization attributes, a layout that pads N, or per-tensor scales that differ)."""
+    (different class / K / quantization attributes, a layout that pads N, per-tensor scales that differ, or 128x128
+    scale blocks with an N that is not a multiple of 128)."""
     from ao_b200.prototype.mx_formats.mx_tensor import MXTensor
     from ao_b200.prototype.mx_formats.nvfp4_tensor import NVFP4Tensor
     from ao_b200.quantization import Float8Tensor, Int4TilePackedTo4dTensor, Int8Tensor
@@ -69,6 +70,12 @@ def cat_out_features(ws: Sequence[torch.Tensor]) -> Optional[torch.Tensor]:
             return None   # N padded to the n-tile, or AWQ-style pre-scales (per linear)
         return cls(torch.cat([w.qdata for w in ws], 0).contiguous(), torch.cat([w.scale_and_zero for w in ws], 1).contiguous(),
                    list(w0.block_size), shape, None)
+    if cls is Float8Tensor and all(list(w.block_size) == [128, 128] for w in ws):
+        if any(w.shape[0] % 128 != 0 or w.scale.shape != (w.shape[0] // 128, w.shape[1] // 128) for w in ws):
+            return None   # a 128x128 scale block would straddle two members
+        return cls(torch.cat([w.qdata for w in ws], 0).contiguous(), torch.cat([w.scale for w in ws], 0).contiguous(),
+                   block_size=[128, 128], mm_config=w0.mm_config, act_quant_kwargs=w0.act_quant_kwargs,
+                   kernel_preference=w0.kernel_preference, dtype=w0.dtype)
     if cls in (Int8Tensor, Float8Tensor):
         rowwise = all(w.scale.dim() == 2 and w.scale.shape[0] == w.shape[0] and w.scale.shape[1] == 1 for w in ws)
         if not rowwise:

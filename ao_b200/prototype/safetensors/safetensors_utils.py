@@ -18,7 +18,7 @@ import torch
 from ao_b200.float8.inference import Float8MMConfig
 from ao_b200.prototype.mx_formats.mx_tensor import MXTensor, QuantizeTensorToMXKwargs, ScaleCalculationMode
 from ao_b200.prototype.mx_formats.nvfp4_tensor import NVFP4Tensor, QuantizeTensorToNVFP4Kwargs
-from ao_b200.quantization.granularity import PerRow, PerTensor
+from ao_b200.quantization.granularity import PerBlock, PerRow, PerTensor
 from ao_b200.quantization.quant_primitives import MappingType
 from ao_b200.quantization.quantize_.common.kernel_preference import KernelPreference
 from ao_b200.quantization.quantize_.workflows.float8.float8_tensor import Float8Tensor, QuantizeTensorToFloat8Kwargs
@@ -35,7 +35,7 @@ _REFERENCE_ONLY_TENSORS = ("Int4Tensor", "IntxUnpackedToInt8Tensor", "Int4PlainI
 ALLOWED_TENSORS_SUBCLASSES = list(_TENSOR_CLASSES) + list(_REFERENCE_ONLY_TENSORS)
 ALLOWED_CLASSES: Dict[str, type] = dict(_TENSOR_CLASSES)
 ALLOWED_CLASSES.update({c.__name__: c for c in (Float8MMConfig, QuantizeTensorToFloat8Kwargs, QuantizeTensorToInt8Kwargs,
-                                                 QuantizeTensorToMXKwargs, QuantizeTensorToNVFP4Kwargs, PerRow, PerTensor,
+                                                 QuantizeTensorToMXKwargs, QuantizeTensorToNVFP4Kwargs, PerBlock, PerRow, PerTensor,
                                                  KernelPreference, MappingType, ScaleCalculationMode)})
 
 

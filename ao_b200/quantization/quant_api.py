@@ -25,7 +25,8 @@ import torch.nn as nn
 
 from ao_b200._native import require_sm90
 from ao_b200.core.config import AOBaseConfig
-from ao_b200.float8.inference import FP8Granularity, Float8MMConfig, _normalize_granularity
+from ao_b200.float8.inference import (FP8Granularity, Float8MMConfig, _granularity_is_a_1_128_w_128_128,
+                                      _normalize_granularity)
 from ao_b200.quantization.granularity import Granularity, PerGroup, PerRow, PerTensor
 from ao_b200.quantization.quant_primitives import MappingType
 from ao_b200.quantization.quantize_.common.kernel_preference import KernelPreference
@@ -355,8 +356,14 @@ class Float8DynamicActivationFloat8WeightConfig(AOBaseConfig):
     def __post_init__(self):
         a, w = _normalize_granularity(self.granularity)
         self.granularity = [a, w]
+        default_use_fast_accum = True
+        if _granularity_is_a_1_128_w_128_128(self.granularity):
+            # reference quant_api.py:1160-1166
+            assert self.kernel_preference in (KernelPreference.AUTO, KernelPreference.TORCH), "unimplemented"
+            assert self.version >= 2, "unimplemented"
+            default_use_fast_accum = False
         if self.mm_config is None:
-            self.mm_config = Float8MMConfig(use_fast_accum=True)
+            self.mm_config = Float8MMConfig(use_fast_accum=default_use_fast_accum)
 
 
 def _fp8_mm_compat(weight: torch.Tensor) -> bool:

@@ -5,6 +5,8 @@ Attribute names / order match torchao's Float8Tensor
 ``_float8_addmm_impl -> addmm_float8_unwrapped_inference -> torch._scaled_mm``
 (:338-469, float8/inference.py:86-123) with two launches: the per-token quantizer and the GEMM with
 a fused ``acc * s_x[m] * s_w[n] + bias -> bf16`` epilogue.
+Blockwise weights (``block_size [128, 128]``, ``PerBlock([1, 128])`` activations) replace the reference's Triton GEMM
+(:431-447) with two launches: the 1x128 quantizer and the blockwise GEMM (DESIGN §2f).
 Without ``act_quant_kwargs`` (Float8WeightOnlyConfig) the linear is one launch: bf16 activations on the e4m3 weights.
 """
 from __future__ import annotations
@@ -15,8 +17,9 @@ from typing import List, Optional
 import torch
 from torch.utils._python_dispatch import return_and_correct_aliasing
 
-from ao_b200.float8.inference import FP8Granularity, Float8MMConfig, _is_rowwise_scaled, _is_tensorwise_scaled
-from ao_b200.quantization.granularity import PerRow, PerTensor
+from ao_b200.float8.inference import (FP8Granularity, Float8MMConfig, _is_1_128_scaled, _is_128_128_scaled,
+                                      _is_rowwise_scaled, _is_tensorwise_scaled)
+from ao_b200.quantization.granularity import PerBlock, PerRow, PerTensor
 from ao_b200.quantization.quant_primitives import (
     choose_scale_float8, dequantize_affine_float8, quantize_affine_float8)
 from ao_b200.quantization.quantize_.common.kernel_preference import KernelPreference
@@ -102,6 +105,8 @@ def _float8_linear_impl(input_tensor, weight_tensor: Float8Tensor, bias):
         return _weight_only_linear(input_tensor, weight_tensor, bias)
     assert not isinstance(input_tensor, TorchAOBaseTensor), "input tensor was already quantized"
     gran = act_quant_kwargs.granularity
+    if isinstance(gran, PerBlock):
+        return _blockwise_linear(input_tensor, weight_tensor, bias)
     w_rowwise = _is_rowwise_scaled(weight_tensor.block_size, weight_tensor.shape)
     w_tensorwise = _is_tensorwise_scaled(weight_tensor.block_size, weight_tensor.shape) and not w_rowwise
     if w_rowwise:
@@ -122,6 +127,32 @@ def _float8_linear_impl(input_tensor, weight_tensor: Float8Tensor, bias):
     y = torch.ops.ao_b200.fp8_rowwise_linear(xq_t.qdata.contiguous(), x_scale.contiguous().float(),
                                              weight_tensor.qdata.contiguous(), w_scale.contiguous().float(), bias)
     return y.reshape(out_shape).to(input_tensor.dtype)
+
+
+def _blockwise_linear(x, w, bias):
+    """1x128 activation blocks on 128x128 weight blocks (reference :431-447, its Triton GEMM then ``res + bias``): two
+    launches, the 1x128 quantizer and the GEMM, which scales each 128-k chunk's partial sums by the token's and the
+    weight block's scales as it adds them up and rounds the sum and the bias add to bf16.  The weight must come from a
+    bf16 model (the blockwise recipe's only dtype here), and the activations are bf16."""
+    kw = w.act_quant_kwargs
+    N, K = w.qdata.shape
+    if not (_is_128_128_scaled(w.block_size) and _is_1_128_scaled(get_block_size(x.shape, kw.granularity))):
+        raise AssertionError(f"unsupported: {list(w.block_size)} weight blocks with {kw.granularity} activations "
+                             f"(PerBlock activations run with 128x128 weight blocks and 1x128 activation blocks only)")
+    if w.dtype != torch.bfloat16 or x.dtype != torch.bfloat16:
+        raise NotImplementedError(f"float8 blockwise linear: bf16 activations and a weight quantized from bf16 only, got "
+                                  f"{x.dtype} activations and a {w.dtype} weight")
+    if w.qdata.dtype != torch.float8_e4m3fn or kw.float8_dtype != torch.float8_e4m3fn:
+        raise NotImplementedError("float8 blockwise linear: e4m3 weights and activations only")
+    if kw.hp_value_lb is not None or kw.hp_value_ub is not None:
+        raise NotImplementedError("float8 blockwise linear: activation_value_lb / activation_value_ub are not supported")
+    out_shape = (*x.shape[:-1], N)
+    x2 = x.reshape(-1, K)
+    if x2.shape[0] == 0:
+        return x.new_empty(out_shape)
+    xq, xs = torch.ops.ao_b200.fp8_quantize_1x128(rows_for_kernel(x2))
+    y = torch.ops.ao_b200.fp8_blockwise_linear(xq, xs, w.qdata.contiguous(), w.scale.contiguous(), bias)
+    return y.reshape(out_shape)
 
 
 def _weight_only_linear(x, w, bias):
@@ -167,10 +198,25 @@ def _(func, types, args, kwargs):
     sc = self.scale
     if sc.numel() > 1 and sc.shape[dim] == self.qdata.shape[dim]:
         sc = aten.slice.Tensor(sc, dim, start, end, step)
+    elif sc.numel() > 1 and sc.dim() == self.qdata.dim() and 1 < sc.shape[dim] < self.qdata.shape[dim]:
+        sc = _slice_block_scale(sc, self.qdata.shape[dim], dim, start, end)
     bs = list(self.block_size)
     if bs[dim] > qd.shape[dim]:
         bs[dim] = qd.shape[dim]
     return Float8Tensor(qd, sc, bs, self.mm_config, self.act_quant_kwargs, self.kernel_preference, self.dtype)
+
+
+def _slice_block_scale(sc, size, dim, start, end):
+    """The scales of rows / columns [start, end) of a block-scaled tensor (128x128 weight blocks) along dim: whole
+    blocks only (reference _slice_scale_for_dimension, :733-790).  A bound inside a block would leave the sliced tensor
+    with a block it only partly holds, whose scale no longer describes it: ValueError."""
+    block = size // sc.shape[dim]
+    start = 0 if start is None else max(0, start + size if start < 0 else start)
+    end = size if end is None else min(size, end + size if end < 0 else end)
+    if start % block != 0 or (end % block != 0 and end != size):
+        raise ValueError(f"Float8Tensor slice [{start}:{end}] along dim {dim} is not aligned to its scale blocks of "
+                         f"{block}")
+    return aten.slice.Tensor(sc, dim, start // block, -(-end // block), 1)
 
 
 @implements(aten.select.int)

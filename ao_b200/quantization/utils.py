@@ -32,9 +32,10 @@ def unpack_tinygemm_scales_and_zeros(scale_and_zero: torch.Tensor):
 def get_block_size(input_shape: Tuple[int, ...], granularity) -> Tuple[int, ...]:
     """elements per quantization block along each dim (reference :589-633)."""
     if isinstance(granularity, PerBlock):
-        bs = granularity.block_size
-        assert len(bs) == len(input_shape)
-        return tuple(bs)
+        # a shorter block size applies to the trailing dims: padded with leading ones (reference :603-611)
+        bs = (1,) * (len(input_shape) - len(granularity.block_size)) + tuple(granularity.block_size)
+        assert len(bs) == len(input_shape), f"Block size {bs} must have the same number of dimensions as input shape {input_shape}"
+        return bs
     if isinstance(granularity, PerTensor):
         return tuple(input_shape)
     if isinstance(granularity, PerAxis):

@@ -228,6 +228,27 @@ int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale, int M, in
                               const int32_t* offs, uint16_t* y, void* workspace,
                               size_t workspace_bytes, void* stream);
 
+/* fp8 e4m3 blockwise: 1x128 activation blocks, 128x128 weight blocks -------------- */
+/* Replaces Float8Tensor.from_hp(x, PerBlock([1, 128])) for activations (_choose_scale_float8 +
+ * _quantize_affine_float8, quant_primitives.py:2173-2212, :2271-2287): per block of 128 elements of a row,
+ * s = f32(bf16(amax/448)) and q = e4m3(clamp(f32(x)/s, -448, 448)); NaN propagates as in torch.amax / torch.clamp, and
+ * an all-zero block has s = 0 and NaN codes (0/0).  x bf16 [M,K] -> q e4m3 [M,K] (the reference's codes) and the
+ * scales TRANSPOSED, scale_t f32 [K/128][ldm] with ldm = M rounded up to a multiple of 4 (the layout the GEMM loads;
+ * scale_t[kb][m] is the reference's scale[m][kb]; the pad entries m >= M are written as 0).  K % 128 == 0. */
+int ao_fp8_quantize_1x128(const uint16_t* x, int M, int K, uint8_t* q, float* scale_t, void* stream);
+/* The same with row pitch ldx (elements; ldx >= K, ldx % 8 == 0, x 16-byte aligned), see the _ld variants below. */
+int ao_fp8_quantize_1x128_ld(const uint16_t* x, int ldx, int M, int K, uint8_t* q, float* scale_t, void* stream);
+/* Replaces the reference's blockwise GEMM (its Triton loop, float8/kernels.py:86-97, called from
+ * float8_tensor.py:431-447):
+ *   acc[m,n] = sum over 128-k blocks kb, in order, of (Xq Wq^T)_kb[m,n] * x_scale[m][kb] * w_scale[n/128][kb]  (f32)
+ *   y = bf16(bf16(acc) + bias[n]); no add without a bias.
+ * Each block's product and scale multiply-add are one fp32 fma on the block's partial times x_scale.
+ * xq e4m3 [M,K] (16-byte aligned); x_scale_t f32 [K/128][round_up(M,4)] as ao_fp8_quantize_1x128 writes it (16-byte
+ * aligned); wq e4m3 [N,K]; w_scale f32 [N/128][K/128].  K % 128 == 0, N % 128 == 0. */
+int ao_fp8_blockwise_linear(const uint8_t* xq, const float* x_scale_t, int M, int K, const uint8_t* wq,
+                            const float* w_scale, int N, const uint16_t* bias, uint16_t* y, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* mxfp8 (e4m3 data, e8m0 block-32 scales) --------------------------------------- */
 /* Replaces MXTensor.to_mx(x, e4m3, 32, RCEIL, is_swizzled_scales) for activations
  * (mx_tensor.py:228-409, :161-225).  x bf16 [M,K] -> q e4m3 [M,K], scales e8m0 bytes;
