@@ -246,27 +246,18 @@ extern "C" int ao_int4_tilepacked_grouped_mm(const uint16_t* x, int M, int K, co
                                              const int32_t* offs, uint16_t* y, void* workspace,
                                              size_t workspace_bytes, void* stream) {
   using namespace ao;
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int4 grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 1024 == 0, "int4 grouped mm: K=%d must be a multiple of 1024 (format pads K)", K);
   AO_REQUIRE(N % 8 == 0, "int4 grouped mm: N=%d must be a multiple of 8", N);
   AO_REQUIRE(N_out > 0 && N_out <= N, "int4 grouped mm: N_out=%d out of range (N=%d)", N_out, N);
   AO_REQUIRE(group_size == 32 || group_size == 64 || group_size == 128 || group_size == 256,
              "int4 grouped mm: group_size=%d not in {32,64,128,256}", group_size);
-  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "int4 grouped mm: E=%d experts must be in [1, %d]", E, tsg::MAX_EXPERTS);
-  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "int4 grouped mm: E*N=%lld weight rows exceed the int32 range", (long long)E * N);
   AO_REQUIRE((long long)E * (K / group_size) <= 0x7FFFFFFF, "int4 grouped mm: E*K/g=%lld scale rows exceed the int32 range",
              (long long)E * (K / group_size));
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(x && qdata && scale_and_zero && offs && y && workspace, "int4 grouped mm: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "int4 grouped mm: x must be 16-byte aligned");
-  using Fmt = tsg::Grouped<int4k::Int4Fmt>;
-  CUtensorMap tm_w, tm_sz;
-  if (int rc = Fmt::make_grouped_maps(qdata, scale_and_zero, E, N, K, group_size, &tm_w, &tm_sz)) return rc;
-  tsg::Params p{};
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.offs = offs;
-  p.E = E;
-  p.M = M; p.N = N; p.N_out = N_out; p.K = K; p.group_size = group_size;
-  return tsg::run<Fmt>(p, tm_w, tm_sz, x, K, workspace, workspace_bytes, "int4 grouped mm",
-                       reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = int4k::Int4Fmt;
+  return tsg::run_grouped<Fmt>("int4 grouped mm", x, M, K, E, N, N_out, offs, y, workspace, workspace_bytes, stream,
+                               [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_sz) {
+    AO_REQUIRE(qdata && scale_and_zero, "int4 grouped mm: null pointer");
+    p.group_size = group_size;
+    return Fmt::make_grouped_maps(qdata, scale_and_zero, E, N, K, group_size, tm_w, tm_sz);
+  });
 }

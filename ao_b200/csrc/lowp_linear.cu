@@ -692,25 +692,16 @@ extern "C" int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale
                                          const uint8_t* wq, const float* w_scale, int E, int N,
                                          const int32_t* offs, uint16_t* y, void* workspace,
                                          size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
-  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "fp8 grouped mm: E=%d experts must be in [1, %d]", E, tsg::MAX_EXPERTS);
   AO_REQUIRE(K % 16 == 0, "fp8 grouped mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
   AO_REQUIRE(N % 16 == 0, "fp8 grouped mm: N=%d must be a multiple of 16", N);
-  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "fp8 grouped mm: E*N=%lld weight rows exceed the int32 range", (long long)E * N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale && wq && w_scale && offs && y && workspace, "fp8 grouped mm: null pointer");
-  using Fmt = tsg::Grouped<lowp::SsFmt<lowp::KIND_F8>>;
-  CUtensorMap tm_w, tm_aux;
-  if (int rc = Fmt::make_maps(wq, E * N, K, &tm_w, &tm_aux)) return rc;
-  tsg::Params p{};
-  p.row_scale = x_scale;
-  p.w_scale = w_scale;
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.offs = offs;
-  p.E = E;
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<Fmt>(p, tm_w, tm_aux, xq, K, workspace, workspace_bytes, "fp8 grouped mm",
-                             reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::SsFmt<lowp::KIND_F8>;
+  return tsg::run_grouped<Fmt>("fp8 grouped mm", xq, M, K, E, N, N, offs, y, workspace, workspace_bytes, stream,
+                               [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(x_scale && wq && w_scale, "fp8 grouped mm: null pointer");
+    p.row_scale = x_scale;
+    p.w_scale = w_scale;
+    return Fmt::make_maps(wq, E * N, K, tm_w, tm_aux);
+  });
 }
 
 // torch._grouped_mm(x, W.transpose(-2, -1), offs) on weight-only e4m3 expert weights (float8_tensor.py:1085-1122,
@@ -720,29 +711,17 @@ extern "C" int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale
 extern "C" int ao_fp8_weight_grouped_mm(const uint16_t* x, int M, int K, const uint8_t* wq, const float* w_scale, int E,
                                         int N, const int32_t* offs, uint16_t* y, void* workspace,
                                         size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 weight grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
-  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "fp8 weight grouped mm: E=%d experts must be in [1, %d]", E,
-             tsg::MAX_EXPERTS);
   AO_REQUIRE(K % 16 == 0, "fp8 weight grouped mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
   // every scale box (element e*N + 128t of w_scale) starts on 32 bytes and every weight box on a row multiple of 8
   AO_REQUIRE(N % 8 == 0, "fp8 weight grouped mm: N=%d must be a multiple of 8", N);
-  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "fp8 weight grouped mm: E*N=%lld weight rows exceed the int32 range",
-             (long long)E * N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(x && wq && w_scale && offs && y && workspace, "fp8 weight grouped mm: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "fp8 weight grouped mm: x must be 16-byte aligned");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(w_scale) & 15) == 0,
-             "fp8 weight grouped mm: w_scale must be 16-byte aligned (it is loaded by TMA)");
-  using Fmt = tsg::Grouped<lowp::Fp8WoFmt>;
-  CUtensorMap tm_w, tm_s;
-  if (int rc = Fmt::make_maps(wq, w_scale, E * N, K, &tm_w, &tm_s)) return rc;
-  tsg::Params p{};
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.offs = offs;
-  p.E = E;
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<Fmt>(p, tm_w, tm_s, x, K, workspace, workspace_bytes, "fp8 weight grouped mm",
-                       reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::Fp8WoFmt;
+  return tsg::run_grouped<Fmt>("fp8 weight grouped mm", x, M, K, E, N, N, offs, y, workspace, workspace_bytes, stream,
+                               [&](tsg::Params&, CUtensorMap* tm_w, CUtensorMap* tm_s) {
+    AO_REQUIRE(wq && w_scale, "fp8 weight grouped mm: null pointer");
+    AO_REQUIRE((reinterpret_cast<uintptr_t>(w_scale) & 15) == 0,
+               "fp8 weight grouped mm: w_scale must be 16-byte aligned (it is loaded by TMA)");
+    return Fmt::make_maps(wq, w_scale, E * N, K, tm_w, tm_s);
+  });
 }
 
 // torch._grouped_mm(x, W.transpose(-2, -1), offs) on weight-only int8 expert weights, 2-D x 3-D: expert e's rows
@@ -752,27 +731,15 @@ extern "C" int ao_fp8_weight_grouped_mm(const uint16_t* x, int M, int K, const u
 extern "C" int ao_int8_weight_grouped_mm(const uint16_t* x, int M, int K, const int8_t* wq, const float* w_scale, int E,
                                          int N, const int32_t* offs, uint16_t* y, void* workspace,
                                          size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int8 weight grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
-  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "int8 weight grouped mm: E=%d experts must be in [1, %d]", E,
-             tsg::MAX_EXPERTS);
   AO_REQUIRE(K % 16 == 0, "int8 weight grouped mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
   // no N rule: weight boxes may start on any row of the [E * N, K] map, and the scales are read by the epilogue
-  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "int8 weight grouped mm: E*N=%lld weight rows exceed the int32 range",
-             (long long)E * N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(x && wq && w_scale && offs && y && workspace, "int8 weight grouped mm: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "int8 weight grouped mm: x must be 16-byte aligned");
-  using Fmt = tsg::Grouped<lowp::Int8WoFmt>;
-  CUtensorMap tm_w, tm_aux;
-  if (int rc = Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), E * N, K, &tm_w, &tm_aux)) return rc;
-  tsg::Params p{};
-  p.w_scale = w_scale;
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.offs = offs;
-  p.E = E;
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<Fmt>(p, tm_w, tm_aux, x, K, workspace, workspace_bytes, "int8 weight grouped mm",
-                       reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::Int8WoFmt;
+  return tsg::run_grouped<Fmt>("int8 weight grouped mm", x, M, K, E, N, N, offs, y, workspace, workspace_bytes, stream,
+                               [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(wq && w_scale, "int8 weight grouped mm: null pointer");
+    p.w_scale = w_scale;
+    return Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), E * N, K, tm_w, tm_aux);
+  });
 }
 
 // torch._grouped_mm(x, W.transpose(-2, -1), offs) on int8 expert weights with per-token int8 activations: expert e's
@@ -782,27 +749,16 @@ extern "C" int ao_int8_weight_grouped_mm(const uint16_t* x, int M, int K, const 
 extern "C" int ao_int8_dyn_grouped_mm(const int8_t* xq, const float* x_scale, int M, int K, const int8_t* wq,
                                       const float* w_scale, int E, int N, const int32_t* offs, uint16_t* y,
                                       void* workspace, size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int8 grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
-  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "int8 grouped mm: E=%d experts must be in [1, %d]", E, tsg::MAX_EXPERTS);
   AO_REQUIRE(K % 16 == 0, "int8 grouped mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
   AO_REQUIRE(N % 8 == 0, "int8 grouped mm: N=%d must be a multiple of 8 (reference: int8/kernels.py:48-58)", N);
-  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "int8 grouped mm: E*N=%lld weight rows exceed the int32 range",
-             (long long)E * N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale && wq && w_scale && offs && y && workspace, "int8 grouped mm: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(xq) & 15) == 0, "int8 grouped mm: xq must be 16-byte aligned");
-  using Fmt = tsg::Grouped<lowp::SsFmt<lowp::KIND_I8>>;
-  CUtensorMap tm_w, tm_aux;
-  if (int rc = Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), E * N, K, &tm_w, &tm_aux)) return rc;
-  tsg::Params p{};
-  p.row_scale = x_scale;
-  p.w_scale = w_scale;
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.offs = offs;
-  p.E = E;
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<Fmt>(p, tm_w, tm_aux, xq, K, workspace, workspace_bytes, "int8 grouped mm",
-                       reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::SsFmt<lowp::KIND_I8>;
+  return tsg::run_grouped<Fmt>("int8 grouped mm", xq, M, K, E, N, N, offs, y, workspace, workspace_bytes, stream,
+                               [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(x_scale && wq && w_scale, "int8 grouped mm: null pointer");
+    p.row_scale = x_scale;
+    p.w_scale = w_scale;
+    return Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), E * N, K, tm_w, tm_aux);
+  });
 }
 
 extern "C" int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,
@@ -888,26 +844,16 @@ extern "C" int ao_nvfp4_grouped_mm(const uint16_t* x, const float* x_scale, int 
                                    const uint8_t* w_scale_blocked, const float* w_pts, int E, int N,
                                    const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes,
                                    void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "nvfp4 grouped mm: bad sizes M=%d K=%d N=%d", M, K, N);
-  AO_REQUIRE(E >= 1 && E <= tsg::MAX_EXPERTS, "nvfp4 grouped mm: E=%d experts must be in [1, %d]", E, tsg::MAX_EXPERTS);
   AO_REQUIRE(K % 128 == 0, "nvfp4 grouped mm: K=%d must be a multiple of 128", K);
   // every expert's weights and scales start on a 128-row block of the stacked [E * N, ..] tensors
   AO_REQUIRE(N % 128 == 0, "nvfp4 grouped mm: N=%d must be a multiple of 128", N);
-  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "nvfp4 grouped mm: E*N=%lld weight rows exceed the int32 range", (long long)E * N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(x && wq && w_scale_blocked && w_pts && offs && y && workspace, "nvfp4 grouped mm: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "nvfp4 grouped mm: x must be 16-byte aligned");
-  using Fmt = tsg::Grouped<nvf4w::Nvfp4Fmt>;
-  CUtensorMap tm_w, tm_sf;
-  if (int rc = Fmt::make_maps(wq, w_scale_blocked, E * N, K, &tm_w, &tm_sf)) return rc;
-  tsg::Params p{};
-  p.row_scale = x_scale;
-  p.out_scale = w_pts;
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.offs = offs;
-  p.E = E;
-  p.aux_col_blocks = ceil_div(K / 16, 4);
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<Fmt>(p, tm_w, tm_sf, x, K, workspace, workspace_bytes, "nvfp4 grouped mm",
-                       reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = nvf4w::Nvfp4Fmt;
+  return tsg::run_grouped<Fmt>("nvfp4 grouped mm", x, M, K, E, N, N, offs, y, workspace, workspace_bytes, stream,
+                               [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
+    AO_REQUIRE(wq && w_scale_blocked && w_pts, "nvfp4 grouped mm: null pointer");
+    p.row_scale = x_scale;
+    p.out_scale = w_pts;
+    p.aux_col_blocks = ceil_div(K / 16, 4);
+    return Fmt::make_maps(wq, w_scale_blocked, E * N, K, tm_w, tm_sf);
+  });
 }

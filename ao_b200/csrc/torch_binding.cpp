@@ -50,6 +50,28 @@ void check_cuda(const Tensor& t, const char* name) {
 const uint16_t* bf16_ptr(const Tensor& t) { return reinterpret_cast<const uint16_t*>(t.data_ptr()); }
 uint16_t* bf16_ptr_mut(Tensor& t) { return reinterpret_cast<uint16_t*>(t.data_ptr()); }
 
+// torch._grouped_mm(x, W.transpose(-2, -1), offs), 2-D x 3-D, as every grouped op runs it once it has checked its own
+// operands: x [M, K] on the GPU, w the experts' weights [E, ...], offs int32 [E] on x's device (cumulative row ends,
+// never read on the host) -> y [M, n_out] bf16.  The kernels read dense rows from a 16-byte aligned start, so an x
+// that is not (a column slice, a view at an odd storage offset) is copied.  launch(x, y, ws, ws_bytes) makes the op's
+// C call; without rows there is none.
+template <class Launch>
+Tensor grouped_mm(const Tensor& x, const char* name, const Tensor& w, const Tensor& offs, int64_t n_out, Launch launch) {
+  TORCH_CHECK(x.is_cuda(), "ao_b200: ", name, " must be a CUDA tensor");
+  check_cuda(offs, "offs");
+  TORCH_CHECK(offs.scalar_type() == at::kInt && offs.dim() == 1 && offs.size(0) == w.size(0),
+              "ao_b200: offs must be int32 [E], E=", w.size(0));
+  TORCH_CHECK(offs.device() == x.device(), "ao_b200: offs must be on the device of ", name);
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor y = at::empty({x.size(0), n_out}, x.options().dtype(at::kBFloat16));
+  if (x.size(0) == 0) return y;
+  Tensor xc = x.contiguous();
+  if (reinterpret_cast<uintptr_t>(xc.data_ptr()) % 16 != 0) xc = xc.clone();
+  Tensor ws = workspace_for(x);
+  launch(xc.data_ptr(), bf16_ptr_mut(y), ws.data_ptr(), (size_t)ws.numel());
+  return y;
+}
+
 // ------------------------------------------------------------------ int4
 Tensor int4_pack_tile4d(const Tensor& q_u8, int64_t inner_k_tiles) {
   check_cuda(q_u8, "q_u8");
@@ -143,33 +165,24 @@ Tensor int4_tilepacked_linear(const Tensor& x, const Tensor& qdata, int64_t grou
   return y;
 }
 
-// torch._grouped_mm on 3-D int4 expert weights (2-D x 3-D): x bf16 [M, K] (contiguous), qdata int32
-// [E, N/8, K/128, 32, 4], scale_and_zero bf16 [E, K/g, N, 2], offs int32 [E] -> y [M, n_out] (n_out <= 0: N).  Rows
-// from offs[E-1] on are left unwritten, as torch leaves them; offs is never read on the host.
+// torch._grouped_mm on 3-D int4 expert weights (2-D x 3-D): x bf16 [M, K], qdata int32 [E, N/8, K/128, 32, 4],
+// scale_and_zero bf16 [E, K/g, N, 2], offs int32 [E] -> y [M, n_out] (n_out <= 0: N).  Rows from offs[E-1] on are left
+// unwritten, as torch leaves them.
 Tensor int4_tilepacked_grouped_mm(const Tensor& x, const Tensor& qdata, int64_t group_size, const Tensor& scale_and_zero,
                                   const Tensor& offs, int64_t n_out) {
-  TORCH_CHECK(x.is_cuda(), "ao_b200: x must be a CUDA tensor");
   check_cuda(qdata, "qdata");
   check_cuda(scale_and_zero, "scale_and_zero");
-  check_cuda(offs, "offs");
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2, "ao_b200: x must be bf16 [M, K]");
-  TORCH_CHECK(x.size(0) <= 1 || (x.stride(0) == x.size(1) && x.stride(1) == 1), "ao_b200: x must be contiguous");
   TORCH_CHECK(qdata.scalar_type() == at::kInt && qdata.dim() == 5 && qdata.size(3) == 32 && qdata.size(4) == 4, "ao_b200: qdata must be int32 [E, N/8, K/128, 32, 4]");
   TORCH_CHECK(scale_and_zero.scalar_type() == at::kBFloat16 && scale_and_zero.dim() == 4 && scale_and_zero.size(3) == 2, "ao_b200: scale_and_zero must be bf16 [E, K/g, N, 2]");
-  TORCH_CHECK(offs.scalar_type() == at::kInt && offs.dim() == 1, "ao_b200: offs must be int32 [E]");
-  TORCH_CHECK(offs.device() == x.device(), "ao_b200: offs must be on the device of x");
-  c10::cuda::CUDAGuard guard(x.device());
   const int64_t M = x.size(0), K = x.size(1), E = qdata.size(0), N = qdata.size(1) * 8;
   TORCH_CHECK(qdata.size(2) * 128 == K, "ao_b200: x has K=", K, " but qdata encodes K=", qdata.size(2) * 128);
   TORCH_CHECK(scale_and_zero.size(0) == E && scale_and_zero.size(1) * group_size == K && scale_and_zero.size(2) == N, "ao_b200: scale_and_zero shape does not match (E, K/g, N)");
-  TORCH_CHECK(offs.size(0) == E, "ao_b200: offs must have E=", E, " elements");
   if (n_out <= 0) n_out = N;
   TORCH_CHECK(n_out <= N, "ao_b200: n_out > N");
-  Tensor y = at::empty({M, n_out}, x.options());
-  if (M == 0) return y;
-  Tensor ws = workspace_for(x);
-  AO_CALL(ao_int4_tilepacked_grouped_mm(bf16_ptr(x), (int)M, (int)K, qdata.data_ptr<int32_t>(), bf16_ptr(scale_and_zero), (int)group_size, (int)E, (int)N, (int)n_out, offs.data_ptr<int32_t>(), bf16_ptr_mut(y), ws.data_ptr(), (size_t)ws.numel(), cur_stream()));
-  return y;
+  return grouped_mm(x, "x", qdata, offs, n_out, [&](const void* xc, uint16_t* y, void* ws, size_t ws_bytes) {
+    AO_CALL(ao_int4_tilepacked_grouped_mm(static_cast<const uint16_t*>(xc), (int)M, (int)K, qdata.data_ptr<int32_t>(), bf16_ptr(scale_and_zero), (int)group_size, (int)E, (int)N, (int)n_out, offs.data_ptr<int32_t>(), y, ws, ws_bytes, cur_stream()));
+  });
 }
 
 // ------------------------------------------------------------------ meta kernels

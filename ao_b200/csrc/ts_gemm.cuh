@@ -725,5 +725,29 @@ inline int run(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, co
   return launch_gemm<Fmt, Fmt::MAX_N_MMA>(p, tm_w, tm_aux, x, ldx, ws, ws_bytes, what, stream);
 }
 
+// torch._grouped_mm(x, W.transpose(-2, -1), offs), 2-D x 3-D, for every format: expert e's rows [offs[e-1], offs[e])
+// of x [M][K] (dense rows) against rows e*N .. e*N+N-1 of the weight map, into y [M][N_out] under Grouped<Fmt>.  The
+// caller has checked its format's K and N rules.  This checks what every grouped launch needs, returns at M == 0
+// before any pointer is looked at, then `setup(p, &tm_w, &tm_aux)` checks the format's own pointers, sets its Params
+// fields and builds its two maps.
+template <class Fmt, class Setup>
+inline int run_grouped(const char* what, const void* x, int M, int K, int E, int N, int N_out, const int32_t* offs,
+                       uint16_t* y, void* ws, size_t ws_bytes, void* stream, Setup setup) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "%s: bad sizes M=%d K=%d N=%d", what, M, K, N);
+  AO_REQUIRE(E >= 1 && E <= MAX_EXPERTS, "%s: E=%d experts must be in [1, %d]", what, E, MAX_EXPERTS);
+  AO_REQUIRE((long long)E * N <= 0x7FFFFFFF, "%s: E*N=%lld weight rows exceed the int32 range", what, (long long)E * N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && offs && y && ws, "%s: null pointer", what);
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "%s: x must be 16-byte aligned", what);
+  Params p{};
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.offs = offs;
+  p.E = E;
+  p.M = M; p.N = N; p.N_out = N_out; p.K = K;
+  CUtensorMap tm_w, tm_aux;
+  if (int rc = setup(p, &tm_w, &tm_aux)) return rc;
+  return run<Grouped<Fmt>>(p, tm_w, tm_aux, x, K, ws, ws_bytes, what, reinterpret_cast<cudaStream_t>(stream));
+}
+
 }  // namespace tsg
 }  // namespace ao

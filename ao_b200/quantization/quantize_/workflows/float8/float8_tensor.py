@@ -312,11 +312,7 @@ def _weight_only_grouped_mm(mat_a, mat_b, offs, args, kwargs):
     wq = mat_b.qdata.transpose(-2, -1)   # back to the stored [E, N, K]
     ws = mat_b.scale.float()
     ws = ws.reshape(E, N) if ws.numel() == E * N else ws.reshape(1, 1).expand(E, N)
-    # the kernel takes contiguous, 16-byte aligned rows (alignment from the storage offset: traceable with fake tensors)
-    x = mat_a.contiguous()
-    if x.storage_offset() % 8 != 0:
-        x = x.clone()
-    return torch.ops.ao_b200.fp8_weight_grouped_mm(x, wq.contiguous(), ws.contiguous(), offs.to(torch.int32))
+    return torch.ops.ao_b200.fp8_weight_grouped_mm(mat_a, wq.contiguous(), ws.contiguous(), offs.to(torch.int32))
 
 
 Float8Tensor.__module__ = "ao_b200.quantization"

@@ -249,10 +249,6 @@ def _(func, types, args, kwargs):
     k_padded = mat_b.qdata.shape[2] * 128
     if x.shape[-1] != k_padded:
         x = torch.nn.functional.pad(x, (0, k_padded - x.shape[-1]))
-    # the kernel takes contiguous, 16-byte aligned rows (alignment from the storage offset: traceable with fake tensors)
-    x = x.contiguous()
-    if x.storage_offset() % 8 != 0:
-        x = x.clone()
     return torch.ops.ao_b200.int4_tilepacked_grouped_mm(x, mat_b.qdata, max(mat_b.block_size),
                                                         mat_b.scale_and_zero, offs.to(torch.int32), N)
 

@@ -299,12 +299,7 @@ def _(func, types, args, kwargs):
     if kw is None:
         if mat_b.act_pre_scale is not None:
             x = x * mat_b.act_pre_scale
-        # the kernel takes contiguous, 16-byte aligned rows (alignment from the storage offset: traceable with fake
-        # tensors)
-        x = x.to(torch.bfloat16).contiguous()
-        if x.storage_offset() % 8 != 0:
-            x = x.clone()
-        return torch.ops.ao_b200.int8_weight_grouped_mm(x, wq, ws, offs)
+        return torch.ops.ao_b200.int8_weight_grouped_mm(x.to(torch.bfloat16), wq, ws, offs)
     if kw.mapping_type != MappingType.SYMMETRIC or mat_b.act_quant_zero_point is not None:
         raise NotImplementedError(
             f"{what}: asymmetric int8 activations (or a static act_quant_zero_point) need each expert's rowsum(Wq) "

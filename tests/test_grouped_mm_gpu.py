@@ -262,3 +262,43 @@ def test_cuda_graph_replay_with_new_routing():
         torch.cuda.synchronize()
         n = gm_offs(rows)[-1]
         assert torch.equal(y[:n], want[:n]), f"routing {rows}"
+
+
+# ------------------------------------------------------------------------------------------------ activation layouts
+def _grouped_ops(ops, E=4, N=256, K=1024, g=128, M=37):
+    """Every grouped op as (activation dtype, call(x) -> y) on random operands, offs [10, 10, 30, 35] of M = 37 rows."""
+    gen = ex.gen(11)
+    offs = torch.tensor([10, 10, 30, 35], dtype=torch.int32, device=ex.DEV)
+    xs = torch.rand(M, device=ex.DEV, generator=gen) + 0.5
+    ws = torch.rand(E, N, device=ex.DEV, generator=gen) + 0.5
+    w8 = ex.randint(-128, 127, (E, N, K), gen).to(torch.int8)
+    w_e4m3 = torch.randn(E, N, K, device=ex.DEV, generator=gen).to(torch.float8_e4m3fn)
+    w4 = ex.randint(-2**31, 2**31 - 1, (E, N // 8, K // 128, 32, 4), gen).to(torch.int32)
+    sz = (torch.randn(E, K // g, N, 2, device=ex.DEV, generator=gen) * 0.1).to(torch.bfloat16)
+    w_fp4 = ex.randint(0, 255, (E, N, K // 2), gen).to(torch.uint8)
+    sf_fp4 = ex.randint(0x30, 0x3F, (E * N * K // 16,), gen).to(torch.uint8)   # e4m3 block scales 0.5 .. 0.94
+    pts = torch.rand(E, device=ex.DEV, generator=gen) + 0.5
+    return {
+        "fp8_rowwise": (torch.float8_e4m3fn, lambda x: ops.fp8_rowwise_grouped_mm(x, xs, w_e4m3, ws, offs)),
+        "fp8_weight": (torch.bfloat16, lambda x: ops.fp8_weight_grouped_mm(x, w_e4m3, ws, offs)),
+        "int8_weight": (torch.bfloat16, lambda x: ops.int8_weight_grouped_mm(x, w8, ws, offs)),
+        "int8_dyn": (torch.int8, lambda x: ops.int8_dyn_grouped_mm(x, xs, w8, ws, offs)),
+        "nvfp4": (torch.bfloat16, lambda x: ops.nvfp4_grouped_mm(x, xs, w_fp4, sf_fp4, pts, offs)),
+        "int4": (torch.bfloat16, lambda x: ops.int4_tilepacked_grouped_mm(x, w4, g, sz, offs, 0)),
+    }
+
+
+@pytest.mark.parametrize("layout", ["column_slice", "storage_offset"])
+@pytest.mark.parametrize("op", ["fp8_rowwise", "fp8_weight", "int8_weight", "int8_dyn", "nvfp4", "int4"])
+def test_misaligned_activation_views_equal_a_contiguous_copy(ops, op, layout):
+    """Every grouped op takes its activations as any 2-D view: one that does not start on 16 bytes (a column slice of
+    a wider buffer, rows at an odd storage offset) gives the bits of the same call on a dense, aligned copy."""
+    M, K = 37, 1024
+    dtype, call = _grouped_ops(ops, M=M, K=K)[op]
+    wide = torch.randn(M, K + 8, device=ex.DEV, generator=ex.gen(12))
+    wide = (wide * 40).clamp(-128, 127).to(torch.int8) if dtype == torch.int8 else wide.to(dtype)
+    x = wide[:, 4:4 + K] if layout == "column_slice" else wide.flatten()[4:4 + M * K].view(M, K)
+    dense = x.clone(memory_format=torch.contiguous_format)
+    assert x.data_ptr() % 16 != 0 and dense.data_ptr() % 16 == 0
+    y, want = call(x), call(dense)
+    assert torch.equal(y[:35].view(torch.int16), want[:35].view(torch.int16))

@@ -43,6 +43,7 @@ def test_c_abi_argument_validation_without_gpu():
         ptrs[i] = None
         assert call(ptrs=ptrs) == -1 and b"null pointer" in lib.ao_b200_last_error(), i
     assert call(ws=None) == -1 and b"null pointer" in lib.ao_b200_last_error()
+    assert call(ptrs=(ctypes.c_void_p(24),) + (one,) * 5) == -1 and b"16-byte aligned" in lib.ao_b200_last_error()
     # no tokens: nothing to do, nothing dereferenced
     assert call(M=0, ptrs=(None,) * 6, ws=None) == 0
 
