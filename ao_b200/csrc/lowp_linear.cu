@@ -100,7 +100,7 @@ struct SsFmt {
   // PROMOTE (e4m3): the rowwise scales stay in the epilogue, each chunk's partial is added as it is
   struct NoScales {};
   template <int N_MMA>
-  __device__ static __forceinline__ NoScales chunk_scales(const tsg::Params&, uint32_t, int, int, int) { return {}; }
+  __device__ static __forceinline__ NoScales chunk_scales(const tsg::Params&, uint32_t, int, int, int, int) { return {}; }
   template <int N_MMA>
   __device__ static __forceinline__ void promote(uint32_t (&acc)[N_MMA / 2], const uint32_t (&part)[N_MMA / 2],
                                                  uint32_t accumulate, NoScales) {
@@ -129,10 +129,14 @@ struct BlockwiseF8Fmt : SsFmt<KIND_F8> {
   static int make_maps(const uint8_t* wq, const float* x_scale_t, int M, int N, int K, CUtensorMap* tm_w,
                        CUtensorMap* tm_xs) {
     if (int rc = kmajor_byte_map(wq, N, K, tm_w)) return rc;
+    return scale_map(x_scale_t, M, K, MAX_N_MMA, tm_xs);
+  }
+  // the transposed token scales [K/128][round_up(M, 4)], one box of `tokens` scales of one chunk
+  static int scale_map(const float* x_scale_t, int M, int K, uint32_t tokens, CUtensorMap* tm_xs) {
     const uint64_t ldm = ((uint64_t)M + 3) & ~3ull;
     const uint64_t dims[2] = {ldm, (uint64_t)K / KCHUNK};
     const uint64_t str[1] = {ldm * 4};
-    const uint32_t box[2] = {MAX_N_MMA, 1};
+    const uint32_t box[2] = {tokens, 1};
     return make_tmap(tm_xs, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, x_scale_t, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
   }
   __device__ static __forceinline__ void issue_x_aux(const CUtensorMap* tm_xs, uint8_t* aux_dst, uint64_t* bar, int m0,
@@ -147,10 +151,10 @@ struct BlockwiseF8Fmt : SsFmt<KIND_F8> {
     float2 a[N_MMA / 8];
   };
   template <int N_MMA>
-  __device__ static __forceinline__ Scales<N_MMA> chunk_scales(const tsg::Params& p, uint32_t aux_s, int n_tile, int kc,
-                                                               int lane) {
+  __device__ static __forceinline__ Scales<N_MMA> chunk_scales(const tsg::Params& p, uint32_t aux_s, int w_blk, int,
+                                                               int kc, int lane) {
     Scales<N_MMA> cs;
-    cs.w = p.w_scale[(size_t)n_tile * p.KT + kc];
+    cs.w = p.w_scale[(size_t)w_blk * p.KT + kc];
     const uint32_t t = lane & 3;
 #pragma unroll
     for (int q = 0; q < N_MMA / 8; ++q) {
@@ -168,6 +172,38 @@ struct BlockwiseF8Fmt : SsFmt<KIND_F8> {
       const float prev = accumulate ? __uint_as_float(acc[j]) : 0.f;
       acc[j] = __float_as_uint(__fmaf_rn(__fmul_rn(__uint_as_float(part[j]), a), cs.w, prev));
     }
+  }
+};
+
+// Blockwise e4m3 under the grouped schedule (torch._grouped_mm on [E, N, K] experts, ts_gemm_kernel<Grouped<...>>): the
+// weights come from SsFmt::issue_w_rows, row e*N + 128t of the [E*N, K] map; the scales [E, N/128, K/128] are
+// [E*N/128][KT], indexed by the block e*(N/128) + t the kernel passes (W_BLOCK_SCALES).  A tile starts at its expert's
+// first row, any row, and a TMA box whose first element is off a 16-byte boundary faulted on the H100 (an illegal
+// instruction; DESIGN §2a): the token scale box starts at row0 & ~3, 4 scales before the tile at most, and holds
+// MAX_N_MMA + 4 scales, read from row0 & 3 on.  Rows of other experts in it are never stored.
+struct BlockwiseF8GroupedFmt : BlockwiseF8Fmt {
+  static constexpr int X_AUX_BYTES = (MAX_N_MMA + 4) * 4;
+  static constexpr int AUX_BYTES = X_AUX_BYTES;
+  static constexpr bool W_BLOCK_SCALES = true;
+  static int make_maps(const uint8_t* wq, const float* x_scale_t, int M, int N, int K, CUtensorMap* tm_w,
+                       CUtensorMap* tm_xs) {
+    if (int rc = kmajor_byte_map(wq, N, K, tm_w)) return rc;
+    return scale_map(x_scale_t, M, K, MAX_N_MMA + 4, tm_xs);
+  }
+  __device__ static __forceinline__ void issue_x_aux(const CUtensorMap* tm_xs, uint8_t* aux_dst, uint64_t* bar, int m0,
+                                                     int kc, uint64_t policy) {
+    tma_load_2d(aux_dst, tm_xs, bar, m0 & ~3, kc, policy);
+  }
+  template <int N_MMA>
+  __device__ static __forceinline__ Scales<N_MMA> chunk_scales(const tsg::Params& p, uint32_t aux_s, int w_blk, int m0,
+                                                               int kc, int lane) {
+    Scales<N_MMA> cs;
+    cs.w = p.w_scale[(size_t)w_blk * p.KT + kc];
+    const uint32_t base = aux_s + (uint32_t)((m0 & 3) + 2 * (lane & 3)) * 4;   // 4-byte aligned only: two 32-bit loads
+#pragma unroll
+    for (int q = 0; q < N_MMA / 8; ++q)
+      cs.a[q] = make_float2(__uint_as_float(tsg::lds32(base + 32 * q)), __uint_as_float(tsg::lds32(base + 32 * q + 4)));
+    return cs;
   }
 };
 
@@ -701,6 +737,26 @@ extern "C" int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale
     p.row_scale = x_scale;
     p.w_scale = w_scale;
     return Fmt::make_maps(wq, E * N, K, tm_w, tm_aux);
+  });
+}
+
+// torch._grouped_mm(x, W.transpose(-2, -1), offs) on blockwise e4m3 operands: expert e's rows [offs[e-1], offs[e]) of
+// xq (x_scale_t [K/128][round_up(M, 4)] of ao_fp8_quantize_1x128 over all M rows) against wq[e] (the stored [E, N, K]
+// qdata) with its 128x128 block scales w_scale[e] ([E, N/128, K/128]), summed and rounded as the dense
+// ao_fp8_blockwise_linear does, without bias.  offs stays on the device (grouped schedule, ts_gemm.cuh).
+extern "C" int ao_fp8_blockwise_grouped_mm(const uint8_t* xq, const float* x_scale_t, int M, int K, const uint8_t* wq,
+                                           const float* w_scale, int E, int N, const int32_t* offs, uint16_t* y,
+                                           void* workspace, size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(K % 128 == 0, "fp8 blockwise grouped mm: K=%d must be a multiple of 128 (one scale per 128 k)", K);
+  AO_REQUIRE(N % 128 == 0, "fp8 blockwise grouped mm: N=%d must be a multiple of 128 (one scale per 128 rows)", N);
+  using Fmt = lowp::BlockwiseF8GroupedFmt;
+  return tsg::run_grouped<Fmt>("fp8 blockwise grouped mm", xq, M, K, E, N, N, offs, y, workspace, workspace_bytes,
+                               stream, [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_xs) {
+    AO_REQUIRE(x_scale_t && wq && w_scale, "fp8 blockwise grouped mm: null pointer");
+    AO_REQUIRE((reinterpret_cast<uintptr_t>(x_scale_t) & 15) == 0,
+               "fp8 blockwise grouped mm: x_scale must be 16-byte aligned (it is loaded by TMA)");
+    p.w_scale = w_scale;
+    return Fmt::make_maps(wq, x_scale_t, M, E * N, K, tm_w, tm_xs);
   });
 }
 

@@ -69,6 +69,17 @@ struct XAux<F, std::void_t<decltype(F::X_AUX_BYTES)>> {
   static constexpr int BYTES = F::X_AUX_BYTES;
 };
 
+// Fmt::W_BLOCK_SCALES (optional, default false): Fmt::chunk_scales reads a scale per 128-row weight block, so a grouped
+// kernel passes it the block of the expert's weights (e * n_tiles + n_tile), looked up once per segment
+template <class F, class = void>
+struct WBlockScales {
+  static constexpr bool value = false;
+};
+template <class F>
+struct WBlockScales<F, std::void_t<decltype(F::W_BLOCK_SCALES)>> {
+  static constexpr bool value = F::W_BLOCK_SCALES;
+};
+
 template <class Fmt, int N_MMA>
 constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA && !IsGrouped<Fmt>::value ? 2 : 1; }
 constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
@@ -91,7 +102,7 @@ struct Params {
   int grid_forced;          // Grouped<Fmt>: the host grid was forced (ao_b200_debug_set_streamk_ctas): no MIN_UNITS rule
   const float* w_scale;     // EPI_I8 / EPI_F8 / EPI_BF16_WSCALE: per-output-feature weight scale [N] (EPI_BF16 never
                             // reads it: its format applies the scale per weight, from the aux operand, or, blockwise
-                            // e4m3, per 128x128 block [N/128][KT] in its promotion)
+                            // e4m3, per 128x128 block [N/128][KT] in its promotion; grouped: [E * N/128][KT])
   __nv_bfloat16* y;         // [M, N_out]
   int32_t* i32_out;         // EPI_I8: raw int32 accumulators [M, N] instead of y
   float* ws_partial;        // [grid][N_MMA*128]   CTA b's CONTRIB partial (streamk.cuh)
@@ -226,7 +237,10 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 //                                                                  [E * N, K] map of all experts, and their aux tiles
 //   EXPERT_SCALE (grouped EPI_FLOAT only): the epilogue multiplies by out_scale[e] (nvfp4: yes, int4: no scale at all)
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
-//   PROMOTE: cs = chunk_scales<N_MMA>(p, aux smem, n_tile, kc, lane)  the chunk's scales (before its wgmmas)
+//   PROMOTE: cs = chunk_scales<N_MMA>(p, aux smem, w_blk, m0, kc, lane)  the chunk's scales (before its wgmmas); w_blk
+//                                                                  is the weight's 128-row block: n_tile, or under the
+//                                                                  grouped schedule (W_BLOCK_SCALES) e * n_tiles +
+//                                                                  n_tile; m0 the tile's first token row
 //            static void promote<N_MMA>(acc, part, accumulate, cs)   acc (+)= the chunk's partial sums, scaled by cs
 //   RA:  struct Raw; static void load(p, w smem, aux smem, row_lo, lane, Raw&)   rows row_lo and row_lo + 8
 //        static void frag(p, raw, kk, a[4])                        bf16 A fragment of k16 step kk (0..7)
@@ -578,6 +592,14 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
     int i = 0;
     for (int seg = 0; seg < walk.nseg; ++seg) {
       const int cnt = walk.seg_count(seg);
+      // grouped, W_BLOCK_SCALES: the 128-row weight block of the segment's tile in [E * N / 128], and its first row
+      int w_blk = 0, row0 = 0;
+      if constexpr (GROUPED && WBlockScales<Fmt>::value) {
+        const int tile = walk.seg_tile(seg);
+        const GroupTile gt = group_tile<N_MMA>(g_end, g_mbp, p.E, tile / p.n_tiles);
+        w_blk = gt.e * p.n_tiles + tile % p.n_tiles;
+        row0 = gt.row0;
+      }
       for (int c = 0; c < cnt; ++c, ++i) {
         const uint32_t scale_d = c > 0;   // the first wgmma of a segment overwrites the accumulator
         const int s = i % S;
@@ -591,7 +613,9 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           // format's chunk scales (none for rowwise) are read before the wgmmas, so their loads overlap them, and
           // before the stage goes back
           mbar_wait(&xfull[s], ph);
-          const auto cs = Fmt::template chunk_scales<N_MMA>(p, aux_s, tile_of(i) % p.n_tiles, kc_of(i), lane);
+          const auto cs = Fmt::template chunk_scales<N_MMA>(p, aux_s, GROUPED ? w_blk : tile_of(i) % p.n_tiles,
+                                                            GROUPED ? row0 : (tile_of(i) / p.n_tiles) * N_MMA,
+                                                            kc_of(i), lane);
           uint32_t part[NACC];
           wgmma_fence();
           Fmt::template mma<N_MMA>(part, w_s, x_s, wg, 0u);

@@ -37,6 +37,11 @@ def _is_128_128_scaled(block_size) -> bool:
     return len(block_size) == 2 and block_size[0] == 128 and block_size[1] == 128
 
 
+def _is_1_128_128_scaled(block_size) -> bool:
+    """128x128 blocks of each expert of a 3-D weight [E, N, K] (or its transposed view), block_size [1, 128, 128]."""
+    return len(block_size) == 3 and block_size[0] == 1 and block_size[1] == 128 and block_size[2] == 128
+
+
 def _granularity_is_a_1_128_w_128_128(g) -> bool:
     """The blockwise pair, by the dataclasses' equality as the reference compares it (reference :217-228): the block
     sizes are compared as given, so PerBlock([1, 128]) matches and PerBlock((1, 128)) does not."""

@@ -17,8 +17,8 @@ from typing import List, Optional
 import torch
 from torch.utils._python_dispatch import return_and_correct_aliasing
 
-from ao_b200.float8.inference import (FP8Granularity, Float8MMConfig, _is_1_128_scaled, _is_128_128_scaled,
-                                      _is_rowwise_scaled, _is_tensorwise_scaled)
+from ao_b200.float8.inference import (FP8Granularity, Float8MMConfig, _is_1_128_128_scaled, _is_1_128_scaled,
+                                      _is_128_128_scaled, _is_rowwise_scaled, _is_tensorwise_scaled)
 from ao_b200.quantization.granularity import PerBlock, PerRow, PerTensor
 from ao_b200.quantization.quant_primitives import (
     choose_scale_float8, dequantize_affine_float8, quantize_affine_float8)
@@ -250,7 +250,8 @@ def _(func, types, args, kwargs):
     """torch._grouped_mm(x, W.transpose(-2, -1), offs=offs) with a Float8Tensor expert weight W [E, N, K] (the
     reference's handler, float8_tensor.py:1085-1122).  Dynamic (rowwise) activations: the routed tokens are quantized
     per row and the grouped GEMM runs on the stored qdata with w_scale[e, n].  Only the 2-D x 3-D form with PerRow
-    activations.  Weight-only: _weight_only_grouped_mm."""
+    activations.  Weight-only: _weight_only_grouped_mm.  PerBlock([1, 128]) activations on [1, 128, 128] weight
+    blocks: _blockwise_grouped_mm."""
     mat_a, mat_b = args[0], args[1]
     offs = args[2] if len(args) > 2 else kwargs.get("offs", None)
     assert isinstance(mat_b, Float8Tensor)
@@ -259,6 +260,10 @@ def _(func, types, args, kwargs):
     act_quant_kwargs = mat_b.act_quant_kwargs
     if act_quant_kwargs is None:
         return _weight_only_grouped_mm(mat_a, mat_b, offs, args, kwargs)
+    gran = act_quant_kwargs.granularity
+    if (isinstance(gran, PerBlock) and _is_1_128_scaled(gran.block_size)
+            and _is_1_128_128_scaled(mat_b.block_size)):
+        return _blockwise_grouped_mm(mat_a, mat_b, offs, args, kwargs)
     if not isinstance(act_quant_kwargs.granularity, PerRow):
         raise NotImplementedError(f"_grouped_mm only supports PerRow granularity, got {act_quant_kwargs.granularity}")
     if mat_a.dim() != 2 or mat_b.dim() != 3:
@@ -275,6 +280,41 @@ def _(func, types, args, kwargs):
                                                  wq.contiguous(), mat_b.scale.reshape(E, N).float().contiguous(),
                                                  offs.to(torch.int32))
     return y.to(mat_a.dtype)
+
+
+def _blockwise_grouped_mm(mat_a, mat_b, offs, args, kwargs):
+    """1x128 activation blocks on [1, 128, 128] expert weight blocks: the reference's per-expert recipe, select and
+    the dense blockwise linear (_blockwise_linear), in two launches.  The 1x128 quantizer runs once over all routed rows
+    (it is per row, so this equals quantizing each expert's rows on their own), then one grouped GEMM sums and rounds
+    each expert's rows as the dense GEMM does.  Rows from offs[-1] on are left unwritten, as torch leaves them.  Only
+    the 2-D x 3-D form of a bf16 model, bf16 mat_a and output, e4m3, no bias and no activation clamp."""
+    kw = mat_b.act_quant_kwargs
+    bias = args[3] if len(args) > 3 else kwargs.get("bias", None)
+    out_dtype = args[4] if len(args) > 4 else kwargs.get("out_dtype", None)
+    if mat_b.dtype != torch.bfloat16:
+        raise NotImplementedError(f"Float8Tensor blockwise _grouped_mm: the weight was quantized from {mat_b.dtype}; "
+                                  f"the sm_90a kernel of this engine serves weights quantized from torch.bfloat16 only")
+    if isinstance(mat_a, TorchAOBaseTensor) or mat_a.dtype != torch.bfloat16 or out_dtype not in (None, torch.bfloat16):
+        raise NotImplementedError(f"Float8Tensor blockwise _grouped_mm: bf16 mat_a and output only, got "
+                                  f"{mat_a.dtype} -> {out_dtype}")
+    if mat_b.qdata.dtype != torch.float8_e4m3fn or kw.float8_dtype != torch.float8_e4m3fn:
+        raise NotImplementedError(f"Float8Tensor blockwise _grouped_mm: e4m3 weights and activations only, got "
+                                  f"{mat_b.qdata.dtype} weights and {kw.float8_dtype} activations")
+    if kw.hp_value_lb is not None or kw.hp_value_ub is not None:
+        raise NotImplementedError("Float8Tensor blockwise _grouped_mm: activation_value_lb / activation_value_ub are "
+                                  "not supported")
+    if bias is not None:
+        raise NotImplementedError("Float8Tensor blockwise _grouped_mm: bias is not supported")
+    if mat_a.dim() != 2 or mat_b.dim() != 3:
+        raise NotImplementedError(f"Float8Tensor blockwise _grouped_mm: only 2-D mat_a x 3-D mat_b, got "
+                                  f"{mat_a.dim()}-D x {mat_b.dim()}-D")
+    E, K, N = mat_b.shape
+    if mat_a.shape[-1] != K:
+        raise ValueError(f"_grouped_mm: mat_a has K={mat_a.shape[-1]}, mat_b K={K}")
+    xq, xs = torch.ops.ao_b200.fp8_quantize_1x128(rows_for_kernel(mat_a))
+    # back to the stored [E, N, K] codes and [E, N/128, K/128] scales
+    return torch.ops.ao_b200.fp8_blockwise_grouped_mm(xq, xs, mat_b.qdata.transpose(-2, -1).contiguous(),
+                                                      mat_b.scale.transpose(-2, -1).contiguous(), offs.to(torch.int32))
 
 
 def _weight_only_grouped_mm(mat_a, mat_b, offs, args, kwargs):

@@ -248,6 +248,19 @@ int ao_fp8_quantize_1x128_ld(const uint16_t* x, int ldx, int M, int K, uint8_t* 
 int ao_fp8_blockwise_linear(const uint8_t* xq, const float* x_scale_t, int M, int K, const uint8_t* wq,
                             const float* w_scale, int N, const uint16_t* bias, uint16_t* y, void* workspace,
                             size_t workspace_bytes, void* stream);
+/* torch._grouped_mm(x, W.transpose(-2, -1), offs) for a 3-D blockwise Float8Tensor expert weight W [E, N, K]
+ * (block_size [1, 128, 128]), 2-D x 3-D form, as the per-expert recipe select + ao_fp8_blockwise_linear computes it:
+ * for offs[e-1] <= m < offs[e] (offs[-1] = 0)
+ *   acc[m,n] = sum over 128-k blocks kb, in order, of (Xq Wq[e]^T)_kb[m,n] * x_scale[m][kb] * w_scale[e][n/128][kb]
+ *   y[m,n] = bf16(acc[m,n]),  no bias.
+ * xq e4m3 [M,K] (tokens sorted by expert, 16-byte aligned); x_scale_t f32 [K/128][round_up(M,4)] as
+ * ao_fp8_quantize_1x128 writes it over all M rows (16-byte aligned); wq e4m3 [E][N][K] (the stored qdata); w_scale f32
+ * [E][N/128][K/128]; offs int32 [E] on the device, cumulative row ends.  The host never reads offs (no sync,
+ * CUDA-graph capturable); the kernel clamps each offs[e] into [offs[e-1], M].  Rows from offs[E-1] on are not written.
+ * 1 <= E <= 1024, K % 128 == 0, N % 128 == 0.  At M == 0 it returns before reading any pointer. */
+int ao_fp8_blockwise_grouped_mm(const uint8_t* xq, const float* x_scale_t, int M, int K, const uint8_t* wq,
+                                const float* w_scale, int E, int N, const int32_t* offs, uint16_t* y, void* workspace,
+                                size_t workspace_bytes, void* stream);
 
 /* mxfp8 (e4m3 data, e8m0 block-32 scales) --------------------------------------- */
 /* Replaces MXTensor.to_mx(x, e4m3, 32, RCEIL, is_swizzled_scales) for activations

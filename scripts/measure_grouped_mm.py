@@ -4,7 +4,7 @@ F.scaled_grouped_mm on identical operands, for MoE expert shapes; with --fmt nvf
 per-expert activation quantizer nvfp4_fakequant_grouped plus nvfp4_grouped_mm) against the fp8 path with its
 quantizer (fp8_quantize_rowwise plus fp8_rowwise_grouped_mm) and bf16 torch._grouped_mm on the unquantized weights.
 
-  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4|fp8wo|int8wo|int8] [--group-size 32] [--replays 20]
+  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4|fp8wo|int8wo|int8|fp8_blockwise] [--group-size 32] [--replays 20]
                                        [--out FILE]
 
   * shapes: Mixtral-8x7B experts (E=8, 4096 -> 14336 and 14336 -> 4096, top-2) and Qwen3-30B-A3B experts (E=128,
@@ -35,7 +35,16 @@ the reference's per-expert recipe restated in torch (int8wo: torch.mm on qdata.t
 per-row quantization, torch._int_mm and the pointwise epilogue), bf16 torch._grouped_mm and the fp8 counterpart (fp8
 weight-only, or fp8 rowwise with its quantizer); bytes are the int8 path's (1 byte per weight and 4 per row scale of
 the active experts, the activations as the GEMM reads them, the outputs, offs), its roofline term their HBM time, and
-vs_select_linear compares the output with select + F.linear on every active expert.
+vs_select_linear compares the output with select + F.linear on every active expert.  --fmt fp8_blockwise: the blockwise
+e4m3 expert path (torch._grouped_mm on 3-D Float8Tensor weights with [1, 128, 128] blocks: the 1x128 quantizer plus
+fp8_blockwise_grouped_mm) against the eager loop of select + the dense blockwise linear on each active expert (its
+quantizer and GEMM, captured with the routing fixed, without the host sync that reads offs), the rowwise fp8 grouped
+op with its quantizer on the same codes, and bf16 torch._grouped_mm, on the shapes above plus DeepSeek-V3's experts
+(E=256, 7168 -> 4096 gate|up and 2048 -> 7168 down, top-8); bytes are the blockwise path's (1 byte per weight and 4 per
+128x128 block scale of the active experts, the e4m3 activations and their 1x128 scales, the outputs, offs), its
+roofline term their HBM time, and vs_select_linear compares the output with the loop's.  Torch's blockwise
+F.scaled_grouped_mm is tried and reported as unavailable when this torch build lacks it (it needs torch built for
+CUDA 12.9 or later).  Prefill (2048-token) cases time one round of weight copies per replay.
 """
 from __future__ import annotations
 
@@ -55,6 +64,7 @@ FP8_FLOPS = 1979e12
 SHAPES = [("mixtral-8x7b w1/w3", 8, 14336, 4096, 2), ("mixtral-8x7b w2", 8, 4096, 14336, 2),
           ("qwen3-30b-a3b gate/up", 128, 768, 2048, 8), ("qwen3-30b-a3b down", 128, 2048, 768, 8)]
 TOKENS = [1, 8, 32, 128, 2048]
+DEEPSEEK_SHAPES = [("deepseek-v3 gate|up", 256, 4096, 7168, 8), ("deepseek-v3 down", 256, 7168, 2048, 8)]
 
 
 def card():
@@ -405,9 +415,102 @@ def measure_int8(a, ops, dev, lines):
         torch.cuda.empty_cache()
 
 
+def measure_fp8_blockwise(a, ops, dev, lines):
+    """The blockwise e4m3 expert path (quantizer + grouped GEMM) against the eager select + dense blockwise loop, the
+    rowwise fp8 grouped op (quantizer + GEMM) on the same codes, and bf16 torch._grouped_mm.  DeepSeek-V3's gate|up is
+    7.5 GB of e4m3 (15 GB of bf16) for all 256 experts: its weights are made and quantized 16 experts at a time, and one
+    copy of its active experts' weights is already far past L2."""
+    import torch
+    import torch.nn.functional as F
+
+    from ao_b200.quantization import Float8Tensor, PerBlock, QuantizeTensorToFloat8Kwargs
+
+    act = QuantizeTensorToFloat8Kwargs(granularity=PerBlock([1, 128]))
+    for name, E, N, K, topk in SHAPES + DEEPSEEK_SHAPES:
+        g = torch.Generator(device=dev).manual_seed(E * N + K)
+        w_bytes_expert = N * K + (N // 128) * (K // 128) * 4
+        copies = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * w_bytes_expert)) + 1)
+        copies_bf16 = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * N * K * 2)) + 1)
+        wt, wb = [], []
+        for c in range(max(copies, copies_bf16)):
+            w = torch.randn(E, N, K, device=dev, generator=g, dtype=torch.bfloat16).mul_(0.05)
+            if c < copies:
+                parts = [Float8Tensor.from_hp(w[e0:e0 + 16], granularity=PerBlock([128, 128])) for e0 in range(0, E, 16)]
+                wt.append(Float8Tensor(torch.cat([p.qdata for p in parts]), torch.cat([p.scale for p in parts]),
+                                       [1, 128, 128], parts[0].mm_config, act, dtype=torch.bfloat16))
+                del parts
+            if c < copies_bf16:
+                wb.append(w)
+            del w
+        ones = torch.ones(E, N, device=dev)   # the rowwise op's scales: only its time is compared
+        for T in TOKENS:
+            for skewed in (False, True):
+                rows = routing(T, E, topk, skewed, seed=T * 131 + E + skewed)
+                M = sum(rows)
+                offs = torch.tensor(rows, dtype=torch.int64).cumsum(0).to(torch.int32).to(dev)
+                x = torch.randn(M, K, device=dev, generator=g).to(torch.bfloat16)
+                active = sum(1 for r in rows if r)
+                need = active * w_bytes_expert + M * K + M * (K // 128) * 4 + M * N * 2 + E * 4
+                rec = dict(fmt="fp8_blockwise", shape=name, E=E, N=N, K=K, topk=topk, tokens=T,
+                           routing="skewed" if skewed else "balanced", rows=M, active_experts=active, bytes=need,
+                           weight_copies=copies, roofline_us=round(need / HBM_BPS * 1e6, 2))
+                spans, start = [], 0
+                for e, r in enumerate(rows):
+                    if r:
+                        spans.append((e, start, start + r))
+                    start += r
+
+                def ours(c):
+                    return torch._grouped_mm(x, wt[c].transpose(-2, -1), offs=offs)
+
+                def loop(c, out=None):
+                    w = wt[c]
+                    for e, s0, s1 in spans:
+                        q, s = ops.fp8_quantize_1x128(x[s0:s1])
+                        y = ops.fp8_blockwise_linear(q, s, w.qdata[e], w.scale[e], None)
+                        if out is not None:
+                            out.append(y)
+
+                def rowwise(c):
+                    xq, sx = ops.fp8_quantize_rowwise(x)
+                    return ops.fp8_rowwise_grouped_mm(xq, sx.reshape(-1), wt[c].qdata, ones, offs)
+
+                def bf16(c):
+                    return torch._grouped_mm(x, wb[c].transpose(-2, -1), offs=offs)
+
+                n = int(offs[-1])
+                y = ours(0)[:n]
+                y_loop = []
+                loop(0, y_loop)
+                y_loop = torch.cat(y_loop)
+                rec["vs_select_linear"] = "identical" if torch.equal(y.view(torch.int16), y_loop.view(torch.int16)) \
+                    else sqnr_db(y_loop, y)
+                rec["sqnr_vs_bf16_db"] = sqnr_db(bf16(0)[:n], y)
+                rounds = 1 if T >= 2048 else None
+                for key, fn, cp in (("ours", ours, copies), ("expert_loop", loop, copies), ("fp8_rowwise", rowwise, copies),
+                                    ("bf16", bf16, copies_bf16)):
+                    us = time_graph(fn, cp, a.replays, rounds)
+                    rec[f"{key}_us"] = round(us, 2)
+                    rec[f"{key}_GBps"] = round(need / us * 1e-3, 1)
+                try:
+                    xq, xs = ops.fp8_quantize_1x128(x)
+                    F.scaled_grouped_mm(xq, wt[0].qdata.transpose(-2, -1), scale_a=xs[:, :M].t().contiguous(),
+                                        scale_recipe_a=F.ScalingType.BlockWise1x128, scale_b=wt[0].scale,
+                                        scale_recipe_b=F.ScalingType.BlockWise128x128, offs=offs,
+                                        output_dtype=torch.bfloat16)
+                    rec["torch_scaled_grouped_mm"] = "ran (not timed)"
+                except Exception as e:   # the blockwise recipes need torch built for CUDA 12.9 or later
+                    rec["torch_scaled_grouped_mm"] = (f"unavailable in torch {torch.__version__} (CUDA {torch.version.cuda}): "
+                                                      f"{str(e).splitlines()[0][:160]}")
+                print(json.dumps(rec), flush=True)
+                lines.append(rec)
+        del wt, wb, ones
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4", "fp8wo", "int8wo", "int8"], default="fp8")
+    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4", "fp8wo", "int8wo", "int8", "fp8_blockwise"], default="fp8")
     ap.add_argument("--group-size", type=int, choices=[32, 64, 128, 256], default=32)
     ap.add_argument("--replays", type=int, default=20)
     ap.add_argument("--out", default=None)
@@ -480,6 +583,8 @@ def main():
         measure_fp8wo(a, ops, dev, lines)
     if a.fmt in ("int8wo", "int8"):
         measure_int8(a, ops, dev, lines)
+    if a.fmt == "fp8_blockwise":
+        measure_fp8_blockwise(a, ops, dev, lines)
     info = dict(card=card(), torch=torch.__version__)
     print(json.dumps(info), flush=True)
     if a.out:
