@@ -3,6 +3,7 @@
 //                         and, per expert, aten._int_mm on select()ed int8 expert weights
 //   e4m3 x e4m3 -> f32    (wgmma e4m3, both operands TMA tiles)    replaces torch._scaled_mm rowwise
 //                         and, 1x128 x 128x128 block scales, the reference's blockwise Triton GEMM
+//                         and, 2:4-sparse weights (wgmma.sp), the reference's CUTLASS sparse GEMM
 //   mxfp8 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm block-scaled
 //   nvfp4 block-16 e4m3   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm fp4 + pts/bias kernels
 //   nvfp4 weight x bf16   (bf16 wgmma, weights dequantised exactly)      replaces F.linear on the dequantised weight
@@ -204,6 +205,81 @@ struct BlockwiseF8GroupedFmt : BlockwiseF8Fmt {
     for (int q = 0; q < N_MMA / 8; ++q)
       cs.a[q] = make_float2(__uint_as_float(tsg::lds32(base + 32 * q)), __uint_as_float(tsg::lds32(base + 32 * q + 4)));
     return cs;
+  }
+};
+
+// 2:4-sparse e4m3 (Float8DynamicActivationFloat8WeightConfig with packing_format SPARSE_2D_DATA_2D_METADATA; reference
+// float8_sparse_2x4_2d_data_2d_metadata_tensor.py and its CUTLASS GEMM rowwise_scaled_linear_sparse_cutlass.cuh).
+// Weights: the compressed codes wq [N][K/2] (each 4-k group keeps its two stored codes) and the metadata wm as CUTLASS's
+// Sm90 sparse compressor writes it: atoms of 64 rows x 128 k, 16 bytes per row (one 4-bit nibble per 4-k group, the
+// two kept positions in bits 1:0 and 3:2), atoms along N first, then along K, so that the metadata of column block kc
+// starts at byte kc * round_up(N, 64) * 16 and a tile's two atoms are 2 KiB in a row.
+// Per 128-k chunk a stage holds the tile's compressed codes (128 rows x 64 bytes, 64-byte swizzle), its two metadata
+// atoms in the aux slot (one 2 KiB box of 8-byte words; past round_up(N, 64) zero-filled) and the e4m3 activation tile.
+// MMA: two wgmma.sp k64 per chunk.  PTX ISA, sparse wgmma metadata for 8-bit types: thread (warp w, lane l) of the
+// warpgroup supplies the 32 k of row 16w + l/4 + 8(l%2), k 32((l/2)%2) .. + 31 of the k64 step, group j at bits 4j+3:4j.
+// The chunks of a segment accumulate in the wgmma accumulator (the reference's FP8FastAccum mainloop: no promotion),
+// each chunk's wgmmas completing before the next chunk's are issued (ts_gemm.cuh), and the epilogue is EPI_F8_SPARSE.
+// Metadata nibbles 0b0000, 0b0101, 0b1010, 0b1111 (both positions equal) are undefined behaviour for the MMA.  The
+// reference's compressor writes 0b0000 for an all-zero group and for its padding, and its allocation leaves any bytes
+// it did not write as they were, so meta() replaces every word of rows >= N or k >= K by 0x44444444 (positions 0, 1)
+// and every 0b0000 nibble by 0b0100.  A 0b0000 group's two stored codes are zero, so the product is unchanged.
+struct SparseF8Fmt {
+  static constexpr bool SS = true;
+  static constexpr bool SPARSE_A = true;
+  static constexpr bool PROMOTE = false;
+  static constexpr bool DECODE_2CTA = true;
+  static constexpr int X_ELEM_BYTES = 1;
+  static constexpr int W_BYTES = ROWS * KCHUNK / 2;   // 8 KiB of compressed codes
+  static constexpr int META_BYTES = 2 * 64 * 16;      // two metadata atoms
+  static constexpr int AUX_BYTES = META_BYTES;
+  static constexpr int EPI = tsg::EPI_F8_SPARSE;
+  static constexpr int ACC_EXP2 = 0;
+  static constexpr int MAX_N_MMA = 128;
+  static int make_maps(const uint8_t* wq, const uint8_t* wm, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_m) {
+    {
+      const uint64_t dims[2] = {(uint64_t)K / 2, (uint64_t)N};
+      const uint64_t str[1] = {(uint64_t)K / 2};
+      const uint32_t box[2] = {64, ROWS};
+      if (int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B))
+        return rc;
+    }
+    // [KT][round_up(N, 64) * 16 bytes] as 8-byte words, one box = one tile's two atoms
+    const uint64_t row_words = (uint64_t)ceil_div(N, 64) * 64 * 16 / 8;
+    const uint64_t dims[2] = {row_words, (uint64_t)ceil_div(K, KCHUNK)};
+    const uint64_t str[1] = {row_words * 8};
+    const uint32_t box[2] = {META_BYTES / 8, 1};
+    return make_tmap(tm_m, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, wm, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
+  __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES + META_BYTES; }
+  __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap* tm_m, const tsg::Params&,
+                                                 uint8_t* w_dst, uint8_t* aux_dst, uint64_t* bar, int n_tile, int kc,
+                                                 uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * (KCHUNK / 2), n_tile * ROWS, policy);
+    tma_load_2d(aux_dst, tm_m, bar, n_tile * (META_BYTES / 8), kc, policy);
+  }
+  // valid words as they are except 0b0000 nibbles -> 0b0100; words of rows >= N or k >= K: 0x44444444
+  __device__ static __forceinline__ uint32_t sanitize(uint32_t w, bool valid) {
+    w = valid ? w : 0x44444444u;
+    uint32_t z = w | (w >> 1);
+    z |= z >> 2;
+    return w | ((~z & 0x11111111u) << 2);
+  }
+  // the thread's metadata words of k64 steps 0 and 1 (row: its metadata row 0..127 of the tile)
+  __device__ static __forceinline__ uint2 meta(const tsg::Params& p, uint32_t aux_s, int n_tile, int kc, int row,
+                                               int lane) {
+    const int half = (lane >> 1) & 1;
+    const uint32_t a = aux_s + (uint32_t)(row >> 6) * 1024u + (uint32_t)(row & 63) * 16u + 4u * half;
+    const bool row_ok = n_tile * ROWS + row < p.N;
+    const int k0 = kc * KCHUNK + 32 * half;
+    return make_uint2(sanitize(tsg::lds32(a), row_ok && k0 < p.K), sanitize(tsg::lds32(a + 8), row_ok && k0 + 64 < p.K));
+  }
+  template <int N_MMA>
+  __device__ static __forceinline__ void mma(uint32_t (&acc)[N_MMA / 2], uint32_t w_s, uint32_t x_s,
+                                             const uint32_t (&mt)[2], int wg, uint32_t scale_d) {
+    // k64 step j: 32 bytes of each compressed row, 64 bytes of each activation row
+    Wgmma<N_MMA>::sp_e4m3(acc, wgmma_desc_k_sw64(w_s + wg * (64 * 64)), wgmma_desc_k_sw128(x_s), mt[0], scale_d);
+    Wgmma<N_MMA>::sp_e4m3(acc, wgmma_desc_k_sw64(w_s + wg * (64 * 64) + 32), wgmma_desc_k_sw128(x_s + 64), mt[1], 1u);
   }
 };
 
@@ -719,6 +795,34 @@ extern "C" int ao_fp8_blockwise_linear(const uint8_t* xq, const float* x_scale_t
   p.M = M; p.N = N; p.N_out = N; p.K = K;
   return tsg::run<lowp::BlockwiseF8Fmt>(p, tm_w, tm_xs, xq, K, workspace, workspace_bytes, "fp8 blockwise linear",
                                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+// F.linear(x, Float8Sparse2x4_2DData2DMetadataTensor) (float8_sparse_2x4_2d_data_2d_metadata_tensor.py): per-token
+// e4m3 xq with x_scale [M], the 2:4-compressed weights wq [N][K/2] with the CUTLASS metadata w_meta
+// (round_up(N, 64) x round_up(K, 128) / 8 bytes, SparseF8Fmt) and w_scale [N]:
+// y = bf16(fma(acc * w_scale[n], x_scale[m], bias[n])), acc summed without promotion (SparseF8Fmt)
+extern "C" int ao_fp8_sparse_linear(const uint8_t* xq, const float* x_scale, int M, int K, const uint8_t* wq,
+                                    const uint8_t* w_meta, const float* w_scale, int N, const uint16_t* bias, uint16_t* y,
+                                    void* workspace, size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 sparse linear: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(K % 32 == 0, "fp8 sparse linear: K=%d must be a multiple of 32 (16-byte rows of compressed codes)", K);
+  AO_REQUIRE(N % 16 == 0, "fp8 sparse linear: N=%d must be a multiple of 16", N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(xq && x_scale && wq && w_meta && w_scale && y, "fp8 sparse linear: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(xq) & 15) == 0, "fp8 sparse linear: xq must be 16-byte aligned");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(wq) & 15) == 0, "fp8 sparse linear: wq must be 16-byte aligned");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(w_meta) & 15) == 0,
+             "fp8 sparse linear: w_meta must be 16-byte aligned (it is loaded by TMA)");
+  CUtensorMap tm_w, tm_m;
+  if (int rc = lowp::SparseF8Fmt::make_maps(wq, w_meta, N, K, &tm_w, &tm_m)) return rc;
+  tsg::Params p{};
+  p.row_scale = x_scale;
+  p.w_scale = w_scale;
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<lowp::SparseF8Fmt>(p, tm_w, tm_m, xq, K, workspace, workspace_bytes, "fp8 sparse linear",
+                                     reinterpret_cast<cudaStream_t>(stream));
 }
 
 // torch._grouped_mm(x, W.transpose(-2, -1), offs) on rowwise e4m3 operands: expert e's rows [offs[e-1], offs[e]) of

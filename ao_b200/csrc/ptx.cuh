@@ -127,5 +127,15 @@ __device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
   d |= (uint64_t)1 << 62;                       // layout type [62,64): 1 = SWIZZLE_128B
   return d;
 }
+// The same with 64-byte swizzle (TMA SWIZZLE_64B): row r at byte r*64, 16-byte chunks XOR-ed with ((r/2)%4); 8-row
+// groups 512 B apart.  The tile base is 512-byte aligned; a K step inside the 64-byte row advances the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw64(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);  // start address      [0,14)
+  d |= (uint64_t)1 << 16;                       // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(512 >> 4) << 32;              // stride byte offset  [32,46)
+  d |= (uint64_t)2 << 62;                       // layout type [62,64): 2 = SWIZZLE_64B
+  return d;
+}
 
 }  // namespace ao

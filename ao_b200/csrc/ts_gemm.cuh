@@ -80,16 +80,28 @@ struct WBlockScales<F, std::void_t<decltype(F::W_BLOCK_SCALES)>> {
   static constexpr bool value = F::W_BLOCK_SCALES;
 };
 
+// Fmt::SPARSE_A (optional, default false): a shared-memory A format whose weights are 2:4 sparse (wgmma.sp); the
+// consumer passes its metadata words (Fmt::meta) to Fmt::mma
+template <class F, class = void>
+struct SparseA {
+  static constexpr bool value = false;
+};
+template <class F>
+struct SparseA<F, std::void_t<decltype(F::SPARSE_A)>> {
+  static constexpr bool value = F::SPARSE_A;
+};
+
 template <class Fmt, int N_MMA>
 constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA && !IsGrouped<Fmt>::value ? 2 : 1; }
 constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
 
 // Epilogue arithmetic, per kind (Fmt::EPI; must stay what each format's reference computes, see Params)
-enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2, EPI_BF16_WSCALE = 3, EPI_BF16 = 4 };
+enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2, EPI_BF16_WSCALE = 3, EPI_BF16 = 4, EPI_F8_SPARSE = 5 };
 
 struct Params {
   const __nv_bfloat16* bias;
-  const float* row_scale;   // EPI_FLOAT: optional per-token scale [M]; EPI_I8 / EPI_F8: the activation scale [M]
+  const float* row_scale;   // EPI_FLOAT: optional per-token scale [M]; EPI_I8 / EPI_F8 / EPI_F8_SPARSE: the activation
+                            // scale [M]
   const float* out_scale;   // EPI_FLOAT: optional device scalar, or (out_scale_per_row) one value per output feature;
                             // Grouped<Fmt>: one value per expert [E] (nvfp4: the per-expert weight scale)
   // The grouped fields share storage and padding with the dense ones, so Params keeps its 120 bytes: a larger
@@ -100,7 +112,8 @@ struct Params {
   };
   int out_scale_per_row;
   int grid_forced;          // Grouped<Fmt>: the host grid was forced (ao_b200_debug_set_streamk_ctas): no MIN_UNITS rule
-  const float* w_scale;     // EPI_I8 / EPI_F8 / EPI_BF16_WSCALE: per-output-feature weight scale [N] (EPI_BF16 never
+  const float* w_scale;     // EPI_I8 / EPI_F8 / EPI_F8_SPARSE / EPI_BF16_WSCALE: per-output-feature weight scale [N]
+                            // (EPI_BF16 never
                             // reads it: its format applies the scale per weight, from the aux operand, or, blockwise
                             // e4m3, per 128x128 block [N/128][KT] in its promotion; grouped: [E * N/128][KT])
   __nv_bfloat16* y;         // [M, N_out]
@@ -237,6 +250,9 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 //                                                                  [E * N, K] map of all experts, and their aux tiles
 //   EXPERT_SCALE (grouped EPI_FLOAT only): the epilogue multiplies by out_scale[e] (nvfp4: yes, int4: no scale at all)
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
+//   SPARSE_A: mt = meta(p, aux smem, n_tile, kc, row, lane)        the thread's metadata words of the chunk (row: its
+//                                                                  metadata row of the tile)
+//             static void mma(acc, w smem, x smem, mt[2], wg, scale_d)  the 2 k64 wgmma.sp of a chunk for rows 64wg..
 //   PROMOTE: cs = chunk_scales<N_MMA>(p, aux smem, w_blk, m0, kc, lane)  the chunk's scales (before its wgmmas); w_blk
 //                                                                  is the weight's 128-row block: n_tile, or under the
 //                                                                  grouped schedule (W_BLOCK_SCALES) e * n_tiles +
@@ -582,6 +598,12 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
               __nv_bfloat16 o = __float2bfloat16_rn(__uint_as_float(raw));
               if (p.bias) o = __float2bfloat16_rn(__bfloat162float(o) + bias);
               *dst = o;
+            } else if constexpr (Fmt::EPI == EPI_F8_SPARSE) {
+              // 2:4-sparse e4m3 reference (CUTLASS EVT, rowwise_scaled_linear_sparse_cutlass.cuh): fp32 nodes
+              // ((acc * w_scale[n]) * x_scale[m]) + bias[n] (0 without bias), then one bf16 rounding.  Its build
+              // contracts the last multiply and the add into one FFMA (its SASS has no FADD: DESIGN §2g)
+              const float t = __fmul_rn(__uint_as_float(raw), sw);
+              *dst = __float2bfloat16_rn(__fmaf_rn(t, p.row_scale[m], bias));
             } else {
               *dst = __float2bfloat16_rn(__uint_as_float(raw) * (p.row_scale[m] * sw) + bias);
             }
@@ -624,6 +646,26 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           wgmma_fence_operand(part);
           release(s);
           Fmt::template promote<N_MMA>(acc, part, scale_d, cs);
+          continue;
+        } else if constexpr (SparseA<Fmt>::value) {
+          // the metadata words arrived with the weights.  A wgmma.sp reads its metadata register while it runs, and
+          // ptxas reuses that register once the instruction is issued: each chunk's wgmmas complete before the next
+          // chunk's metadata is loaded (no wgmma in flight across chunks, as CUTLASS's sparse mainloop does)
+          uint32_t mt[2];
+          {
+            const uint2 m2 = Fmt::meta(p, aux_s, tile_of(i) % p.n_tiles, kc_of(i), row_lo + 8 * (lane & 1), lane);
+            mt[0] = m2.x;
+            mt[1] = m2.y;
+          }
+          mbar_wait(&xfull[s], ph);
+          wgmma_fence_operand(acc);
+          wgmma_fence();
+          Fmt::template mma<N_MMA>(acc, w_s, x_s, mt, wg, scale_d);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_operand(acc);
+          wgmma_fence_operand(mt);
+          release(s);
           continue;
         } else if constexpr (Fmt::SS) {
           mbar_wait(&xfull[s], ph);

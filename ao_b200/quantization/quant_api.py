@@ -31,8 +31,8 @@ from ao_b200.quantization.granularity import Granularity, PerGroup, PerRow, PerT
 from ao_b200.quantization.quant_primitives import MappingType
 from ao_b200.quantization.quantize_.common.kernel_preference import KernelPreference
 from ao_b200.quantization.quantize_.workflows import (
-    Float8PackingFormat, Float8Tensor, Int4ChooseQParamsAlgorithm, Int4PackingFormat, Int4TilePackedTo4dTensor,
-    Int8Tensor, QuantizeTensorToFloat8Kwargs, QuantizeTensorToInt8Kwargs)
+    Float8PackingFormat, Float8Sparse2x4_2DData2DMetadataTensor, Float8Tensor, Int4ChooseQParamsAlgorithm,
+    Int4PackingFormat, Int4TilePackedTo4dTensor, Int8Tensor, QuantizeTensorToFloat8Kwargs, QuantizeTensorToInt8Kwargs)
 from ao_b200.quantization.transform_module import _QUANTIZE_CONFIG_HANDLER, register_quantize_module_handler
 
 logger = logging.getLogger(__name__)
@@ -377,12 +377,41 @@ def _fp8_mm_compat(weight: torch.Tensor) -> bool:
     return True
 
 
+def _fp8_sparse_kernel_compat(weight) -> bool:
+    """The 2:4-sparse kernel reads 16-byte rows of compressed codes, K / 2 bytes each: K % 32.  The reference would
+    quantize such a layer and fail at its first forward; here it stays unquantized, with a log line, as the other
+    float8 flows skip incompatible shapes (_fp8_mm_compat)."""
+    if weight.shape[-1] % 32 != 0:
+        logger.info(f"Skipping 2:4-sparse float8 quantization: in_features={weight.shape[-1]} is not a multiple of 32; "
+                    f"weight shape {tuple(weight.shape)} stays {weight.dtype}")
+        return False
+    return True
+
+
 def _float8_dynamic_activation_float8_weight_quantize_tensor(weight, config):
-    if config.packing_format != Float8PackingFormat.PLAIN:
-        raise NotImplementedError(f"float8 packing_format={config.packing_format}: only PLAIN is implemented")
+    if config.packing_format == Float8PackingFormat.SPARSE_1D_DATA_1D_METADATA:
+        raise NotImplementedError("float8 packing_format SPARSE_1D_DATA_1D_METADATA is the reference's hipSPARSELt "
+                                  "(ROCm) format; on sm_90a use SPARSE_2D_DATA_2D_METADATA")
+    if config.packing_format not in (Float8PackingFormat.PLAIN, Float8PackingFormat.SPARSE_2D_DATA_2D_METADATA):
+        raise NotImplementedError(f"float8 packing_format={config.packing_format}: only PLAIN and "
+                                  f"SPARSE_2D_DATA_2D_METADATA are implemented")
     a_gran, w_gran = config.granularity
     if not _fp8_mm_compat(weight):
         return weight
+    if config.packing_format == Float8PackingFormat.SPARSE_2D_DATA_2D_METADATA:
+        # reference quant_api.py:1233-1245 and the tensor's from_hp assertions
+        assert isinstance(w_gran, PerRow), "Sparse packing format only supports per-row quantization"
+        assert config.weight_dtype == torch.float8_e4m3fn, "CUTLASS sparse kernel only supports float8_e4m3fn dtype"
+        if weight.dtype != torch.bfloat16:
+            raise NotImplementedError(f"2:4-sparse float8: bf16 weights only, got {weight.dtype}")
+        if not _fp8_sparse_kernel_compat(weight):
+            return weight
+        act_quant_kwargs = QuantizeTensorToFloat8Kwargs(config.activation_dtype, a_gran,
+                                                        hp_value_lb=config.activation_value_lb,
+                                                        hp_value_ub=config.activation_value_ub,
+                                                        kernel_preference=config.kernel_preference)
+        return Float8Sparse2x4_2DData2DMetadataTensor.from_hp(weight, float8_dtype=config.weight_dtype,
+                                                              granularity=w_gran, act_quant_kwargs=act_quant_kwargs)
     if isinstance(w_gran, PerRow):
         assert weight.dtype == torch.bfloat16, "PerRow quantization only works for bfloat16 precision input weight"
     act_quant_kwargs = QuantizeTensorToFloat8Kwargs(config.activation_dtype, a_gran, hp_value_lb=config.activation_value_lb,

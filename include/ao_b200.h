@@ -248,6 +248,17 @@ int ao_fp8_quantize_1x128_ld(const uint16_t* x, int ldx, int M, int K, uint8_t* 
 int ao_fp8_blockwise_linear(const uint8_t* xq, const float* x_scale_t, int M, int K, const uint8_t* wq,
                             const float* w_scale, int N, const uint16_t* bias, uint16_t* y, void* workspace,
                             size_t workspace_bytes, void* stream);
+/* F.linear(x, Float8Sparse2x4_2DData2DMetadataTensor): 2:4-sparse e4m3 weights with per-row scales and per-token
+ * e4m3 activations, as the reference's CUTLASS sparse GEMM computes it:
+ *   acc[m,n] = sum_k xq[m,k] * W[n,k]   (W the decompressed codes; no per-chunk promotion)
+ *   y[m,n] = bf16(fma(acc[m,n] * w_scale[n], x_scale[m], bias[n]))   (fp32; bias 0 if null)
+ * xq e4m3 [M,K] (16-byte aligned); x_scale f32 [M]; wq e4m3 [N][K/2], the two kept codes of each 4-k group (16-byte
+ * aligned); w_meta uint8, round_up(N,64) x round_up(K,128)/8 bytes in CUTLASS's Sm90 8-bit metadata layout (16-byte
+ * aligned); w_scale f32 [N].  K % 32 == 0, N % 16 == 0.  Metadata of rows >= N or k >= K is never used, and an
+ * all-zero group's nibble (0b0000) is fed as 0b0100.  At M == 0 it returns before reading any pointer. */
+int ao_fp8_sparse_linear(const uint8_t* xq, const float* x_scale, int M, int K, const uint8_t* wq, const uint8_t* w_meta,
+                         const float* w_scale, int N, const uint16_t* bias, uint16_t* y, void* workspace,
+                         size_t workspace_bytes, void* stream);
 /* torch._grouped_mm(x, W.transpose(-2, -1), offs) for a 3-D blockwise Float8Tensor expert weight W [E, N, K]
  * (block_size [1, 128, 128]), 2-D x 3-D form, as the per-expert recipe select + ao_fp8_blockwise_linear computes it:
  * for offs[e-1] <= m < offs[e] (offs[-1] = 0)
