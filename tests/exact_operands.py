@@ -58,15 +58,18 @@ def fp32_exact(t, what):
     assert torch.equal(t.float().double(), t), f"premise: {what} is not exact in fp32"
 
 
-def premise(X, W, bias_acc=None, chunk=False):
+def premise(X, W, bias_acc=None, chunk=False, segment=False):
     """Asserts max(|X| @ |W|^T) + |bias| < 2^24 u (u = the quantum of every product); returns u.  chunk: the e4m3
     wgmma chain of one 128-k chunk adds in the tensor core's reduced-precision accumulator (DESIGN.md §1), so each
     chunk's sum is also kept under 2^13 u, an assumed width under which that adder is exact.  Above ANALYTIC_ABOVE
-    elements of M x N x KT the chunk sums are bounded by 128 max|X| max|W| instead of materialised."""
+    elements of M x N x KT the chunk sums are bounded by 128 max|X| max|W| instead of materialised.  segment: the
+    kernel never promotes (2:4-sparse e4m3), so a whole segment's K sum stays in that accumulator: the whole sum is
+    kept under 2^13 u."""
     u = lowbit(X) * lowbit(W)
     extra = float(bias_acc.abs().max()) if bias_acc is not None else 0.0
     top = float((X.abs() @ W.abs().t()).max()) + extra
     assert top < 2.0**24 * u, f"premise: sums reach {top / u:.0f} u >= 2^24 u"
+    assert not segment or top < 2.0**13 * u, f"premise: a segment's sum reaches {top / u:.0f} u >= 2^13 u"
     if chunk and X.shape[0] * W.shape[0] * -(-X.shape[1] // 128) > ANALYTIC_ABOVE:
         top_c = 128 * float(X.abs().max()) * float(W.abs().max())
         assert top_c < 2.0**13 * u, f"premise: a 128-k chunk may reach {top_c / u:.0f} u >= 2^13 u"
@@ -174,13 +177,82 @@ def int4_weights(n, K, group_size, g):
     return W, qdata, sz
 
 
+def transposed_scales(s):
+    """1x128 token scales [M, K/128] -> the kernel's [K/128, round_up(M, 4)] layout (ao_fp8_quantize_1x128), pads 0."""
+    M, KB = s.shape
+    out = torch.zeros(KB, (M + 3) // 4 * 4, dtype=torch.float32, device=s.device)
+    out[:, :M] = s.t()
+    return out
+
+
+def blockwise_values(codes, scales, rows):
+    """fp64 codes [R, K] times their block scales [R / rows, K/128] (rows = 1: 1x128 token scales, 128: 128x128
+    weight blocks).  Every scale is a power of two, so the reference loop's sum over chunks of dot(x_kb, w_kb) a_s w_s
+    is X @ W^T of these values, exactly."""
+    return codes * scales.double().repeat_interleave(rows, 0).repeat_interleave(128, 1)
+
+
+def blockwise_epilogue(acc, bias):
+    """EPI_BF16 on exact sums acc (fp64 [M, n]): bf16(acc), then the bf16 add of the bias."""
+    fp32_exact(acc, "fp8_blockwise: the sums")
+    y = acc.float().to(torch.bfloat16)
+    return y if bias is None else y + bias
+
+
+def sparse_codes(n, K, r, g):
+    """n rows of 2:4-pruned nonzero integer codes -r..r (fp64 [n, K]): two random positions of each 4-k group kept,
+    except that one group in sixteen is left empty and one in sixteen, for each position p, holds a single code at p."""
+    keep = torch.rand(n, K // 4, 4, device=DEV, generator=g).argsort(-1)[..., :2]
+    mask = torch.zeros(n, K // 4, 4, dtype=torch.bool, device=DEV).scatter_(-1, keep, True)
+    kind = randint(0, 15, (n, K // 4), g)
+    mask[kind == 0] = False
+    for p in range(4):
+        mask[kind == 1 + p] = torch.arange(4, device=DEV) == p
+    codes = randint(1, r, (n, K), g) * (randint(0, 1, (n, K), g) * 2 - 1)
+    return codes.double() * mask.reshape(n, K)
+
+
+def sparse_activations(M, K, r, nnz, g):
+    """codes -r..r [M, K] (fp64) with at most nnz nonzeros per row (None: no cap) at random positions, so that every
+    position of every 4-k group still meets nonzero activations"""
+    X = randint(-r, r, (M, K), g).double()
+    if nnz is not None and nnz < K:
+        X.scatter_(1, torch.rand(M, K, device=DEV, generator=g).argsort(-1)[:, nnz:], 0.0)
+    return X
+
+
+def sparse_scales(n, g):
+    """per-row scales 2^[-3, 1] ODD / 8: mantissa bits, so the epilogue's rounding order shows"""
+    return (pow2(randint(-3, 1, (n,), g)) * pick(ODD, (n,), g) / 8).float()
+
+
+def sparse_compress(wq):
+    """The package's 2:4 compressor on the e4m3 codes wq [N, K]; asserts that decompressing gives every code back."""
+    from ao_b200.quantization.quantize_.workflows.float8.float8_sparse_2x4_2d_data_2d_metadata_tensor import (
+        compress_2x4_e4m3, decompress_2x4_e4m3)
+
+    qd, meta = compress_2x4_e4m3(wq)
+    assert torch.equal(decompress_2x4_e4m3(qd, meta).float(), wq.float()), "premise: the compressor keeps every code"
+    return qd, meta
+
+
+def sparse_epilogue(acc, x_s, w_s, bias):
+    """EPI_F8_SPARSE on exact sums acc (fp64 [M, n]): t = fp32(acc * w_s[n]), then fp32(t * x_s[m] + bias[n]) rounded
+    once (an FFMA); fp64 of that fp32 value."""
+    fp32_exact(acc, "fp8_sparse: the sums")
+    t = (acc.float() * w_s[None, :]).double() * x_s[:, None].double()   # exact in fp64
+    if bias is not None:
+        t = t + bias.double()[None, :]
+    return t.float().double()
+
+
 def build(op, M, N, K, seed=0, n_out=None, w_bytes=None, group_size=64):
     """op: int4 | int8_dyn | int8_mm_i32 | fp8 | mxfp8 | nvfp4 | nvfp4w | nvfp4w_xs | nvfp4w_rowpts | int8wo | fp8wo |
-    mxfp4.
+    mxfp4 | fp8_blockwise | fp8_sparse.
     n_out: int4 output features (<= N).  w_bytes: nvfp4 weight scale bytes [N, K/16] (default: a window of normal
     bytes with mantissa bits set).  group_size: int4 (32, 64, 128 or 256).  The value windows are fixed and the
     premise is checked on the drawn values: for the test shapes (K <= 16384, M x N small); served() picks the windows
-    from K instead."""
+    from K instead (fp8_blockwise and fp8_sparse take that window here too)."""
     o = ops()
     g = gen(seed * 7919 + M * 31 + N * 7 + K)
     if op == "int4":
@@ -342,6 +414,39 @@ def build(op, M, N, K, seed=0, n_out=None, w_bytes=None, group_size=64):
                 cache[m] = to_blocked(xs8[:m])
             return o.mxfp4_linear(xq[:m], cache[m], wq, wsb, b)
         return Case(op, "mxfp4", M, N, K, N, None, run, ref=recipe(op, X @ W.t(), bias=b))
+    if op == "fp8_blockwise":
+        # integer codes, power-of-two 1x128 / 128x128 scales: each chunk's code sum under 2^13, the whole scaled sum
+        # under 2^24 of the smallest quantum; the epilogue rounds as the reference does (blockwise_epilogue)
+        win = window(op, K)
+        Xc = randint(-win["xr"], win["xr"], (M, K), g).double()
+        Wc = randint(-win["wr"], win["wr"], (N, K), g).double()
+        a_s = pow2(randint(-2, -2 + win["da"], (M, K // 128), g)).float()
+        w_s = pow2(randint(-1, -1 + win["dw"], (N // 128, K // 128), g)).float()
+        X, W = blockwise_values(Xc, a_s, 1), blockwise_values(Wc, w_s, 128)
+        premise(Xc, Wc, chunk=True)
+        premise(X, W)
+        b = (torch.randn(N, device=DEV, generator=g) * 4.0).to(torch.bfloat16)
+        xq, wq = Xc.to(torch.float8_e4m3fn), Wc.to(torch.float8_e4m3fn)
+        cache = {}
+
+        def run(m):
+            if m not in cache:   # the layout depends on round_up(m, 4): one tensor per token count
+                cache[m] = transposed_scales(a_s[:m])
+            return o.fp8_blockwise_linear(xq[:m], cache[m], wq, w_s, b)
+        return Case(op, "fp8_blockwise", M, N, K, N, None, run, ref=blockwise_epilogue(X @ W.t(), b))
+    if op == "fp8_sparse":
+        # no promotion: the whole K sum stays under 2^13 (the activation rows' nonzeros capped where K needs it)
+        win = window(op, K)
+        X = sparse_activations(M, K, win["xr"], win["nnz"], g)
+        W = sparse_codes(N, K, win["wr"], g)
+        premise(X, W, segment=True)
+        x_s, w_s = sparse_scales(M, g), sparse_scales(N, g)
+        b = (torch.randn(N, device=DEV, generator=g) * 4.0).to(torch.bfloat16)
+        xq = X.to(torch.float8_e4m3fn)
+        qd, meta = sparse_compress(W.to(torch.float8_e4m3fn))
+        ref = sparse_epilogue(X @ W.t(), x_s, w_s, b).float().to(torch.bfloat16)
+        return Case(op, "fp8_sparse", M, N, K, N, None,
+                    lambda m: o.fp8_sparse_linear(xq[:m], x_s[:m], qd, meta, w_s, b), ref=ref)
     raise ValueError(op)
 
 
@@ -431,6 +536,11 @@ def served_candidates(op):
         return [dict(xr=a, wr=b) for a, b in ((8, 7), (4, 7), (2, 3), (1, 1))]
     if op == "mxfp4":
         return [dict(xc=list(range(16)), d=1), dict(xc=list(range(16)), d=0), dict(xc=E2M1_UPTO1, d=0)]
+    if op == "fp8_blockwise":   # token scales 2^[-2, -2 + da], weight block scales 2^[-1, -1 + dw]
+        return [dict(xr=r, wr=r, da=3, dw=2) for r in (7, 4, 2, 1)]
+    if op == "fp8_sparse":      # nnz: nonzero activations per row at most (None: every k)
+        return [dict(xr=2, wr=2, nnz=None), dict(xr=2, wr=1, nnz=None), dict(xr=1, wr=1, nnz=None),
+                dict(xr=1, wr=1, nnz=2**13 - 1)]
     raise ValueError(op)
 
 
@@ -461,6 +571,11 @@ def factors(op, win):
     if op == "mxfp4":
         pw = span([2.0**j for j in range(win["d"] + 1)])
         return [span([E2M1[c] for c in win["xc"]]), pw], [span(E2M1), pw], []
+    if op == "fp8_blockwise":   # the codes first: bound() takes the chunk's code sum from them
+        return ([span(_codes(win["xr"])), span([2.0**e for e in range(-2, -1 + win["da"])])],
+                [span(_codes(win["wr"])), span([2.0**e for e in range(-1, win["dw"])])], [])
+    if op == "fp8_sparse":
+        return [span(_codes(win["xr"]))], [span(_codes(win["wr"]))], []
     raise ValueError(op)
 
 
@@ -469,6 +584,11 @@ def bound(op, K, win):
     and 128 max|X| max|W| for the e4m3 chunk.  Exact when the first is < 2^24 and the second < 2^13."""
     xf, wf, ef = factors(op, win)
     xw = units(xf) * units(wf)
+    if op == "fp8_blockwise":   # the chunk's wgmma adds codes; the epilogue rounds as the reference does
+        return K * xw, 128 * units(xf[:1]) * units(wf[:1])
+    if op == "fp8_sparse":      # one accumulator chain over the whole K; a 4-k group holds at most two weights
+        c = min(win["nnz"] or K, K // 2) * xw
+        return c, c
     if op in ("int8_dyn", "int8_mm_i32", "int8wo", "fp8wo", "mxfp4"):
         return K * xw, None   # the sum is exact in fp32; the epilogue rounds as the reference does (recipe())
     return K * xw * units(ef) + BIAS_UNITS, (128 * xw if op == "fp8" else None)
@@ -494,7 +614,7 @@ def _quantum(fs):
     return q
 
 
-def _reference(op, X, n, wblock, epi, chunk):
+def _reference(op, X, n, wblock, epi, chunk, segment=False):
     """The bf16 (int32) reference [M, n], W_BLOCK features at a time: wblock(n0, n1) -> fp64 W rows; epi(acc, n0, n1)
     -> fp64 output.  The premise is checked on the drawn values of each block as well."""
     M = X.shape[0]
@@ -502,7 +622,7 @@ def _reference(op, X, n, wblock, epi, chunk):
     for n0 in range(0, n, W_BLOCK):
         n1 = min(n, n0 + W_BLOCK)
         W = wblock(n0, n1)
-        premise(X, W, chunk=chunk)
+        premise(X, W, chunk=chunk, segment=segment)
         y = epi(X @ W.t(), n0, n1)
         del W
         if op == "int8_mm_i32":
@@ -720,4 +840,44 @@ def served(op, M, N, K, seed=0, group_size=32, n_out=None, x_seed=None):
                 cache[m] = to_blocked(xs8[:m])
             return o.mxfp4_linear(xq[:m], cache[m], wq, wsb, b)
         return Case(op, "mxfp4", M, N, K, N, None, run, ref=ref)
+    if op == "fp8_blockwise":
+        KB = K // 128
+        Xc = randint(-win["xr"], win["xr"], (M, K), gx).double()
+        a_s = pow2(randint(-2, -2 + win["da"], (M, KB), gx)).float()
+        b = (torch.randn(N, device=DEV, generator=gx) * 4.0).to(torch.bfloat16)
+        X = blockwise_values(Xc, a_s, 1)
+
+        def make(nb):
+            Wc = randint(-win["wr"], win["wr"], (nb, K), gw).double()
+            w_s = pow2(randint(-1, -1 + win["dw"], (nb // 128, KB), gw)).float()
+            return blockwise_values(Wc, w_s, 128), (Wc.to(torch.float8_e4m3fn), w_s)
+        # the chunk's code sums are bounded by the window (window()); the block premise checks the scaled sums
+        ref = _reference(op, X, N, blocks(N, make), lambda acc, n0, n1: blockwise_epilogue(acc, b[n0:n1]).double(),
+                         False)
+        xq, wq = Xc.to(torch.float8_e4m3fn), torch.cat([p[0] for p in parts], 0)
+        w_s = torch.cat([p[1] for p in parts], 0)
+        cache = {}
+
+        def run(m):
+            if m not in cache:
+                cache[m] = transposed_scales(a_s[:m])
+            return o.fp8_blockwise_linear(xq[:m], cache[m], wq, w_s, b)
+        return Case(op, "fp8_blockwise", M, N, K, N, None, run, ref=ref)
+    if op == "fp8_sparse":
+        X = sparse_activations(M, K, win["xr"], win["nnz"], gx)
+        x_s, w_s = sparse_scales(M, gx), sparse_scales(N, gw)
+        b = (torch.randn(N, device=DEV, generator=gx) * 4.0).to(torch.bfloat16)
+
+        def make(nb):
+            W = sparse_codes(nb, K, win["wr"], gw)
+            return W, W.to(torch.float8_e4m3fn)
+        ref = _reference(op, X, N, blocks(N, make), lambda acc, n0, n1: sparse_epilogue(acc, x_s, w_s[n0:n1], b[n0:n1]),
+                         False, segment=True)
+        xq = X.to(torch.float8_e4m3fn)
+        qd, meta = sparse_compress(torch.cat(parts, 0))   # the metadata's atoms interleave row blocks: compress once
+        parts.clear()
+        c = Case(op, "fp8_sparse", M, N, K, N, None, lambda m: o.fp8_sparse_linear(xq[:m], x_s[:m], qd, meta, w_s, b),
+                 ref=ref)
+        c.inputs = [xq, x_s, b]
+        return c
     raise ValueError(op)

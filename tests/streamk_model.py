@@ -16,10 +16,12 @@ KIND_NAMES = {FULL: "FULL", CONTRIB: "CONTRIB", OWNER: "OWNER"}
 # token-tile widths each format's launcher can pick (fp8 keeps a second accumulator per chunk: 64 at most)
 WIDTHS = {"int4": (16, 32, 64, 128), "int8": (16, 32, 64, 128), "fp8": (16, 32, 64), "mxfp8": (16, 32, 64, 128),
           "nvfp4": (16, 32, 64, 128), "mxfp4": (16, 32, 64, 128), "int8wo": (16, 32, 64, 128),
-          "fp8wo": (16, 32, 64, 128)}
+          "fp8wo": (16, 32, 64, 128), "fp8_sparse": (16, 32, 64, 128), "fp8_blockwise": (16, 32, 64)}
 
 # Each format policy's stage layout, from its Fmt struct: (W_BYTES, AUX_BYTES, X_ELEM_BYTES, DECODE_2CTA, PROMOTE,
-# MAX_N_MMA).  int8 is SsFmt<KIND_I8>, fp8 SsFmt<KIND_F8> (e4m3 x e4m3), int8wo Int8WoFmt, fp8wo Fp8WoFmt.
+# MAX_N_MMA).  int8 is SsFmt<KIND_I8>, fp8 SsFmt<KIND_F8> (e4m3 x e4m3), int8wo Int8WoFmt, fp8wo Fp8WoFmt,
+# fp8_sparse SparseF8Fmt (8 KiB of compressed codes, two 1 KiB metadata atoms) and fp8_blockwise BlockwiseF8Fmt (256
+# bytes of token scales; the 272 of BlockwiseF8GroupedFmt round up to the same 1 KiB aux slot).
 POLICIES = {
     "int4": (8192, 2048, 2, True, False, 128),
     "int8": (16384, 0, 1, True, False, 128),
@@ -29,6 +31,8 @@ POLICIES = {
     "nvfp4": (8192, 1024, 2, False, False, 128),
     "int8wo": (16384, 0, 2, True, False, 128),
     "fp8wo": (16384, 512, 2, False, False, 128),
+    "fp8_sparse": (8192, 2048, 1, True, False, 128),
+    "fp8_blockwise": (16384, 256, 1, False, True, 64),
 }
 SMEM_PER_SM, RESERVED_PER_CTA, MAX_STAGES = 228 * 1024, 1024, 12
 

@@ -19,10 +19,10 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 OPS = ("int4", "int8_dyn", "int8_mm_i32", "fp8", "mxfp8", "nvfp4", "nvfp4w", "nvfp4w_xs", "nvfp4w_rowpts", "int8wo",
-       "fp8wo", "mxfp4")
+       "fp8wo", "mxfp4", "fp8_blockwise", "fp8_sparse")
 OP_FORMAT = {"int4": "int4", "int8_dyn": "int8", "int8_mm_i32": "int8", "fp8": "fp8", "mxfp8": "mxfp8", "nvfp4": "nvfp4",
              "nvfp4w": "nvfp4", "nvfp4w_xs": "nvfp4", "nvfp4w_rowpts": "nvfp4", "int8wo": "int8wo", "fp8wo": "fp8wo",
-             "mxfp4": "mxfp4"}
+             "mxfp4": "mxfp4", "fp8_blockwise": "fp8_blockwise", "fp8_sparse": "fp8_sparse"}
 
 # (M, N, K, forced grids; None = every grid from 1 to min(units, SMs))
 #   * N = 256, K = 4096: every token-tile width and two m-blocks, all grids
@@ -45,6 +45,10 @@ def shape_supported(op, M, N, K):
         return K % 16 == 0
     if fmt == "fp8":
         return K % 16 == 0 and N % 16 == 0
+    if fmt == "fp8_blockwise":
+        return K % 128 == 0 and N % 128 == 0
+    if fmt == "fp8_sparse":
+        return K % 32 == 0 and N % 16 == 0
     return K % 16 == 0 and N % 8 == 0
 
 
@@ -129,25 +133,29 @@ TAILS = ([("int4", 7, n, 2048, n_out) for n, n_out in ((8, 8), (128, 120), (136,
          + [(op, M, 256, k, None) for op in ("int8_dyn", "int8_mm_i32", "fp8") for k in (16, 144, 1040) for M in (9, 70)]
          + [(op, M, n, 1024, None) for op in ("int8wo", "fp8wo", "mxfp4") for n in (77, 200) for M in (5, 40)]
          + [(op, M, 256, k, None) for op in ("int8wo", "fp8wo") for k in (16, 144, 1040) for M in (9, 70)]
-         + [("mxfp4", M, 256, k, None) for k in (32, 160, 1056) for M in (9, 70)])
+         + [("mxfp4", M, 256, k, None) for k in (32, 160, 1056) for M in (9, 70)]
+         + [("fp8_sparse", M, n, 1024, None) for n in (48, 80, 208) for M in (5, 40)]
+         + [("fp8_sparse", M, 256, k, None) for k in (32, 160, 1056, 4128) for M in (9, 70)])
 
 
 @pytest.mark.parametrize("op,M,N,K,n_out", TAILS)
 def test_feature_and_k_tails_bit_exact(ops, set_ctas, op, M, N, K, n_out):
     """Output-feature tails (a partial 128-row tile, int4 n_out < N) and K tails (TMA zero fill of the last chunk);
-    the mxfp8 K tails are in test_parity_holes_gpu.py::test_k_tail_is_zero_filled."""
+    the mxfp8 K tails are in test_parity_holes_gpu.py::test_k_tail_is_zero_filled.  2:4-sparse e4m3: the metadata
+    rows past N (up to the next 64) and the metadata words of a K-tail chunk past K are sanitized, not used.
+    Blockwise e4m3 has no tails: its K and N are multiples of 128."""
     case = ex.build(op, M, N, K, seed=2, n_out=n_out)
     U = sk.plan(case.fmt, M, case.n_plan, K, grid=1).U
     _sweep(ops, set_ctas, case, sorted({None, 1, min(U, ex.sm_count())}, key=lambda g: g or 0))
 
 
 def test_mixed_formats_and_grids_in_one_cuda_graph(ops, set_ctas):
-    """int4, nvfp4, int8, fp8, mxfp8, the weight-only int8 and fp8, mxfp4 and int4 again back to back in one CUDA
-    graph, PDL on, each under its own forced grid; a large grid followed by a small one would expose a flag the owners
-    did not re-arm.  Two replays."""
+    """int4, nvfp4, int8, fp8, mxfp8, the weight-only int8 and fp8, mxfp4, blockwise fp8, 2:4-sparse fp8 and int4
+    again back to back in one CUDA graph, PDL on, each under its own forced grid; a large grid followed by a small one
+    would expose a flag the owners did not re-arm.  Two replays."""
     M, N, K = 20, 384, 4096
     plan = [("int4", 96), ("nvfp4", 5), ("int8_dyn", 80), ("fp8", 3), ("mxfp8", 64), ("int8wo", 90), ("fp8wo", 4),
-            ("mxfp4", 70), ("int4", 7)]
+            ("mxfp4", 70), ("fp8_blockwise", 6), ("fp8_sparse", 90), ("int4", 7)]
     cases = [ex.build(op, M, N, K, seed=3 + i) for i, (op, _) in enumerate(plan)]
     st = torch.cuda.Stream()
     st.wait_stream(torch.cuda.current_stream())

@@ -151,12 +151,12 @@ class Exact:
         y = self.run(ops, m)
         bad = bits(y) != bits(self.ref[:m])
         assert not bool(bad.any()), f"M={m} N={self.N} K={self.K} {what}: {int(bad.sum())} wrong, first at {bad.nonzero()[0].tolist()}"
+        assert not bool(ops.debug_workspace(y).view(torch.int32)[:4096].ne(0).any()), f"M={m} {what}: flags left raised"
         bits(y).fill_(POISON_BF16)
 
 
 def grids(M, N, K):
-    # the rowwise e4m3 kernel's tiles: token widths 16, 32, 64 and 128-k chunks
-    U = sk.plan("fp8", M, N, K, grid=1).U
+    U = sk.plan("fp8_blockwise", M, N, K, grid=1).U
     return list(range(1, min(U, 132) + 1))
 
 

@@ -12,6 +12,7 @@ import pytest
 import torch
 import torch.nn as nn
 
+import streamk_model as sk
 from test_decode_residency import RESERVED_PER_CTA, SMEM_PER_SM, resource_usage
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -264,14 +265,8 @@ def test_c_abi_rejections():
 
 
 # ---------------------------------------------------------------- the budget of the format
-def _ring_smem(n_mma):
-    """Cfg<BlockwiseF8Fmt, N>: a stage is the 16 KiB weight tile, the 1 KiB aux slot (256 bytes of token scales) and
-    N x 128 activation bytes; one CTA per SM (PROMOTE), a 200 KB ring of at most 12 stages."""
-    stage = 16384 + 1024 + n_mma * 128
-    stages = min(12, 200 * 1024 // stage)
-    return stages, stages * stage + 3 * stages * 8 + 1024
-
-
+# Cfg<BlockwiseF8Fmt, N> is streamk_model.ring("fp8_blockwise", N): a stage is the 16 KiB weight tile, the 1 KiB aux
+# slot (256 bytes of token scales) and N x 128 activation bytes; one CTA per SM (PROMOTE), a 200 KB ring
 @pytest.mark.parametrize("n_mma", [16, 32, 64])
 def test_tiles_registers_stack_and_shared_memory(n_mma):
     src = open(os.path.join(ROOT, "ao_b200", "csrc", "lowp_linear.cu")).read()
@@ -283,5 +278,7 @@ def test_tiles_registers_stack_and_shared_memory(n_mma):
     assert ("BlockwiseF8Fmt", 128) not in usage   # MAX_N_MMA = 64, as SsFmt<KIND_F8>
     reg, stack = usage[("BlockwiseF8Fmt", n_mma)]
     assert reg <= 168 and stack == 0, (reg, stack)
-    stages, smem = _ring_smem(n_mma)
+    stage, ctas, stages, staging = sk.ring("fp8_blockwise", n_mma)
+    assert stage == 16384 + 1024 + n_mma * 128 and ctas == 1 and not staging
+    smem = sk.ring_smem("fp8_blockwise", n_mma)
     assert stages >= 2 and smem + RESERVED_PER_CTA <= SMEM_PER_SM

@@ -156,11 +156,12 @@ class Exact:
         y = self.run(ops, m, meta)
         bad = bits(y) != bits(self.ref[:m])
         assert not bool(bad.any()), f"M={m} N={self.N} K={self.K} {what}: {int(bad.sum())} wrong, first at {bad.nonzero()[0].tolist()}"
+        assert not bool(ops.debug_workspace(y).view(torch.int32)[:4096].ne(0).any()), f"M={m} {what}: flags left raised"
         bits(y).fill_(POISON_BF16)
 
 
 def grids(M, N, K):
-    U = sk.plan("fp8", M, N, K, grid=1).U
+    U = sk.plan("fp8_sparse", M, N, K, grid=1).U
     return list(range(1, min(U, 132) + 1))
 
 

@@ -13,6 +13,7 @@ import pytest
 import torch
 import torch.nn as nn
 
+import streamk_model as sk
 from test_decode_residency import RESERVED_PER_CTA, SMEM_PER_SM, resource_usage
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -242,15 +243,8 @@ def test_c_abi_rejections():
 
 
 # ---------------------------------------------------------------- the budget of the format
-def _ring_smem(n_mma, ctas):
-    """Cfg<SparseF8Fmt, N>: a stage is 8 KiB of compressed codes, the 2 KiB metadata slot and N x 128 activation bytes;
-    two CTAs per SM at decode tiles (DECODE_2CTA), else a 200 KB ring; at most 12 stages"""
-    stage = 8192 + 2048 + n_mma * 128
-    fit = 200 * 1024 // stage if ctas == 1 else (SMEM_PER_SM // 2 - RESERVED_PER_CTA - 1024) // (stage + 24)
-    stages = min(12, fit)
-    return stages, stages * stage + 3 * stages * 8 + 1024
-
-
+# Cfg<SparseF8Fmt, N> is streamk_model.ring("fp8_sparse", N): a stage is 8 KiB of compressed codes, the 2 KiB metadata
+# slot and N x 128 activation bytes; two CTAs per SM at decode tiles (DECODE_2CTA), else a 200 KB ring
 @pytest.mark.parametrize("n_mma", [16, 32, 64, 128])
 def test_tiles_registers_stack_and_shared_memory(n_mma):
     src = open(os.path.join(ROOT, "ao_b200", "csrc", "lowp_linear.cu")).read()
@@ -260,8 +254,9 @@ def test_tiles_registers_stack_and_shared_memory(n_mma):
     usage = resource_usage()
     assert ("SparseF8Fmt", n_mma) in usage, f"ts_gemm_kernel<SparseF8Fmt, {n_mma}> not built"
     reg, stack = usage[("SparseF8Fmt", n_mma)]
-    ctas = 2 if n_mma <= 32 else 1
+    stage, ctas, stages, _ = sk.ring("fp8_sparse", n_mma)
+    assert stage == 8192 + 2048 + n_mma * 128 and ctas == (2 if n_mma <= 32 else 1)
     # two CTAs per SM: 80 registers per thread at launch (the consumers grow to 104 with setmaxnreg)
     assert stack == 0 and reg <= (80 if ctas == 2 else 168), (reg, stack)
-    stages, smem = _ring_smem(n_mma, ctas)
+    smem = sk.ring_smem("fp8_sparse", n_mma)
     assert stages >= 2 and ctas * (smem + RESERVED_PER_CTA) <= SMEM_PER_SM

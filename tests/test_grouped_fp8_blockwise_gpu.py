@@ -13,8 +13,8 @@ Float8Tensor handler) on the GPU:
 
 Exact operands: the scheme of test_fp8_blockwise_gpu.py::Exact per expert.  Codes in -2..2, token scales 2^[-2, 1] and
 weight block scales 2^[-1, 1] divided by 2^(e % 3), so a wrong expert's scale block cannot pass: each chunk's wgmma sum
-is an integer below 2^9, its scaled value a multiple of 2^-5 below 2^11, and K <= 2048 keeps the sum below 2^24
-quanta, exact in fp32 in any order and under any stream-K split.
+is an integer below 2^9, its scaled value a multiple of 2^-5 below 2^11 (2^16 quanta), and K <= 16384 (128 chunks)
+keeps the sum below 2^24 quanta, exact in fp32 in any order and under any stream-K split (fp32_exact asserts it).
 """
 import copy
 import ctypes
@@ -46,6 +46,11 @@ GROUPED_CASES = [
     ([1, 0, 2, 1, 0, 0, 3, 1] * 8, 128, 256, 5, None),            # E = 64
     ([0] * 30 + [16] + [0] * 33, 256, 2048, 0, (1, 2, 5, 16, 64)),  # E = 64, one expert with every row
     ([1, 0, 2, 0, 0, 3, 1, 1] * 32, 256, 512, 3, (1, 2, 7, 50, 131, 132)),   # E = 256
+    # K = 16384, one tile split over up to 128 CTAs: owners gather 32 to 127 partials (N_MMA 16, 32 and 64; at 32
+    # also 4 and 5, and 25 valid token columns of the 32)
+    ([0, 16, 0], 128, 16384, 0, (33, 64, 65, 127, 128)),
+    ([0, 25, 0], 128, 16384, 0, (5, 6, 33, 64, 65, 127, 128)),
+    ([0, 64, 0], 128, 16384, 0, (33, 64, 65, 127, 128)),
 ]
 # offs values that are not cumulative row ends: the kernel clamps each into [end[e-1], M]
 MALFORMED = [([9, 4, -3, 30, 12, 500], 40), ([-5, -1, 0, 3], 8), ([100, 200], 64)]
@@ -61,7 +66,7 @@ def gm_offs(rows):
 
 def grids_of(case_rows, N, K, tail, grids, sm):
     M = sum(case_rows) + tail
-    p = gm.plan(gm_offs(case_rows), M, N, K, grid=1, sm=sm)   # the rowwise e4m3 tiles: 16, 32, 64 tokens
+    p = gm.plan(gm_offs(case_rows), M, N, K, grid=1, sm=sm, fmt="fp8_blockwise")
     top = min(p.U_bound, sm)
     return list(range(1, top + 1)) if grids is None else [G for G in grids if G <= top]
 
@@ -137,7 +142,7 @@ def _sweep(ops, set_ctas, case, grids, what):
     wrong = [(G, b, r) for G, b, r in zip(grids, bad, raised) if b or r]
     if wrong:
         G, nb, nr = wrong[0]
-        p = gm.plan(case.offs.tolist(), case.M, case.N, case.K, grid=G, sm=ex.sm_count())
+        p = gm.plan(case.offs.tolist(), case.M, case.N, case.K, grid=G, sm=ex.sm_count(), fmt="fp8_blockwise")
         pytest.fail(f"{what} M={case.M} N={case.N} K={case.K} E={case.E} grid={G or 'default'}: {nb} wrong elements, "
                     f"{nr} flags left raised (U={p.U}, device grid {p.G} of {p.G_host}); "
                     f"{len(wrong)} of {len(grids)} launches wrong")

@@ -29,6 +29,11 @@ GROUPED_CASES = [
     ([20, 30], 640, 1024, 0, (3, 6, 7, 11)),                      # five n-tiles: CONTRIB, FULL and OWNER in one CTA
     ([1, 0, 2, 1, 0, 0, 3, 1] * 8, 128, 256, 5, None),            # E = 64
     ([0] * 30 + [16] + [0] * 33, 256, 2048, 0, (1, 2, 5, 16, 64)),  # E = 64, one expert with every row
+    # K = 16384, one tile split over up to 128 CTAs: owners gather 32 to 127 partials (N_MMA 16, 32 and 64; at 32
+    # also 4 and 5, and 25 valid token columns of the 32)
+    ([0, 16, 0], 128, 16384, 0, (33, 64, 65, 127, 128)),
+    ([0, 25, 0], 128, 16384, 0, (5, 6, 33, 64, 65, 127, 128)),
+    ([0, 64, 0], 128, 16384, 0, (33, 64, 65, 127, 128)),
 ]
 # offs values that are not cumulative row ends: the kernel clamps each into [end[e-1], M]
 MALFORMED = [([9, 4, -3, 30, 12, 500], 40), ([-5, -1, 0, 3], 8), ([100, 200], 64)]

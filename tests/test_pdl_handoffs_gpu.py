@@ -8,7 +8,8 @@ launches rarely do.  So every chain here starts behind a STALL HEAD: fp8_quantiz
 [8, 2^25] tensor, one CTA per row on 8 SMs, milliseconds long, which triggers its dependents at entry.  Behind it
 every kernel of the chain becomes resident, triggers and parks in griddepcontrol.wait, so each consumer's pre-wait
 reads happen before its producers have written anything, as far as the chain fits on the SMs the head leaves free
-(test_stall_head_opens_the_window checks under torch.profiler that the consumers start before the head ends).
+(test_stall_head_opens_the_window checks under torch.profiler, on a CUDA graph replay, that the consumers start before
+the head ends).
 
 The kernels are deterministic (stream-K adds partials in a fixed order), so the oracle is the same launches on the same
 inputs with torch.cuda.synchronize() between them.  Every buffer a chain writes is filled with 0xFF bytes (NaN in bf16,
@@ -494,11 +495,22 @@ def test_stall_head_opens_the_window(lib, head, name):
     """Premise of the module: behind the head, every kernel of these chains starts before the head ends, so its
     pre-wait reads happen while its producers are still parked.  The weight chains run here WITHOUT their fence, to
     show the window the fence closes: the linear is running, and requesting its weights, before the weight quantizer
-    ahead of it has written anything.  (Their outputs are not looked at.)"""
+    ahead of it has written anything.  (Their outputs are not looked at.)
+    Measured on a replay of the head and the chain captured in one CUDA graph: the graph hands every launch to the
+    device at once, so whether a kernel starts inside the window depends on PDL alone.  Launched eagerly, a kernel
+    the host enqueues after the head has ended (a host thread descheduled for the head's ~16 ms on a loaded machine)
+    would start late without anything on the device being wrong."""
     c = dict(CHAINS)[name](lib)
     c.poison()
     steps = [s for s in c.steps if s[0] != FENCE]
-    spans = _kernel_spans(lambda: c.run(head=head, steps=steps))
+    st = torch.cuda.Stream()
+    st.wait_stream(torch.cuda.current_stream())
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph, stream=st):
+        c.run(head=head, steps=steps)
+    graph.replay()   # the first replay uploads the graph
+    torch.cuda.synchronize()
+    spans = _kernel_spans(graph.replay)
     assert spans and "rowwise_cta_kernel" in spans[0][0], spans[:3]
     head_end = spans[0][2]
     assert len(spans) >= 1 + len(steps), [s[0] for s in spans]   # the head, then at least one kernel per call

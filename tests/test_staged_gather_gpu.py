@@ -9,13 +9,14 @@ after staging), over owner tiles whose valid token columns fill the width and fa
 
 * dense: one 128-row tile at K = 8192 (64 chunks) over G = c + 1 CTAs, at M = the width, the width - 1 and (width 16)
   M = 1, through tests/exact_operands.py and the shared sweep of test_exact_gemm_gpu.py.  int8 weight-only at width 64
-  copies a partial that fills its stage exactly.  fp8 (e4m3 x e4m3) does not stage: it runs the register path at
-  the same counts, as a control.
-* grouped (int4, nvfp4, fp8 weight-only): experts of width - 1 and 1 rows, and one of width rows, so the copy length
+  copies a partial that fills its stage exactly; 2:4-sparse e4m3 stages at width 16 only, two CTAs per SM.  fp8 and
+  blockwise fp8 (e4m3 x e4m3, PROMOTE) do not stage: they run the register path at the same counts, as controls.
+* grouped (int4, nvfp4, fp8 weight-only, int8, int8 weight-only): experts of width - 1 and 1 rows, and one of width rows, so the copy length
   comes from each owner's expert; each file's exact grouped case and flag-checking sweep.
 
 * every count at once: one tile at K = 4096 (32 chunks) over G = 2 .. 14 and 32 CTAs, so each format runs one owner
-  with 1 to 13 and 31 contributors, at M = 1, 5, 16, 17 and 32 (two CTAs per SM at the decode widths of int4 and int8).
+  with 1 to 13 and 31 contributors, at M = 1, 5, 16, 17 and 32 (two CTAs per SM at the decode widths of int4, int8
+  and 2:4-sparse e4m3).
 
 Every run asserts through tests/streamk_model.py that it has the contributor counts it claims, and
 tests/test_streamk_plan.py checks on the CPU that the boundary cases reach every boundary.
@@ -30,9 +31,9 @@ from test_exact_gemm_gpu import OP_FORMAT, _sweep
 pytestmark = pytest.mark.gpu
 
 N, K = 128, 8192
-STAGED_OPS = ("int4", "int8_dyn", "mxfp8", "nvfp4", "nvfp4w", "mxfp4", "int8wo", "fp8wo")
-CONTROL_OPS = ("fp8",)
-GROUPED_FORMATS = ("int4", "nvfp4", "fp8wo")
+STAGED_OPS = ("int4", "int8_dyn", "mxfp8", "nvfp4", "nvfp4w", "mxfp4", "int8wo", "fp8wo", "fp8_sparse")
+CONTROL_OPS = ("fp8", "fp8_blockwise")
+GROUPED_FORMATS = ("int4", "nvfp4", "fp8wo", "int8", "int8wo")
 K_COUNTS, GRIDS_COUNTS = 4096, list(range(2, 15)) + [32]
 
 
@@ -113,6 +114,10 @@ def _grouped_case(fmt, offs, M, seed):
         from test_grouped_int4_gpu import GroupedCase, _sweep as sweep
 
         return GroupedCase(offs, M, N, K, 128, seed), sweep
+    if fmt in ("int8", "int8wo"):
+        from test_grouped_int8_gpu import GroupedCase, _sweep as sweep
+
+        return GroupedCase(fmt, offs, M, N, K, seed), sweep
     if fmt == "nvfp4":
         from test_grouped_nvfp4_gpu import GroupedCase, _sweep as sweep
     else:
@@ -132,7 +137,7 @@ def test_grouped_staged_gather_boundaries_bit_exact(ops, set_ctas, ci):
 
 
 @pytest.mark.parametrize("M", [1, 5, 16, 17, 32])
-@pytest.mark.parametrize("op", ["int4", "int8_dyn", "fp8", "nvfp4"])
+@pytest.mark.parametrize("op", ["int4", "int8_dyn", "fp8", "nvfp4", "fp8_sparse"])
 def test_owner_contributor_counts_bit_exact(ops, set_ctas, op, M):
     for G in GRIDS_COUNTS:
         p = sk.plan(OP_FORMAT[op], M, N, K_COUNTS, grid=G, sm=ex.sm_count())

@@ -4,12 +4,14 @@
 * the ring of every format policy (streamk_model.ring), pinned, so that a change to a policy's stage layout fails here
   first;
 * coverage: the case lists of the exact GPU sweeps (test_exact_gemm_gpu.GRID_CASES and TAILS, the staged-gather
-  cases, the grouped cases of the int4, nvfp4 and fp8 weight-only grouped tests) reach every segment pattern and every
-  owner gather the kernel has, for every token-tile width of every format, so that an edit of a case list or of the
-  walk that loses a pattern fails here, before a GPU run.  Where a kernel stages partials in its ring, the gather's
-  boundaries are counted from S, its stage count: owners with 1, S - 1, S and S + 1 contributors, every remainder
-  (c - S) mod GB of the register path behind the staged ones, more than 32 (and 64) flags polled after staging, and an
-  owner tile with fewer valid token columns than the width.
+  cases, the grouped cases of the int4, nvfp4, fp8 weight-only, int8 and int8 weight-only grouped tests, and of the
+  rowwise and blockwise e4m3 grouped tests) reach every segment pattern and every owner gather the kernel has, for
+  every token-tile width of every format, so that an edit of a case list or of the walk that loses a pattern fails
+  here, before a GPU run.  Where a kernel stages partials in its ring, the gather's boundaries are counted from S, its
+  stage count: owners with 1, S - 1, S and S + 1 contributors, every remainder (c - S) mod GB of the register path
+  behind the staged ones, more than 32 (and 64) flags polled after staging, and an owner tile with fewer valid token
+  columns than the width.  Where it does not, the register gather's: 1 to 5 contributors, every c mod GB, more than
+  32 and 64.
 """
 import pytest
 
@@ -62,15 +64,18 @@ def test_partition_invariants(KT):
 # grouped ones (None: no grouped kernel); from the policy structs of ao_b200/csrc
 RINGS = {
     "int4": ((7, 6, 7, 4), (16, 32), (12, 11, 7, 4)),
-    "int8": ((6, 5, 8, 6), (16, 32), None),
+    "int8": ((6, 5, 8, 6), (16, 32), (11, 10, 8, 6)),
     "fp8": ((11, 10, 8), (), ()),
     "mxfp8": ((9, 8, 6, 4), (16, 32, 64), None),
     "mxfp4": ((12, 11, 8, 4), (16, 32), None),
     "nvfp4": ((12, 11, 8, 4), (16, 32), (12, 11, 8, 4)),
-    "int8wo": ((5, 4, 6, 4), (16, 32, 64), None),
+    "int8wo": ((5, 4, 6, 4), (16, 32, 64), (10, 8, 6, 4)),
     "fp8wo": ((9, 8, 6, 4), (16, 32, 64), (9, 8, 6, 4)),
+    "fp8_sparse": ((9, 7, 11, 7), (16,), None),
+    "fp8_blockwise": ((10, 9, 8), (), (10, 9, 8)),
 }
-TWO_CTAS = {("int4", 16), ("int4", 32), ("int8", 16), ("int8", 32), ("int8wo", 16), ("int8wo", 32)}
+TWO_CTAS = {("int4", 16), ("int4", 32), ("int8", 16), ("int8", 32), ("int8wo", 16), ("int8wo", 32),
+            ("fp8_sparse", 16), ("fp8_sparse", 32)}
 
 
 @pytest.mark.parametrize("fmt", sorted(RINGS))
@@ -232,23 +237,31 @@ def test_staged_gather_cases_reach_every_staged_boundary():
                 assert not msg, "the staged-gather cases: " + msg
 
 
-@pytest.mark.parametrize("fmt,module", [("int4", "test_grouped_int4_gpu"), ("nvfp4", "test_grouped_nvfp4_gpu"),
-                                        ("fp8wo", "test_grouped_fp8_weight_only_gpu")])
-def test_grouped_cases_reach_every_staged_boundary(fmt, module):
-    """The grouped sweeps of a format (its GROUPED_CASES and the staged-gather cases) reach every boundary of the
-    staged gather at every width whose partials are staged."""
+def _grouped_suite_features(fmt, module):
+    """{width: gather features} of the grid sweep of a grouped test module's GROUPED_CASES."""
     import importlib
-
-    import test_staged_gather_gpu as staged
 
     suite = importlib.import_module(module)
     reached = {}
     for case in suite.GROUPED_CASES:
         rows, N, K, tail, grids = (case[0], case[1], case[2], case[-2], case[-1])
         offs, M = gm.cumulative(rows), sum(rows) + tail
-        for G in [None] + suite.grids_of(rows, N, K, tail, grids, 132):
+        args = (rows, N, K, tail, grids, 132)
+        for G in [None] + (suite.grids_of(fmt, *args) if module == "test_grouped_int8_gpu" else suite.grids_of(*args)):
             p = gm.plan(offs, M, N, K, grid=G, fmt=fmt)
             reached.setdefault(p.width, set()).update(_gather_features(p, grouped=True))
+    return reached
+
+
+@pytest.mark.parametrize("fmt,module", [("int4", "test_grouped_int4_gpu"), ("nvfp4", "test_grouped_nvfp4_gpu"),
+                                        ("fp8wo", "test_grouped_fp8_weight_only_gpu"), ("int8", "test_grouped_int8_gpu"),
+                                        ("int8wo", "test_grouped_int8_gpu")])
+def test_grouped_cases_reach_every_staged_boundary(fmt, module):
+    """The grouped sweeps of a format (its GROUPED_CASES and the staged-gather cases) reach every boundary of the
+    staged gather at every width whose partials are staged."""
+    import test_staged_gather_gpu as staged
+
+    reached = _grouped_suite_features(fmt, module)
     for f, width, rows, grids, found in staged.GROUPED_CASES:
         if f == fmt:
             for G in grids:
@@ -259,3 +272,16 @@ def test_grouped_cases_reach_every_staged_boundary(fmt, module):
             msg = _missing(f"grouped {fmt}", fmt, width, True, _required_gather(fmt, width, True, gt64=False),
                            reached.get(width, set()))
             assert not msg, f"{module}.GROUPED_CASES and the staged-gather cases: " + msg
+
+
+@pytest.mark.parametrize("fmt,module", [("fp8", "test_grouped_mm_gpu"),
+                                        ("fp8_blockwise", "test_grouped_fp8_blockwise_gpu")])
+def test_grouped_cases_reach_every_register_gather(fmt, module):
+    """The grouped e4m3 kernels do not stage (PROMOTE): every owner reads its contributors' partials from L2.  Their
+    GROUPED_CASES reach owners with 1 to 5 contributors, every remainder c mod GB of the partial groups, and more than
+    32 and 64 contributors (flags polled 32 at a time), at every token-tile width."""
+    reached = _grouped_suite_features(fmt, module)
+    for width in sk.WIDTHS[fmt]:
+        assert not sk.ring(fmt, width, grouped=True)[3], (fmt, width)
+        msg = _missing(f"grouped {fmt}", fmt, width, True, _required_gather(fmt, width, True), reached.get(width, set()))
+        assert not msg, f"{module}.GROUPED_CASES: " + msg
