@@ -111,6 +111,13 @@ struct SsFmt {
   }
 };
 
+// Static e4m3 activations (PrototypeFloat8Tensor): the operands, wgmmas and promotion of SsFmt<KIND_F8>, and the EPI_F8
+// output with a per-tensor weight scale read as one value, followed, with output_act_quant_scale, by its e4m3
+// quantize-dequantize (EPI_F8_STATIC)
+struct F8StaticFmt : SsFmt<KIND_F8> {
+  static constexpr int EPI = tsg::EPI_F8_STATIC;
+};
+
 // Blockwise e4m3 (Float8DynamicActivationFloat8WeightConfig with PerBlock([1, 128]) activations and PerBlock([128,
 // 128]) weights; reference float8_tensor.py:431-447 and its Triton loop, kernels.py:86-97): the operands, wgmmas and
 // per-chunk promotion of SsFmt<KIND_F8>.  A tile is 128 weight rows and a chunk 128 k, i.e. exactly one weight block
@@ -770,6 +777,34 @@ extern "C" int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, in
   AO_REQUIRE(xq && x_scale && wq && w_scale && y, "fp8 linear: null pointer");
   return lowp::rowwise<lowp::KIND_F8>(xq, x_scale, M, K, wq, w_scale, N, bias, y, nullptr, workspace, workspace_bytes,
                                       stream);
+}
+
+// F.linear(x, PrototypeFloat8Tensor) (prototype_float8_tensor.py:329-474) on the static quantizer's codes: the output of
+// ao_fp8_rowwise_linear, y = bf16(acc * (x_scale[m] * w_scale[n]) + bias[n]), with w_scale[0] for every n when
+// w_scale_per_row == 0; with out_scale, y is then quantized to e4m3 with the output scale and dequantized:
+// bf16(fp32(e4m3(clamp(y / s, -448, 448))) * s), s = out_scale[0] or (out_scale_per_row) out_scale[m]
+extern "C" int ao_fp8_static_linear(const uint8_t* xq, const float* x_scale, int M, int K, const uint8_t* wq,
+                                    const float* w_scale, int w_scale_per_row, int N, const uint16_t* bias,
+                                    const float* out_scale, int out_scale_per_row, uint16_t* y, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 static linear: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE(K % 16 == 0, "fp8 static linear: K=%d must be a multiple of 16 (reference: quantization/utils.py:663-687)", K);
+  AO_REQUIRE(N % 16 == 0, "fp8 static linear: N=%d must be a multiple of 16 (reference: quantization/utils.py:663-687)", N);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(xq && x_scale && wq && w_scale && y, "fp8 static linear: null pointer");
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(xq) & 15) == 0, "fp8 static linear: xq must be 16-byte aligned");
+  CUtensorMap tm_w, tm_aux;
+  if (int rc = lowp::F8StaticFmt::make_maps(wq, N, K, &tm_w, &tm_aux)) return rc;
+  tsg::Params p{};
+  p.row_scale = x_scale;
+  p.w_scale = w_scale;
+  p.out_scale = out_scale;
+  p.out_scale_per_row = (out_scale_per_row ? tsg::F8S_OUT_PER_TOKEN : 0) | (w_scale_per_row ? 0 : tsg::F8S_W_PER_TENSOR);
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.M = M; p.N = N; p.N_out = N; p.K = K;
+  return tsg::run<lowp::F8StaticFmt>(p, tm_w, tm_aux, xq, K, workspace, workspace_bytes, "fp8 static linear",
+                                     reinterpret_cast<cudaStream_t>(stream));
 }
 
 // F.linear(x, Float8Tensor with 128x128 weight blocks and 1x128 activation blocks) (float8_tensor.py:431-447):

@@ -19,6 +19,7 @@
 // the partial + flag, OWNER: add the contributors' partials in CTA order, then outputs).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 
 #include <type_traits>
 
@@ -96,23 +97,37 @@ constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA && !IsGroup
 constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
 
 // Epilogue arithmetic, per kind (Fmt::EPI; must stay what each format's reference computes, see Params)
-enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2, EPI_BF16_WSCALE = 3, EPI_BF16 = 4, EPI_F8_SPARSE = 5 };
+enum Epi { EPI_FLOAT = 0, EPI_I8 = 1, EPI_F8 = 2, EPI_BF16_WSCALE = 3, EPI_BF16 = 4, EPI_F8_SPARSE = 5, EPI_F8_STATIC = 6 };
+// EPI_F8_STATIC: Params::out_scale_per_row is a set of these flags
+enum F8StaticFlags { F8S_OUT_PER_TOKEN = 1, F8S_W_PER_TENSOR = 2 };
+
+// The output fake-quant of PrototypeFloat8Tensor (EPI_F8_STATIC), on the bf16 value y of the EPI_F8 epilogue:
+// fp32(e4m3(clamp(y / s, -448, 448))) * s, the division a true one (torch divides by the scale tensor) and a NaN
+// quotient kept NaN by the clamp (x / 0 = +-inf gives +-448, 0 / 0 NaN).  The caller rounds the product to bf16.
+__device__ __forceinline__ float e4m3_qdq(float y, float s) {
+  float v = __fdiv_rn(y, s);
+  if (!isnan(v)) v = fminf(fmaxf(v, -448.f), 448.f);
+  const __half_raw h = __nv_cvt_fp8_to_halfraw(__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3), __NV_E4M3);
+  return __half2float(__half(h)) * s;
+}
 
 struct Params {
   const __nv_bfloat16* bias;
-  const float* row_scale;   // EPI_FLOAT: optional per-token scale [M]; EPI_I8 / EPI_F8 / EPI_F8_SPARSE: the activation
-                            // scale [M]
+  const float* row_scale;   // EPI_FLOAT: optional per-token scale [M]; EPI_I8 / EPI_F8 / EPI_F8_SPARSE / EPI_F8_STATIC: the
+                            // activation scale [M]
   const float* out_scale;   // EPI_FLOAT: optional device scalar, or (out_scale_per_row) one value per output feature;
-                            // Grouped<Fmt>: one value per expert [E] (nvfp4: the per-expert weight scale)
+                            // Grouped<Fmt>: one value per expert [E] (nvfp4: the per-expert weight scale);
+                            // EPI_F8_STATIC: the output fake-quant scale (nullptr: none), one value or one per token [M]
   // The grouped fields share storage and padding with the dense ones, so Params keeps its 120 bytes: a larger
   // parameter block changed the code ptxas generates for every dense instantiation.
   union {
     const float* out_scale2;  // EPI_FLOAT: optional second device scalar multiplied into out_scale (nvfp4 a_pts * b_pts)
     const int* offs;          // Grouped<Fmt>: [E] on the device, see below (the grouped epilogue never reads out_scale2)
   };
-  int out_scale_per_row;
+  int out_scale_per_row;     // EPI_F8_STATIC: F8StaticFlags
   int grid_forced;          // Grouped<Fmt>: the host grid was forced (ao_b200_debug_set_streamk_ctas): no MIN_UNITS rule
-  const float* w_scale;     // EPI_I8 / EPI_F8 / EPI_F8_SPARSE / EPI_BF16_WSCALE: per-output-feature weight scale [N]
+  const float* w_scale;     // EPI_I8 / EPI_F8 / EPI_F8_SPARSE / EPI_F8_STATIC / EPI_BF16_WSCALE: per-output-feature weight
+                            // scale [N] (EPI_F8_STATIC with F8S_W_PER_TENSOR: one value)
                             // (EPI_BF16 never
                             // reads it: its format applies the scale per weight, from the aux operand, or, blockwise
                             // e4m3, per 128x128 block [N/128][KT] in its promotion; grouped: [E * N/128][KT])
@@ -563,6 +578,8 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
             if (p.out_scale2) osc *= *p.out_scale2;
           }
           osc *= __int_as_float((127 + Fmt::ACC_EXP2) << 23);
+        } else if constexpr (Fmt::EPI == EPI_F8_STATIC) {
+          sw = w_scale[p.out_scale_per_row & F8S_W_PER_TENSOR ? 0 : n];
         } else if constexpr (Fmt::EPI != EPI_BF16) {
           sw = w_scale ? w_scale[n] : 1.f;
         }
@@ -604,6 +621,12 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
               // contracts the last multiply and the add into one FFMA (its SASS has no FADD: DESIGN §2g)
               const float t = __fmul_rn(__uint_as_float(raw), sw);
               *dst = __float2bfloat16_rn(__fmaf_rn(t, p.row_scale[m], bias));
+            } else if constexpr (Fmt::EPI == EPI_F8_STATIC) {
+              // EPI_F8's bf16 output; with out_scale, then the output fake-quant with the token's (or the one) scale
+              const __nv_bfloat16 y = __float2bfloat16_rn(__uint_as_float(raw) * (p.row_scale[m] * sw) + bias);
+              *dst = p.out_scale ? __float2bfloat16_rn(e4m3_qdq(__bfloat162float(y),
+                                                               p.out_scale[p.out_scale_per_row & F8S_OUT_PER_TOKEN ? m : 0]))
+                                 : y;
             } else {
               *dst = __float2bfloat16_rn(__uint_as_float(raw) * (p.row_scale[m] * sw) + bias);
             }

@@ -12,6 +12,7 @@ from .quant_api import (  # noqa: F401
 from .transform_module import register_quantize_module_handler  # noqa: F401
 from .utils import compute_error  # noqa: F401
 from ao_b200.float8.inference import Float8MMConfig  # noqa: F401
+from ao_b200.prototype.quantization.quant_api import Float8StaticActivationFloat8WeightConfig  # noqa: F401,E402
 
 import torch as _torch
 

@@ -215,6 +215,26 @@ int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, int M, int K,
                           const uint8_t* wq, const float* w_scale, int N,
                           const uint16_t* bias, uint16_t* y, void* workspace,
                           size_t workspace_bytes, void* stream);
+/* Static (calibrated) e4m3 quantisation of activations, one launch: replaces PrototypeFloat8Tensor.from_hp(x,
+ * scale=act_quant_scale) (prototype_float8_tensor.py:182-203, quant_primitives.py:2271-2287) on CUDA tensors:
+ *   q[m,k] = e4m3(clamp(fp32(x[m,k]) / scale[m], -448, 448)),
+ * an IEEE division (not a reciprocal multiply); a NaN quotient stays NaN, x / 0 = +-inf gives +-448, 0 / 0 NaN.
+ * scale f32 is device memory, one value or (scale_per_row != 0) one per row [M]; it is never read on the host.
+ * Outputs: q e4m3 [M,K] (dense bytes), x_scale f32 [M] (the per-row scale ao_fp8_rowwise_linear takes).
+ * x bf16 [M][ldx] (ldx >= K, ldx % 8 == 0, 16-byte aligned), K % 8 == 0.                                           */
+int ao_fp8_quantize_static(const uint16_t* x, int ldx, int M, int K, const float* scale, int scale_per_row, uint8_t* q,
+                           float* x_scale, void* stream);
+/* The linear of PrototypeFloat8Tensor (prototype_float8_tensor.py:329-474) on the codes of ao_fp8_quantize_static:
+ *   y[m,n] = bf16( (Xq Wq^T)[m,n] * (x_scale[m] * w_scale[n]) + bias[n] ),
+ * as ao_fp8_rowwise_linear computes it, with w_scale[0] for every n when w_scale_per_row == 0 (a PerTensor weight:
+ * no [N] copy of its scale).  With out_scale (NULL: none), the output fake-quant (output_act_quant_scale, :461-472)
+ * follows in the GEMM's epilogue:
+ *   out[m,n] = bf16(fp32(e4m3(clamp(fp32(y[m,n]) / s, -448, 448))) * s),
+ * s = out_scale[0], or out_scale[m] when out_scale_per_row != 0 (device memory, never read on the host); the division
+ * is IEEE, as in ao_fp8_quantize_static.  xq 16-byte aligned, K % 16 == 0, N % 16 == 0.                             */
+int ao_fp8_static_linear(const uint8_t* xq, const float* x_scale, int M, int K, const uint8_t* wq, const float* w_scale,
+                         int w_scale_per_row, int N, const uint16_t* bias, const float* out_scale, int out_scale_per_row,
+                         uint16_t* y, void* workspace, size_t workspace_bytes, void* stream);
 /* Replaces torchao's aten._grouped_mm handler for a rowwise Float8Tensor expert weight, i.e.
  * torch._scaled_grouped_mm / F.scaled_grouped_mm rowwise (float8_tensor.py:1085-1122), 2-D x 3-D form:
  * for offs[e-1] <= m < offs[e] (offs[-1] = 0):
