@@ -5,6 +5,7 @@
 //                         and, 1x128 x 128x128 block scales, the reference's blockwise Triton GEMM
 //                         and, 2:4-sparse weights (wgmma.sp), the reference's CUTLASS sparse GEMM
 //   mxfp8 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm block-scaled
+//                         and, mxfp8 and mxfp4 per expert, torch._grouped_mm on 3-D MX expert weights
 //   nvfp4 block-16 e4m3   (bf16 wgmma on exactly dequantised operands)   replaces torch._scaled_mm fp4 + pts/bias kernels
 //   nvfp4 weight x bf16   (bf16 wgmma, weights dequantised exactly)      replaces F.linear on the dequantised weight
 //   mxfp4 block-32 e8m0   (bf16 wgmma on exactly dequantised operands)   replaces F.linear on both dequantize()s
@@ -316,6 +317,7 @@ struct Mxfp8Fmt {
   static constexpr int EPI = tsg::EPI_FLOAT;
   static constexpr int ACC_EXP2 = 0;
   static constexpr int MAX_N_MMA = 128;
+  static constexpr bool EXPERT_SCALE = false;   // grouped: y = acc, the dense MX epilogue without bias
   // the weights and the blocked scale tiles, one 512-byte tile per box
   static int make_maps(const uint8_t* wq, const uint8_t* w_sf, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
     if (int rc = kmajor_byte_map(wq, N, K, tm_w)) return rc;
@@ -327,6 +329,15 @@ struct Mxfp8Fmt {
                                                  uint64_t policy) {
     tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, n_tile * ROWS, policy);
     tma_load_2d(aux_dst, tm_sf, bar, 0, n_tile * p.aux_col_blocks + kc, policy);
+  }
+  // grouped kernels: the 128 weight rows from `row` = e*N + 128t of the [E * N, K] map of all experts' weights, and
+  // their scale tile at row block row / 128 of the blocked [E * N, K / 32] scales.  The launcher requires N % 128 == 0,
+  // which keeps every expert's weights and scales in whole 128-row blocks, so no tile has a tail (Nvfp4Fmt::issue_w_rows)
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, const CUtensorMap* tm_sf,
+                                                      const tsg::Params& p, uint8_t* w_dst, uint8_t* aux_dst,
+                                                      uint64_t* bar, int row, int kc, uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * KCHUNK, row, policy);
+    tma_load_2d(aux_dst, tm_sf, bar, 0, (row / ROWS) * p.aux_col_blocks + kc, policy);
   }
   // the thread's two fragment rows: for k16 step kk the e4m3 pair at k 16kk + 2t (low half) and + 8 (high half)
   struct Raw {
@@ -383,6 +394,7 @@ struct Mxfp4Fmt {
   static constexpr int EPI = tsg::EPI_FLOAT;
   static constexpr int ACC_EXP2 = 0;
   static constexpr int MAX_N_MMA = 128;
+  static constexpr bool EXPERT_SCALE = false;   // grouped: y = acc, the dense MX epilogue without bias
   static int make_maps(const uint8_t* wq, const uint8_t* w_sf, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
     const uint64_t dims[2] = {(uint64_t)K / 2, (uint64_t)N};
     const uint64_t str[1] = {(uint64_t)K / 2};
@@ -397,6 +409,13 @@ struct Mxfp4Fmt {
                                                  uint64_t policy) {
     tma_load_2d(w_dst, tm_w, bar, kc * 64, n_tile * ROWS, policy);
     tma_load_2d(aux_dst, tm_sf, bar, 0, n_tile * p.aux_col_blocks + kc, policy);
+  }
+  // grouped kernels: Mxfp8Fmt::issue_w_rows on the [E * N, K / 2] map of all experts' packed weights
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, const CUtensorMap* tm_sf,
+                                                      const tsg::Params& p, uint8_t* w_dst, uint8_t* aux_dst,
+                                                      uint64_t* bar, int row, int kc, uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * 64, row, policy);
+    tma_load_2d(aux_dst, tm_sf, bar, 0, (row / ROWS) * p.aux_col_blocks + kc, policy);
   }
   // c[h][j]: row h's code bytes of k16 steps 2j, 2j + 1 (step kk reads byte t of bytes 8kk..8kk+3, the k pair
   // 16kk + 2t, and byte t of 8kk+4..8kk+7, the pair 8 further), as bytes (2j lo, 2j hi, 2j+1 lo, 2j+1 hi);
@@ -1029,6 +1048,38 @@ extern "C" int ao_nvfp4_weight_linear(const uint16_t* x, const float* x_scale, i
                                       void* stream) {
   return ao_nvfp4_weight_linear_ex(x, K, x_scale, M, K, wq, w_scale_blocked, b_pts, 0, N, bias, y, workspace, workspace_bytes,
                                    stream);
+}
+
+// torch._grouped_mm(x, W.transpose(-2, -1), offs) on MX expert weights, 2-D x 3-D: expert e's rows [offs[e-1], offs[e])
+// of x (bf16: the exactly dequantised activation codes of ao_mx*_fakequant) against wq[e] with its blocked e8m0 scales,
+// y = bf16(acc), the dense MX linear's epilogue without bias.  offs stays on the device (grouped schedule, ts_gemm.cuh).
+template <class Fmt>
+static int mx_grouped_mm(const char* what, const uint16_t* x, int M, int K, const uint8_t* wq,
+                         const uint8_t* w_scale_blocked, int E, int N, const int32_t* offs, uint16_t* y, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(K % 32 == 0, "%s: K=%d must be a multiple of 32 (mx_tensor.py:244-246)", what, K);
+  // every expert's weights and scales start on a 128-row block of the stacked [E * N, ..] tensors
+  AO_REQUIRE(N % 128 == 0, "%s: N=%d must be a multiple of 128", what, N);
+  return tsg::run_grouped<Fmt>(what, x, M, K, E, N, N, offs, y, workspace, workspace_bytes, stream,
+                               [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
+    AO_REQUIRE(wq && w_scale_blocked, "%s: null pointer", what);
+    p.aux_col_blocks = ceil_div(K / 32, 4);
+    return Fmt::make_maps(wq, w_scale_blocked, E * N, K, tm_w, tm_sf);
+  });
+}
+
+extern "C" int ao_mxfp8_grouped_mm(const uint16_t* x, int M, int K, const uint8_t* wq, const uint8_t* w_scale_blocked,
+                                   int E, int N, const int32_t* offs, uint16_t* y, void* workspace,
+                                   size_t workspace_bytes, void* stream) {
+  return mx_grouped_mm<lowp::Mxfp8Fmt>("mxfp8 grouped mm", x, M, K, wq, w_scale_blocked, E, N, offs, y, workspace,
+                                       workspace_bytes, stream);
+}
+
+extern "C" int ao_mxfp4_grouped_mm(const uint16_t* x, int M, int K, const uint8_t* wq, const uint8_t* w_scale_blocked,
+                                   int E, int N, const int32_t* offs, uint16_t* y, void* workspace,
+                                   size_t workspace_bytes, void* stream) {
+  return mx_grouped_mm<lowp::Mxfp4Fmt>("mxfp4 grouped mm", x, M, K, wq, w_scale_blocked, E, N, offs, y, workspace,
+                                       workspace_bytes, stream);
 }
 
 // torch._grouped_mm(x, W.transpose(-2, -1), offs) on NVFP4 expert weights (nvfp4_tensor.py:709-753), 2-D x 3-D:

@@ -54,6 +54,9 @@ class MXDynamicActivationMXWeightConfig(AOBaseConfig):
 def _mx_inference_linear_transform(module, config: MXDynamicActivationMXWeightConfig, *, parameter_name="weight"):
     weight = getattr(module, parameter_name)
     assert weight.dtype == torch.bfloat16, f"Only supporting bf16 out dtype for now, got {weight.dtype}"
+    if weight.dim() == 3 and not _expert_rows_compat(weight, "MX"):
+        # MoE expert weights [E, N, K] for torch._grouped_mm (MXTensor, aten._grouped_mm)
+        return module
     act = QuantizeTensorToMXKwargs(elem_dtype=config.activation_dtype, block_size=config.block_size,
                                    kernel_preference=config.kernel_preference, is_swizzled_scales=True,
                                    scaling_mode=config.scaling_mode)
@@ -81,12 +84,13 @@ def _nvfp4_kernel_compat(weight, k_multiple: int) -> bool:
     return True
 
 
-def _nvfp4_expert_rows_compat(weight) -> bool:
-    """The grouped expert GEMM reads each expert's weights and blocked scales as whole 128-row blocks of the stacked
-    [E * N, ..] tensors (ts_gemm.cuh, Grouped<Nvfp4Fmt>), so it needs out_features % 128 == 0; the reference's 3-D
-    blocked scale layout has the same requirement (to_blocked over E * N rows).  Other layers stay unquantized."""
+def _expert_rows_compat(weight, fmt="NVFP4") -> bool:
+    """The grouped expert GEMMs read each expert's weights and blocked scales as whole 128-row blocks of the stacked
+    [E * N, ..] tensors (ts_gemm.cuh, Grouped<Nvfp4Fmt> / <Mxfp8Fmt> / <Mxfp4Fmt>), so they need out_features % 128
+    == 0; the reference's 3-D blocked scale layout has the same requirement (to_blocked over E * N rows).  Other layers
+    stay unquantized."""
     if weight.shape[-2] % 128 != 0:
-        logger.info(f"Skipping NVFP4 quantization: expert out_features={weight.shape[-2]} is not a multiple of 128; "
+        logger.info(f"Skipping {fmt} quantization: expert out_features={weight.shape[-2]} is not a multiple of 128; "
                     f"weight shape {tuple(weight.shape)} stays {weight.dtype}")
         return False
     return True
@@ -118,7 +122,7 @@ def _nvfp4_inference_linear_transform(module, config, *, parameter_name="weight"
         if not config.use_dynamic_per_tensor_scale:
             raise NotImplementedError("NVFP4DynamicActivationNVFP4WeightConfig on 3-D (MoE) weights needs "
                                       "use_dynamic_per_tensor_scale=True")
-        if not _nvfp4_kernel_compat(weight, 128) or not _nvfp4_expert_rows_compat(weight):
+        if not _nvfp4_kernel_compat(weight, 128) or not _expert_rows_compat(weight):
             return module
         pts = per_tensor_amax_to_scale(torch.amax(torch.abs(weight), dim=(1, 2))).view(-1, 1, 1)
     else:

@@ -56,9 +56,11 @@ class MXTensor(TorchAOBaseTensor):
 
     def __new__(cls, qdata, scale, elem_dtype, block_size, orig_dtype, kernel_preference, act_quant_kwargs,
                 is_swizzled_scales):
-        shape = qdata.shape
+        shape = list(qdata.shape)
         if elem_dtype == torch.float4_e2m1fn_x2:
-            shape = (*shape[:-1], shape[-1] * 2)   # two codes per byte: the high-precision shape
+            # two codes per byte: the high-precision shape.  A transposed 3-D expert weight (qdata [E, K/2, N], how
+            # torch._grouped_mm receives it) packs dim -2
+            shape[-2 if _is_transposed_3d(qdata) else -1] *= 2
         return torch.Tensor._make_wrapper_subclass(cls, shape, dtype=orig_dtype, device=qdata.device,
                                                    requires_grad=False)
 
@@ -95,13 +97,16 @@ class MXTensor(TorchAOBaseTensor):
         if scaling_mode != ScaleCalculationMode.RCEIL:
             raise NotImplementedError("only ScaleCalculationMode.RCEIL (the inference default) is implemented")
         lead, K = data_hp.shape[:-1], data_hp.shape[-1]
-        x2 = data_hp.reshape(-1, K)
-        if elem_dtype == torch.float4_e2m1fn_x2:
-            q, s = torch.ops.ao_b200.mxfp4_quantize(x2, is_swizzled_scales)
-            q = q.reshape(*lead, K // 2)
+        quantize = torch.ops.ao_b200.mxfp4_quantize if elem_dtype == torch.float4_e2m1fn_x2 else torch.ops.ao_b200.mxfp8_quantize
+        if data_hp.dim() == 3 and is_swizzled_scales:
+            # a 3-D expert weight [E, N, K]: expert by expert (setup time only), each expert's blocked scales one after
+            # the other, [E, 32 * ceil(N/128), 16 * ceil(K/128)].  For N % 128 == 0 that is the reference's to_blocked of
+            # the [E*N, K/32] scales (mx_tensor.py:401-407); otherwise every expert starts on its own 128-row block
+            qs, ss = zip(*(quantize(data_hp[e], True) for e in range(data_hp.shape[0])))
+            q, s = torch.stack(qs), torch.stack(ss)
         else:
-            q, s = torch.ops.ao_b200.mxfp8_quantize(x2, is_swizzled_scales)
-            q = q.reshape(*lead, K)
+            q, s = quantize(data_hp.reshape(-1, K), is_swizzled_scales)
+            q = q.reshape(*lead, q.shape[-1])
         s = s.view(torch.float8_e8m0fnu)
         if not is_swizzled_scales:
             s = s.reshape(*lead, K // block_size)
@@ -109,27 +114,47 @@ class MXTensor(TorchAOBaseTensor):
                         is_swizzled_scales)
 
     def dequantize(self, output_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+        """code x 2^(e - 127) in fp32, then cast.  A 3-D expert weight is dequantized expert by expert, its transposed
+        view as the transpose of that."""
         out = output_dtype or self.orig_dtype
-        K = self.shape[-1]
-        rows = self.qdata.numel() // self.qdata.shape[-1]
-        s = self.scale.view(torch.uint8)
-        if self.is_swizzled_scales:
-            s = from_blocked(s.reshape(-1), rows, K // self.block_size)
-        s = s.reshape(rows, K // self.block_size)
-        e = torch.pow(2.0, s.to(torch.float32) - 127.0)
-        e = torch.where(s == 255, torch.full_like(e, float("nan")), e)
-        if self.elem_dtype == torch.float4_e2m1fn_x2:
-            q = self.qdata.view(torch.uint8).reshape(rows, K // 2)
-            c = torch.stack([q & 15, q >> 4], dim=-1).reshape(rows, K).to(torch.int32)   # even k in the low nibble
-            ce, cm = (c >> 1) & 3, (c & 1).to(torch.float32)
-            # e2m1 (s e1 e0 m): m / 2 for e = 0, else 2^(e-1) * (1 + m / 2); no host table, so it can be graph-captured
-            p2 = torch.bitwise_left_shift(torch.ones_like(ce), (ce - 1).clamp(min=0)).to(torch.float32)
-            v = torch.where(ce == 0, 0.5 * cm, p2 * (1.0 + 0.5 * cm))
-            v = torch.where((c & 8) != 0, -v, v)
-        else:
-            v = self.qdata.reshape(rows, K).to(torch.float32)
-        v = v * e.repeat_interleave(self.block_size, dim=1)
-        return v.reshape(self.shape).to(out)
+        if self.qdata.dim() == 3:
+            q, s = self.qdata, self.scale
+            transposed = _is_transposed_3d(q)
+            if transposed:
+                q, s = q.transpose(-2, -1), s.transpose(-2, -1)
+            y = torch.stack([_dequant_2d(q[e], s[e], self.elem_dtype, self.block_size, self.is_swizzled_scales, out)
+                             for e in range(q.shape[0])])
+            return y.transpose(-2, -1) if transposed else y
+        y = _dequant_2d(self.qdata, self.scale, self.elem_dtype, self.block_size, self.is_swizzled_scales, out)
+        return y.reshape(self.shape)
+
+
+def _is_transposed_3d(qdata):
+    return qdata.dim() == 3 and qdata.stride(-2) < qdata.stride(-1)
+
+
+def _dequant_2d(qdata, scale, elem_dtype, block_size, swizzled, out):
+    """[rows, K] codes ([rows, K/2] bytes for mxfp4, or any leading dims) with their scales (plain or blocked) -> [rows, K]."""
+    fp4 = elem_dtype == torch.float4_e2m1fn_x2
+    K = qdata.shape[-1] * (2 if fp4 else 1)
+    rows = qdata.numel() // qdata.shape[-1]
+    s = scale.view(torch.uint8)
+    if swizzled:
+        s = from_blocked(s.reshape(-1), rows, K // block_size)
+    s = s.reshape(rows, K // block_size)
+    e = torch.pow(2.0, s.to(torch.float32) - 127.0)
+    e = torch.where(s == 255, torch.full_like(e, float("nan")), e)
+    if fp4:
+        q = qdata.view(torch.uint8).reshape(rows, K // 2)
+        c = torch.stack([q & 15, q >> 4], dim=-1).reshape(rows, K).to(torch.int32)   # even k in the low nibble
+        ce, cm = (c >> 1) & 3, (c & 1).to(torch.float32)
+        # e2m1 (s e1 e0 m): m / 2 for e = 0, else 2^(e-1) * (1 + m / 2); no host table, so it can be graph-captured
+        p2 = torch.bitwise_left_shift(torch.ones_like(ce), (ce - 1).clamp(min=0)).to(torch.float32)
+        v = torch.where(ce == 0, 0.5 * cm, p2 * (1.0 + 0.5 * cm))
+        v = torch.where((c & 8) != 0, -v, v)
+    else:
+        v = qdata.reshape(rows, K).to(torch.float32)
+    return (v * e.repeat_interleave(block_size, dim=1)).to(out)
 
 
 implements = MXTensor.implements
@@ -141,6 +166,9 @@ implements_torch_function = MXTensor.implements_torch_function
 def _(func, types, args, kwargs):
     x, w, bias = args[0], args[1], args[2] if len(args) > 2 else None
     assert isinstance(w, MXTensor), "MXTensor: weight must be MXTensor"
+    if w.qdata.dim() != 2:
+        raise NotImplementedError("MXTensor linear: 2-D weights only; a 3-D expert weight runs through "
+                                  "torch._grouped_mm(x, w.transpose(-2, -1), offs=offs)")
     k = w.act_quant_kwargs
     if k is None:
         raise NotImplementedError("MX weight-only linear is outside this engine's scope (SURVEY §8)")
@@ -172,9 +200,67 @@ def _(func, types, args, kwargs):
     self, dim, index = args
     assert dim == 0, f"MXTensor aten.select.int with {dim=} is not yet supported"
     assert self.qdata.dim() == self.scale.dim(), "unsupported"
-    assert not self.is_swizzled_scales, "unsupported"
+    # expert e of a 3-D weight [E, N, K] with N % 128 == 0: its blocked scales are the contiguous
+    # [32 * N/128, 16 * ceil(K/128)] slice e of the stacked ones (to_mx), what F.linear(x, w[e]) runs on
+    expert = self.qdata.dim() == 3 and not _is_transposed_3d(self.qdata) and self.shape[-2] % 128 == 0
+    assert not self.is_swizzled_scales or expert, "unsupported"
     qd, sc = self.qdata[index], self.scale[index]
     return return_and_correct_aliasing(func, args, kwargs, MXTensor(qd, sc, self.elem_dtype, self.block_size, self.orig_dtype, self.kernel_preference, self.act_quant_kwargs, self.is_swizzled_scales))
+
+
+@implements(aten.transpose.int)
+def _(func, types, args, kwargs):
+    """A view of a 3-D expert weight with qdata and scale transposed: how W [E, N, K] reaches torch._grouped_mm as
+    mat_b [E, K, N]."""
+    self, dim0, dim1 = args
+    assert self.qdata.dim() == 3, f"MXTensor transpose: 3-D tensors only, got rank {self.qdata.dim()}"
+    assert (dim0, dim1) in ((1, 2), (2, 1), (-1, -2), (-2, -1)), f"transpose unsupported for {dim0=} {dim1=}"
+    new = MXTensor(self.qdata.transpose(dim0, dim1), self.scale.transpose(dim0, dim1), self.elem_dtype, self.block_size,
+                   self.orig_dtype, self.kernel_preference, self.act_quant_kwargs, self.is_swizzled_scales)
+    return return_and_correct_aliasing(func, args, kwargs, new)
+
+
+@implements(aten._grouped_mm.default)
+def _(func, types, args, kwargs):
+    """torch._grouped_mm(x, W.transpose(-2, -1), offs=offs) with an MXTensor expert weight W [E, N, K]
+    (MXDynamicActivationMXWeightConfig, mxfp8 or mxfp4): expert e's rows of the output are the dense MX linear of its
+    rows of x against W[e].  The activations are quantized to the weight's format and dequantized exactly as bf16
+    (mx*_fakequant: MX scales belong to one block of one row, so no expert bookkeeping), then multiplied by each
+    expert's weights, dequantized exactly inside the grouped GEMM.  Only the 2-D x 3-D form, with offs and without
+    bias."""
+    mat_a, mat_b = args[0], args[1]
+    offs = args[2] if len(args) > 2 else kwargs.get("offs", None)
+    bias = args[3] if len(args) > 3 else kwargs.get("bias", None)
+    if not isinstance(mat_b, MXTensor) or isinstance(mat_a, MXTensor):
+        raise NotImplementedError("MXTensor _grouped_mm: only a bf16 mat_a times an MXTensor mat_b")
+    if mat_a.dim() != 2 or mat_b.dim() != 3:
+        raise NotImplementedError(f"MXTensor _grouped_mm: only 2-D mat_a x 3-D mat_b, got {mat_a.dim()}-D x {mat_b.dim()}-D")
+    if offs is None:
+        raise NotImplementedError("MXTensor _grouped_mm: offs is required")
+    if bias is not None:
+        raise NotImplementedError("MXTensor _grouped_mm: bias is not supported")
+    if not _is_transposed_3d(mat_b.qdata):
+        raise NotImplementedError("MXTensor _grouped_mm: mat_b must be the transposed [E, N, K] weight")
+    if not mat_b.is_swizzled_scales:
+        raise NotImplementedError("MXTensor _grouped_mm: the kernel consumes blocked (swizzled) weight scales")
+    k = mat_b.act_quant_kwargs
+    if k is None:
+        raise NotImplementedError("MXTensor _grouped_mm: MX weight-only is outside this engine's scope; only "
+                                  "MXDynamicActivationMXWeightConfig (act_quant_kwargs set)")
+    if k.elem_dtype != mat_b.elem_dtype:
+        raise NotImplementedError(f"MXTensor _grouped_mm: activation element dtype {k.elem_dtype} differs from the "
+                                  f"weight's {mat_b.elem_dtype}")
+    E, K, N = mat_b.shape
+    if mat_a.shape[-1] != K:
+        raise ValueError(f"_grouped_mm: mat_a has K={mat_a.shape[-1]}, mat_b K={K}")
+    ops = torch.ops.ao_b200
+    fp4 = mat_b.elem_dtype == torch.float4_e2m1fn_x2
+    xhat = (ops.mxfp4_fakequant if fp4 else ops.mxfp8_fakequant)(rows_for_kernel(mat_a.to(torch.bfloat16)))
+    wq = mat_b.qdata.transpose(-2, -1)   # back to the stored [E, N, K] / [E, N, K/2]
+    ws = mat_b.scale.transpose(-2, -1)
+    mm = ops.mxfp4_grouped_mm if fp4 else ops.mxfp8_grouped_mm
+    y = mm(xhat, wq.contiguous(), ws.contiguous().view(torch.uint8), offs.to(torch.int32))
+    return y.to(mat_a.dtype)
 
 
 MXTensor.__module__ = "ao_b200.prototype.mx_formats"

@@ -374,6 +374,25 @@ int ao_nvfp4_grouped_mm(const uint16_t* x, const float* x_scale, int M, int K, c
  * Two kernels; offs is never read on the host.                                                                      */
 int ao_nvfp4_fakequant_grouped(const uint16_t* x, int ldx, int M, int K, const int32_t* offs, int E,
                                uint16_t* xhat, float* x_scale, float* row_amax, void* stream);
+/* torch._grouped_mm(x, W.transpose(-2, -1), offs) for a 3-D MXTensor expert weight W [E, N, K] (mxfp8 / mxfp4), 2-D x
+ * 3-D form, as the per-expert recipe select + ao_mx*_linear computes it: for offs[e-1] <= m < offs[e] (offs[-1] = 0)
+ *   y[m, :] = bf16( sum_k x[m,k] * what[e][:,k] ),  f32 accumulate, what = code x 2^(e8 - 127) dequantised exactly
+ * inside the wgmma kernel.  x bf16 [M,K] (tokens sorted by expert, rows contiguous, 16-byte aligned: the xhat of
+ * ao_mx*_fakequant); wq [E][N][K] e4m3 (mxfp8) or [E][N][K/2] packed e2m1, even k in the low nibble (mxfp4);
+ * w_scale_blocked: the blocked e8m0 scales of the [E*N, K/32] scales (each expert's blocked scales one after the
+ * other); offs int32 [E] on the device, cumulative row ends.  The host never reads offs (no sync, CUDA-graph
+ * capturable); the kernel clamps each offs[e] into [offs[e-1], M].  Rows from offs[E-1] on are not written.
+ * 1 <= E <= 1024, K % 32 == 0, N % 128 == 0, no bias.                                                              */
+int ao_mxfp8_grouped_mm(const uint16_t* x, int M, int K, const uint8_t* wq, const uint8_t* w_scale_blocked, int E,
+                        int N, const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes, void* stream);
+int ao_mxfp4_grouped_mm(const uint16_t* x, int M, int K, const uint8_t* wq, const uint8_t* w_scale_blocked, int E,
+                        int N, const int32_t* offs, uint16_t* y, void* workspace, size_t workspace_bytes, void* stream);
+/* The activations of the above: every row of x quantized as ao_mx*_quantize quantizes it (RCEIL e8m0 per 32-element
+ * block) and written back as xhat bf16 [M,K] = code x 2^(e8 - 127), bit for bit what the dense MX linear dequantises
+ * its activations to.  offs is not needed: MX scales couple no rows.  x bf16 [M][ldx] (ldx >= K, ldx % 8 == 0, 16-byte
+ * aligned), K % 32 == 0.  One kernel.                                                                               */
+int ao_mxfp8_fakequant(const uint16_t* x, int ldx, int M, int K, uint16_t* xhat, void* stream);
+int ao_mxfp4_fakequant(const uint16_t* x, int ldx, int M, int K, uint16_t* xhat, void* stream);
 /* Per-token e4m3 quantisation that keeps the codes as bf16 values (exact): xq = bf16(e4m3(x/s)),
  * s = f32(bf16(amax/448)) -- the codes of ao_fp8_quantize_rowwise, i.e. the values Float8Tensor.from_hp(x, PerRow())
  * stores (quant_primitives.py:2172-2287), in the operand type the bf16 MMA consumes.  An all-zero row (s = 0) gives

@@ -4,7 +4,8 @@ F.scaled_grouped_mm on identical operands, for MoE expert shapes; with --fmt nvf
 per-expert activation quantizer nvfp4_fakequant_grouped plus nvfp4_grouped_mm) against the fp8 path with its
 quantizer (fp8_quantize_rowwise plus fp8_rowwise_grouped_mm) and bf16 torch._grouped_mm on the unquantized weights.
 
-  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4|fp8wo|int8wo|int8|fp8_blockwise] [--group-size 32] [--replays 20]
+  python scripts/measure_grouped_mm.py [--fmt fp8|nvfp4|int4|fp8wo|int8wo|int8|fp8_blockwise|mxfp8|mxfp4] [--group-size 32]
+                                       [--replays 20] [--prologue]
                                        [--out FILE]
 
   * shapes: Mixtral-8x7B experts (E=8, 4096 -> 14336 and 14336 -> 4096, top-2) and Qwen3-30B-A3B experts (E=128,
@@ -44,7 +45,14 @@ op with its quantizer on the same codes, and bf16 torch._grouped_mm, on the shap
 128x128 block scale of the active experts, the e4m3 activations and their 1x128 scales, the outputs, offs), its
 roofline term their HBM time, and vs_select_linear compares the output with the loop's.  Torch's blockwise
 F.scaled_grouped_mm is tried and reported as unavailable when this torch build lacks it (it needs torch built for
-CUDA 12.9 or later).  Prefill (2048-token) cases time one round of weight copies per replay.
+CUDA 12.9 or later).  --fmt mxfp8 / mxfp4: the MX expert path (torch._grouped_mm on 3-D MXTensor weights:
+mx*_fakequant plus mx*_grouped_mm) against the eager loop of select + the dense MX linear on each active expert (its
+quantizer and GEMM, captured with the routing fixed), the fp8 rowwise path with its quantizer and bf16
+torch._grouped_mm; bytes are the MX path's (1 or 0.5 bytes per weight and 1 per 32-weight scale of the active experts,
+the bf16 activations read once, the outputs, offs) and its roofline term their HBM time; vs_select_linear compares the
+output with the loop's.  With --prologue it gives instead the kernel time of the one-launch prologue (mx*_fakequant)
+and of the two launches it replaces (mx*_quantize, then the dense linear's dequant_act_kernel), alternated in one
+torch.profiler run with PDL off.  Prefill (2048-token) cases time one round of weight copies per replay.
 """
 from __future__ import annotations
 
@@ -508,13 +516,149 @@ def measure_fp8_blockwise(a, ops, dev, lines):
         torch.cuda.empty_cache()
 
 
+def measure_mx_prologue(a, ops, dev, lines):
+    """Kernel time per call of the one-launch MX prologue (mx*_fakequant) and of the two launches it replaces:
+    mx*_quantize with blocked scales, then the dequant_act_kernel of the dense MX linear (run on a 128-row weight; its
+    GEMM is not counted), on the activations of every case of measure_mx, the two alternated call by call in one
+    torch.profiler run.  main() turns PDL off for this mode (AO_B200_NO_PDL=1): a PDL kernel starts while the one
+    before it still runs, and its time would include that wait."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    from ao_b200.prototype.mx_formats import MXTensor
+
+    fp4 = a.fmt == "mxfp4"
+    elem = torch.float4_e2m1fn_x2 if fp4 else torch.float8_e4m3fn
+    fq = ops.mxfp4_fakequant if fp4 else ops.mxfp8_fakequant
+    quant, lin = (ops.mxfp4_quantize, ops.mxfp4_linear) if fp4 else (ops.mxfp8_quantize, ops.mxfp8_linear)
+    reps = 20
+    for name, E, N, K, topk in SHAPES:
+        g = torch.Generator(device=dev).manual_seed(E * N + K)
+        w = MXTensor.to_mx(torch.randn(128, K, device=dev, generator=g).to(torch.bfloat16), elem, 32,
+                           is_swizzled_scales=True)
+        w128, s128 = w.qdata, w.scale.view(torch.uint8)
+        for T in TOKENS:
+            for skewed in (False, True):
+                M = sum(routing(T, E, topk, skewed, seed=T * 131 + E + skewed))
+                x = torch.randn(M, K, device=dev, generator=g).to(torch.bfloat16)
+                for _ in range(2):   # warm-up outside the profile
+                    fq(x)
+                    lin(*quant(x, True), w128, s128, None)
+                torch.cuda.synchronize()
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    for _ in range(reps):
+                        fq(x)
+                        lin(*quant(x, True), w128, s128, None)
+                    torch.cuda.synchronize()
+                us = {"mx_fakequant_kernel": 0.0, "_quant_kernel": 0.0, "dequant_act_kernel": 0.0}
+                for e in prof.key_averages():
+                    t = getattr(e, "device_time_total", None)
+                    t = e.cuda_time_total if t is None else t
+                    for k in us:
+                        if k in e.key:
+                            us[k] += t / reps
+                rec = dict(fmt=a.fmt, shape=name, K=K, tokens=T, routing="skewed" if skewed else "balanced", rows=M,
+                           prologue_us=round(us["mx_fakequant_kernel"], 2), quantize_us=round(us["_quant_kernel"], 2),
+                           dequant_us=round(us["dequant_act_kernel"], 2),
+                           composition_us=round(us["_quant_kernel"] + us["dequant_act_kernel"], 2))
+                print(json.dumps(rec), flush=True)
+                lines.append(rec)
+
+
+def measure_mx(a, ops, dev, lines):
+    """The MX expert path (mx*_fakequant + mx*_grouped_mm) against the eager select + dense MX linear loop, the fp8
+    rowwise path with its quantizer and bf16 torch._grouped_mm."""
+    import torch
+
+    from ao_b200.prototype.mx_formats import MXTensor
+
+    fp4 = a.fmt == "mxfp4"
+    elem = torch.float4_e2m1fn_x2 if fp4 else torch.float8_e4m3fn
+    fq, gmm = (ops.mxfp4_fakequant, ops.mxfp4_grouped_mm) if fp4 else (ops.mxfp8_fakequant, ops.mxfp8_grouped_mm)
+    quant, lin = (ops.mxfp4_quantize, ops.mxfp4_linear) if fp4 else (ops.mxfp8_quantize, ops.mxfp8_linear)
+    for name, E, N, K, topk in SHAPES:
+        g = torch.Generator(device=dev).manual_seed(E * N + K)
+        w_bytes_expert = N * K // (2 if fp4 else 1) + N * K // 32
+        copies = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * w_bytes_expert)) + 1)
+        copies_bf16 = max(2, math.ceil(2 * L2_BYTES / (min(topk, E) * N * K * 2)) + 1)
+        wm, ws, w8, s8, wb = [], [], [], [], []
+        for c in range(max(copies, copies_bf16)):
+            w = (torch.randn(E, N, K, device=dev, generator=g) * 0.05).to(torch.bfloat16)
+            if c < copies:
+                t = MXTensor.to_mx(w, elem, 32, is_swizzled_scales=True)
+                wm.append(t.qdata)
+                ws.append(t.scale.view(torch.uint8))
+                q, s = ops.fp8_quantize_rowwise(w.reshape(E * N, K))
+                w8.append(q.reshape(E, N, K))
+                s8.append(s.reshape(E, N))
+            if c < copies_bf16:
+                wb.append(w)
+            del w
+        for T in TOKENS:
+            for skewed in (False, True):
+                rows = routing(T, E, topk, skewed, seed=T * 131 + E + skewed)
+                M = sum(rows)
+                offs = torch.tensor(rows, dtype=torch.int64).cumsum(0).to(torch.int32).to(dev)
+                x = torch.randn(M, K, device=dev, generator=g).to(torch.bfloat16)
+                active = sum(1 for r in rows if r)
+                need = active * w_bytes_expert + M * K * 2 + M * N * 2 + E * 4
+                rec = dict(fmt=a.fmt, shape=name, E=E, N=N, K=K, topk=topk, tokens=T,
+                           routing="skewed" if skewed else "balanced", rows=M, active_experts=active, bytes=need,
+                           weight_copies=copies, roofline_us=round(need / HBM_BPS * 1e6, 2))
+                spans, start = [], 0
+                for e, r in enumerate(rows):
+                    if r:
+                        spans.append((e, start, start + r))
+                    start += r
+
+                def ours(c):
+                    return gmm(fq(x), wm[c], ws[c], offs)
+
+                def loop(c, out=None):
+                    for e, s0, s1 in spans:
+                        q, s = quant(x[s0:s1], True)
+                        y = lin(q, s, wm[c][e], ws[c][e], None)
+                        if out is not None:
+                            out.append(y)
+
+                def fp8(c):
+                    xq, sx = ops.fp8_quantize_rowwise(x)
+                    return ops.fp8_rowwise_grouped_mm(xq, sx.reshape(-1), w8[c], s8[c], offs)
+
+                def bf16(c):
+                    return torch._grouped_mm(x, wb[c].transpose(-2, -1), offs=offs)
+
+                n = int(offs[-1])
+                y = ours(0)[:n]
+                y_loop = []
+                loop(0, y_loop)
+                y_loop = torch.cat(y_loop)
+                rec["vs_select_linear"] = "identical" if torch.equal(y.view(torch.int16), y_loop.view(torch.int16)) \
+                    else sqnr_db(y_loop, y)
+                rec["sqnr_vs_bf16_db"] = sqnr_db(bf16(0)[:n], y)
+                rounds = 1 if T >= 2048 else None
+                for key, fn, cp in (("ours", ours, copies), ("expert_loop", loop, copies), ("fp8", fp8, copies),
+                                    ("bf16", bf16, copies_bf16)):
+                    us = time_graph(fn, cp, a.replays, rounds)
+                    rec[f"{key}_us"] = round(us, 2)
+                    rec[f"{key}_GBps"] = round(need / us * 1e-3, 1)
+                print(json.dumps(rec), flush=True)
+                lines.append(rec)
+        del wm, ws, w8, s8, wb
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4", "fp8wo", "int8wo", "int8", "fp8_blockwise"], default="fp8")
+    ap.add_argument("--fmt", choices=["fp8", "nvfp4", "int4", "fp8wo", "int8wo", "int8", "fp8_blockwise", "mxfp8", "mxfp4"],
+                    default="fp8")
     ap.add_argument("--group-size", type=int, choices=[32, 64, 128, 256], default=32)
     ap.add_argument("--replays", type=int, default=20)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--prologue", action="store_true", help="mxfp8 / mxfp4: the activation prologue alone (PDL off)")
     a = ap.parse_args()
+    if a.prologue:
+        os.environ["AO_B200_NO_PDL"] = "1"   # read once, when the library first launches
     import torch
     import torch.nn.functional as F
 
@@ -585,6 +729,8 @@ def main():
         measure_int8(a, ops, dev, lines)
     if a.fmt == "fp8_blockwise":
         measure_fp8_blockwise(a, ops, dev, lines)
+    if a.fmt in ("mxfp8", "mxfp4"):
+        (measure_mx_prologue if a.prologue else measure_mx)(a, ops, dev, lines)
     info = dict(card=card(), torch=torch.__version__)
     print(json.dumps(info), flush=True)
     if a.out:
