@@ -119,6 +119,77 @@ struct F8StaticFmt : SsFmt<KIND_F8> {
   static constexpr int EPI = tsg::EPI_F8_STATIC;
 };
 
+// Rowwise e4m3 expert weights stored [E, K, N] (N-major: torch.bmm(x, w) on Llama-4-style experts), under the grouped
+// schedule only: the operands, wgmmas, promotion and EPI_F8 epilogue of SsFmt<KIND_F8>, with w_scale [E, N].  A stage
+// holds a [128 k][128 n] box of a 3-D map over [E, K, N] (128-byte swizzle): k past K and n past N are zero-filled,
+// never read from the next expert.  Each consumer warpgroup transposes its 64 n of it into the K-major 128-byte-swizzled
+// [64 n][128 k] layout SsFmt::mma reads (W_XPOSE_BYTES, ts_gemm.cuh).
+struct F8NMajorFmt : SsFmt<KIND_F8> {
+  static constexpr int W_XPOSE_BYTES = ROWS * KCHUNK;   // 8 KiB per consumer warpgroup
+  static int make_maps(const uint8_t* wq, int E, int K, int N, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    const uint64_t dims[3] = {(uint64_t)N, (uint64_t)K, (uint64_t)E};
+    const uint64_t str[2] = {(uint64_t)N, (uint64_t)K * N};
+    const uint32_t box[3] = {ROWS, KCHUNK, 1};
+    if (int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, wq, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))
+      return rc;
+    *tm_aux = *tm_w;
+    return AO_OK;
+  }
+  __device__ static __forceinline__ void issue_w_rows(const CUtensorMap* tm_w, const CUtensorMap*, const tsg::Params& p,
+                                                      uint8_t* w_dst, uint8_t*, uint64_t* bar, int row, int kc,
+                                                      uint64_t policy) {
+    const int e = row / p.N;
+    tma_load_3d(w_dst, tm_w, bar, row - e * p.N, kc * KCHUNK, e, policy);
+  }
+  // Thread t of warpgroup wg: warp w = t / 32 reads the 16 n of column chunk c = 4wg + w, lane (kg = lane % 8, ng =
+  // lane / 8) the 4 n at 16c + 4ng of k rows 16kg .. 16kg + 15, one 32-bit word per row, and stores the 16 k of each of
+  // its 4 n as one 16-byte chunk of that n's row.  Byte (k, n) of the stage is at k*128 + ((n/16) ^ (k%8))*16 + n%16,
+  // byte (n, k) of the buffer at n*128 + ((k/16) ^ (n%8))*16 + k%16.  Word j of a thread is row 16kg + (j ^ kg): the 8
+  // lanes of one ng then read 8 distinct swizzle phases, so each load's 32 words fall in 32 banks, and the 8 lanes of
+  // a quarter-warp store 8 distinct 16-byte chunks of one row.  That load order is undone in the byte transposes: word
+  // (4q + t) ^ kg = 4(q ^ (kg/4)) + (t ^ kg%4), a byte permutation within each 4x4 block (the prmt selectors) and a
+  // swap of neighbouring blocks (kg >= 4).
+  __device__ static __forceinline__ void xpose(uint32_t src, uint32_t dst, int wg, int t) {
+    const int w = t >> 5, lane = t & 31;
+    const int kg = lane & 7, ng = lane >> 3, c = 4 * wg + w;
+    uint32_t r[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int k = 16 * kg + (j ^ kg);
+      r[j] = tsg::lds32(src + k * 128 + ((c ^ (k & 7)) << 4) + 4 * ng);
+    }
+    // stage 2 selectors: byte t of [a0 b0 c0 d0] (0x5410) taken from byte t ^ (kg % 4); [a1 b1 c1 d1] is 0x2222 above
+    const int m = kg & 3;
+    uint32_t s_lo = 0;
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+      const int u = b ^ m;
+      s_lo |= (uint32_t)((u & 1) | ((u & 2) << 1)) << (4 * b);
+    }
+    const uint32_t s_hi = s_lo + 0x2222u;
+    uint32_t o[4][4];   // o[i][q]: the bytes of n 16c + 4ng + i, k 16kg + 4(q ^ (kg/4)) ..
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint32_t lo01 = __byte_perm(r[4 * q], r[4 * q + 1], 0x5140), hi01 = __byte_perm(r[4 * q], r[4 * q + 1], 0x7362);
+      const uint32_t lo23 = __byte_perm(r[4 * q + 2], r[4 * q + 3], 0x5140);
+      const uint32_t hi23 = __byte_perm(r[4 * q + 2], r[4 * q + 3], 0x7362);
+      o[0][q] = __byte_perm(lo01, lo23, s_lo);
+      o[1][q] = __byte_perm(lo01, lo23, s_hi);
+      o[2][q] = __byte_perm(hi01, hi23, s_lo);
+      o[3][q] = __byte_perm(hi01, hi23, s_hi);
+    }
+    const bool swap = kg >= 4;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int n = 16 * w + 4 * ng + i;   // the row within the warpgroup's 64
+      const uint32_t a = dst + wg * (64 * 128) + n * 128 + ((kg ^ (n & 7)) << 4);
+      const uint32_t v0 = swap ? o[i][1] : o[i][0], v1 = swap ? o[i][0] : o[i][1];
+      const uint32_t v2 = swap ? o[i][3] : o[i][2], v3 = swap ? o[i][2] : o[i][3];
+      asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v0), "r"(v1), "r"(v2), "r"(v3) : "memory");
+    }
+  }
+};
+
 // Blockwise e4m3 (Float8DynamicActivationFloat8WeightConfig with PerBlock([1, 128]) activations and PerBlock([128,
 // 128]) weights; reference float8_tensor.py:431-447 and its Triton loop, kernels.py:86-97): the operands, wgmmas and
 // per-chunk promotion of SsFmt<KIND_F8>.  A tile is 128 weight rows and a chunk 128 k, i.e. exactly one weight block
@@ -896,6 +967,53 @@ extern "C" int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale
     p.w_scale = w_scale;
     return Fmt::make_maps(wq, E * N, K, tm_w, tm_aux);
   });
+}
+
+namespace ao {
+namespace lowp {
+// torch.bmm runs as the grouped schedule with B groups of M rows: offs[b] = (b + 1) * M, written on the device (no
+// host copy: a CUDA graph replays it) between the stream-K flags and the partial slots of the workspace.  It waits for
+// the previous kernel first, which may be a batched GEMM still reading the last offs.
+constexpr size_t BMM_OFFS_OFF = streamk::WS_FLAGS_BYTES;
+static_assert(BMM_OFFS_OFF + 4 * tsg::MAX_EXPERTS <= streamk::WS_PARTIAL_OFF, "bmm offs do not fit the workspace");
+__global__ void bmm_offs_kernel(int32_t* offs, int B, int M) {
+  pdl_launch_dependents();
+  pdl_wait();
+  for (int b = threadIdx.x; b < B; b += blockDim.x) offs[b] = (b + 1) * M;
+}
+}  // namespace lowp
+}  // namespace ao
+
+// torch.bmm(x, w) on rowwise e4m3 operands, w a [B, K, N] Float8Tensor: xq [B*M, K] (x's rows, batch-major) with
+// x_scale [B*M], against batch b's weights with w_scale [B, N], y [B*M, N] = bf16(acc * x_scale[m] * w_scale[b, n]),
+// no bias.  w_kn = 0: wq is stored [B, N, K] (K-major, w the transposed view: the grouped kernel of
+// ao_fp8_rowwise_grouped_mm); w_kn = 1: wq is stored [B, K, N] (N-major: F8NMajorFmt, no transposed copy).
+extern "C" int ao_fp8_rowwise_bmm(const uint8_t* xq, const float* x_scale, int B, int M, int K, const uint8_t* wq,
+                                  const float* w_scale, int N, int w_kn, uint16_t* y, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  AO_REQUIRE(B >= 1 && B <= tsg::MAX_EXPERTS, "fp8 bmm: B=%d must be in [1, %d]", B, tsg::MAX_EXPERTS);
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 bmm: bad sizes M=%d K=%d N=%d", M, K, N);
+  AO_REQUIRE((long long)B * M <= 0x7FFFFFFF, "fp8 bmm: B*M=%lld rows exceed the int32 range", (long long)B * M);
+  AO_REQUIRE(K % 16 == 0, "fp8 bmm: K=%d must be a multiple of 16 (TMA row pitch)", K);
+  AO_REQUIRE(N % 16 == 0, "fp8 bmm: N=%d must be a multiple of 16", N);
+  AO_REQUIRE(w_kn == 0 || w_kn == 1, "fp8 bmm: w_kn=%d must be 0 ([B, N, K] weights) or 1 ([B, K, N])", w_kn);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(xq && x_scale && wq && w_scale && y && workspace, "fp8 bmm: null pointer");
+  AO_REQUIRE(workspace_bytes >= streamk::WS_PARTIAL_OFF, "fp8 bmm: workspace too small (%zu bytes)", workspace_bytes);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int32_t* offs = reinterpret_cast<int32_t*>(reinterpret_cast<uint8_t*>(workspace) + lowp::BMM_OFFS_OFF);
+  AO_CUDA_CHECK(ao::launch(lowp::bmm_offs_kernel, dim3(1), dim3(256), 0, st, pdl_enabled(), offs, B, M));
+  auto setup = [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    p.row_scale = x_scale;
+    p.w_scale = w_scale;
+    return w_kn ? lowp::F8NMajorFmt::make_maps(wq, B, K, N, tm_w, tm_aux)
+                : lowp::SsFmt<lowp::KIND_F8>::make_maps(wq, B * N, K, tm_w, tm_aux);
+  };
+  if (w_kn)
+    return tsg::run_grouped<lowp::F8NMajorFmt>("fp8 bmm", xq, B * M, K, B, N, N, offs, y, workspace, workspace_bytes,
+                                               stream, setup);
+  return tsg::run_grouped<lowp::SsFmt<lowp::KIND_F8>>("fp8 bmm", xq, B * M, K, B, N, N, offs, y, workspace,
+                                                      workspace_bytes, stream, setup);
 }
 
 // torch._grouped_mm(x, W.transpose(-2, -1), offs) on blockwise e4m3 operands: expert e's rows [offs[e-1], offs[e]) of

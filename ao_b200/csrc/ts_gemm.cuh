@@ -92,6 +92,18 @@ struct SparseA<F, std::void_t<decltype(F::SPARSE_A)>> {
   static constexpr bool value = F::SPARSE_A;
 };
 
+// Fmt::W_XPOSE_BYTES (optional, default 0): a PROMOTE format whose stage holds its weights N-major ([128 k][128 n]);
+// e4m3 wgmma reads K-major shared-memory operands only, so each consumer warpgroup transposes its 64 rows of every
+// chunk (Fmt::xpose) into its half of a W_XPOSE_BYTES buffer beside the ring, and its wgmmas read them there
+template <class F, class = void>
+struct WXpose {
+  static constexpr int BYTES = 0;
+};
+template <class F>
+struct WXpose<F, std::void_t<decltype(F::W_XPOSE_BYTES)>> {
+  static constexpr int BYTES = F::W_XPOSE_BYTES;
+};
+
 template <class Fmt, int N_MMA>
 constexpr int ctas_per_sm() { return N_MMA <= 32 && Fmt::DECODE_2CTA && !IsGrouped<Fmt>::value ? 2 : 1; }
 constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 104;   // 128 * 24 + 256 * 104 <= 384 * 80
@@ -217,12 +229,16 @@ struct Cfg {
   static constexpr int AUX_SLOT = (Fmt::AUX_BYTES + 1023) & ~1023;
   static constexpr int STAGE_BYTES = Fmt::W_BYTES + AUX_SLOT + X_BYTES;
   static constexpr int CTAS = ctas_per_sm<Fmt, N_MMA>();
-  // one CTA per SM: a 200 KB ring; two: the CTA's share less its barriers (3 x 8 bytes per stage) and alignment pad
-  static constexpr int STAGES_FIT = CTAS == 1 ? 200 * 1024 / STAGE_BYTES
+  static constexpr int XPOSE_BYTES = WXpose<Fmt>::BYTES;   // after the ring (1024-aligned: stages are 1 KiB multiples)
+  static_assert(XPOSE_BYTES == 0 || CTAS == 1, "the transpose buffer is sized for one CTA per SM");
+  // one CTA per SM: a 200 KB ring (less the transpose buffer); two: the CTA's share less its barriers (3 x 8 bytes per
+  // stage) and alignment pad
+  static constexpr int STAGES_FIT = CTAS == 1 ? (200 * 1024 - XPOSE_BYTES) / STAGE_BYTES
                                               : (SMEM_PER_SM / 2 - SMEM_RESERVED_PER_CTA - 1024) / (STAGE_BYTES + 24);
   static constexpr int STAGES = STAGES_FIT > MAX_STAGES ? MAX_STAGES : STAGES_FIT;
   static_assert(STAGES >= 2, "stage does not fit");
-  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+  static constexpr int XPOSE_OFF = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFF = XPOSE_OFF + XPOSE_BYTES;
   static constexpr int BAR_BYTES = 3 * STAGES * 8;   // wfull, xfull, sempty per stage
   static constexpr size_t SMEM_BYTES = (size_t)BAR_OFF + BAR_BYTES + 1024;   // + the 1024-byte alignment of the base
   static_assert(CTAS * (SMEM_BYTES + SMEM_RESERVED_PER_CTA) <= SMEM_PER_SM, "CTAs per SM do not fit");
@@ -263,6 +279,9 @@ __device__ __forceinline__ uint32_t lds16(uint32_t addr) {
 //   static void issue_w_rows(tm_w, tm_aux, p, w smem dst, aux smem dst, full barrier, row, kc, policy)
 //                                                                  grouped only: the 128 weight rows from `row` of the
 //                                                                  [E * N, K] map of all experts, and their aux tiles
+//                                                                  (row = e * N + n)
+//   W_XPOSE_BYTES: static void xpose(w smem, buffer, wg, t)      thread t < 128 of warpgroup wg: its share of the
+//                                                                  stage's rows 64wg.. into buffer + 64wg rows, K-major
 //   EXPERT_SCALE (grouped EPI_FLOAT only): the epilogue multiplies by out_scale[e] (nvfp4: yes, int4: no scale at all)
 //   SS:  static void mma(acc, w smem, x smem, wg, scale_d)          the 4 k32 wgmmas of a chunk for rows 64wg..
 //   SPARSE_A: mt = meta(p, aux smem, n_tile, kc, row, lane)        the thread's metadata words of the chunk (row: its
@@ -657,13 +676,24 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           // wgmmas go to a fresh accumulator that is added to the fp32 registers here (fp32 accuracy across K).  The
           // format's chunk scales (none for rowwise) are read before the wgmmas, so their loads overlap them, and
           // before the stage goes back
+          uint32_t a_s = w_s;
+          if constexpr (WXpose<Fmt>::BYTES > 0) {
+            // N-major weights: the warpgroup's 64 rows, K-major, into its half of the transpose buffer.  Its wgmmas of
+            // the previous chunk have completed (wait_group 0 below), so none reads the buffer any more.  Its 128
+            // threads' stores (generic proxy), then the proxy fence, then the wgmmas (async proxy) that read them.  The
+            // stage goes back after those wgmmas, long after the loads of the transpose, whose values the stores used
+            a_s = smem_u32(smem + C::XPOSE_OFF);
+            Fmt::xpose(w_s, a_s, wg, threadIdx.x & 127);
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+            fence_proxy_async();
+          }
           mbar_wait(&xfull[s], ph);
           const auto cs = Fmt::template chunk_scales<N_MMA>(p, aux_s, GROUPED ? w_blk : tile_of(i) % p.n_tiles,
                                                             GROUPED ? row0 : (tile_of(i) / p.n_tiles) * N_MMA,
                                                             kc_of(i), lane);
           uint32_t part[NACC];
           wgmma_fence();
-          Fmt::template mma<N_MMA>(part, w_s, x_s, wg, 0u);
+          Fmt::template mma<N_MMA>(part, a_s, x_s, wg, 0u);
           wgmma_commit();
           wgmma_wait<0>();
           wgmma_fence_operand(part);

@@ -8,6 +8,8 @@ a fused ``acc * s_x[m] * s_w[n] + bias -> bf16`` epilogue.
 Blockwise weights (``block_size [128, 128]``, ``PerBlock([1, 128])`` activations) replace the reference's Triton GEMM
 (:431-447) with two launches: the 1x128 quantizer and the blockwise GEMM (DESIGN §2f).
 Without ``act_quant_kwargs`` (Float8WeightOnlyConfig) the linear is one launch: bf16 activations on the e4m3 weights.
+``torch.bmm`` on per-row [B, K, N] weights, stored [B, K, N] or as the transposed view of a stored [B, N, K], replaces
+the reference's mslk batched GEMM (:472-522) without its transposed weight copy (DESIGN §2a).
 """
 from __future__ import annotations
 
@@ -188,6 +190,58 @@ def _weight_only_linear(x, w, bias):
 def _(func, types, args, kwargs):
     input_tensor, weight_tensor, bias = args[0], args[1], args[2] if len(args) > 2 else None
     return _float8_linear_impl(input_tensor, weight_tensor, bias)
+
+
+@implements(aten.bmm.default)
+@implements_torch_function(torch.bmm)
+def _(func, types, args, kwargs):
+    return _float8_bmm_impl(args[0], args[1])
+
+
+def _float8_bmm_impl(x, w):
+    """torch.bmm(x, w) with a per-row Float8Tensor w of shape [B, K, N] (the reference's handler,
+    float8_tensor.py:472-522): x's B*M rows are quantized per row to e4m3, then one batched GEMM computes
+    bf16(acc * x_scale[m] * w_scale[b, n]) with no bias term.  w arrives in one of two layouts, told apart by qdata's
+    strides, both with block_size [1, K, 1] and a scale of B*N values:
+      * the transposed view of a stored [B, N, K] weight (torch.bmm(x, w.transpose(-2, -1))): the grouped e4m3 kernel;
+      * a stored [B, K, N] weight quantized with PerRow(1) (Llama-4 expert layers, torch.bmm(x, w)): an N-major kernel
+        that transposes each weight tile on chip, so no transposed copy of the weights is made.
+    Only bf16 x; the weight-only form, per-tensor or blockwise scales and KernelPreference.TORCH are rejected."""
+    assert isinstance(w, Float8Tensor), (
+        f"Don't expect to reach here with an override other than weight currently, {type(x)} {type(w)}")
+    assert w.kernel_preference != KernelPreference.TORCH, "bmm is not supported for TORCH"
+    kw = w.act_quant_kwargs
+    if kw is None:
+        raise NotImplementedError("bmm only support float8 dynamic activation + float8 weight")
+    if x.dim() != 3 or w.dim() != 3:
+        raise NotImplementedError(f"Float8Tensor bmm: 3-D x and weight only, got {x.dim()}-D x {w.dim()}-D")
+    B, K, N = w.shape
+    if isinstance(kw.granularity, PerBlock) or _is_1_128_128_scaled(w.block_size):
+        raise NotImplementedError(f"Float8Tensor bmm: 128x128 blockwise weights (block_size {list(w.block_size)}) have "
+                                  f"no batched kernel in this engine; quantize the weight with PerRow scales")
+    assert list(w.block_size) == [1, K, 1], "bmm only works for per row weight quantization"
+    assert isinstance(kw.granularity, PerRow), "bmm only works for per row activation quantization"
+    if isinstance(x, TorchAOBaseTensor) or x.dtype != torch.bfloat16:
+        raise NotImplementedError(f"Float8Tensor bmm: bf16 x only, got {type(x).__name__} {x.dtype}")
+    if w.qdata.dtype != torch.float8_e4m3fn or kw.float8_dtype != torch.float8_e4m3fn:
+        raise NotImplementedError("Float8Tensor bmm: e4m3 weights and activations only")
+    if x.shape[0] != B or x.shape[-1] != K:
+        raise ValueError(f"bmm: x {tuple(x.shape)} does not match the weight {tuple(w.shape)}")
+    M = x.shape[1]
+    if M == 0:
+        return x.new_empty(B, 0, N)
+    qd = w.qdata
+    if qd.stride(-2) < qd.stride(-1):      # the transposed view of a stored [B, N, K] weight
+        wq = qd.transpose(-2, -1).contiguous().transpose(-2, -1)
+    elif qd.stride(-1) == 1:               # a stored [B, K, N] weight
+        wq = qd.contiguous()
+    else:
+        raise NotImplementedError(f"Float8Tensor bmm: weight qdata strides {qd.stride()} are neither a stored "
+                                  f"[B, K, N] nor the transposed view of a stored [B, N, K]")
+    xq_t = Float8Tensor.from_hp(x.reshape(-1, K), kw.float8_dtype, kw.granularity, kw.mm_config, kw.hp_value_lb,
+                                kw.hp_value_ub, kw.kernel_preference)
+    return torch.ops.ao_b200.fp8_rowwise_bmm(xq_t.qdata.reshape(B, M, K), xq_t.scale.reshape(-1).float().contiguous(),
+                                             wq, w.scale.reshape(B, N).float().contiguous())
 
 
 @implements(aten.slice.Tensor)

@@ -247,6 +247,15 @@ int ao_fp8_rowwise_grouped_mm(const uint8_t* xq, const float* x_scale, int M, in
                               const uint8_t* wq, const float* w_scale, int E, int N,
                               const int32_t* offs, uint16_t* y, void* workspace,
                               size_t workspace_bytes, void* stream);
+/* Replaces torch.bmm(x, w) on a [B, K, N] rowwise Float8Tensor (float8_tensor.py:472-522, mslk's
+ * f8f8bf16_rowwise_batched on a transposed copy): xq e4m3 [B*M, K] with x_scale [B*M] (per row), batch b's weights
+ * with w_scale [B, N]: y bf16 [B*M, N] = bf16(acc * x_scale[m] * w_scale[b, n]), no bias term.  w_kn = 0: wq is stored
+ * [B, N, K] (w is its transposed view); w_kn = 1: wq is stored [B, K, N], read as it is (no transposed copy).
+ * Two launches: the row ends (b + 1) * M written into the workspace on the device, then the grouped GEMM.
+ * 1 <= B <= 1024, K % 16 == 0, N % 16 == 0.  At M == 0 it returns before reading any pointer. */
+int ao_fp8_rowwise_bmm(const uint8_t* xq, const float* x_scale, int B, int M, int K, const uint8_t* wq,
+                       const float* w_scale, int N, int w_kn, uint16_t* y, void* workspace, size_t workspace_bytes,
+                       void* stream);
 
 /* fp8 e4m3 blockwise: 1x128 activation blocks, 128x128 weight blocks -------------- */
 /* Replaces Float8Tensor.from_hp(x, PerBlock([1, 128])) for activations (_choose_scale_float8 +
