@@ -40,12 +40,15 @@ def pick(values, shape, g):
 
 def lowbit(t):
     """The largest power of two that divides every entry of the fp64 tensor t."""
-    nz = t[t != 0].abs().cpu()   # on the CPU: torch.pow(2.0, e) on CUDA is not exact
+    nz = t[t != 0].abs()
     if nz.numel() == 0:
         return 1.0
     m, e = torch.frexp(nz)
     mi = (m * 2.0**53).to(torch.int64)
-    return float(((mi & -mi).double() * torch.pow(2.0, (e - 53).double())).min())
+    # the lowest set bit of each 53-bit significand, 2^(j - 1) with j its frexp exponent: only integer exponents are
+    # formed on the device (torch.pow on CUDA is not exact), the one power of two on the host
+    j = torch.frexp((mi & -mi).double())[1]
+    return 2.0 ** int((j - 1 + e - 53).min())
 
 
 def pow2(e):
@@ -98,6 +101,16 @@ def recipe(op, acc, scale=None, bias=None):
     else:
         raise ValueError(op)
     return y if bias is None else y + bias
+
+
+def int8_epilogue(acc, x_scale, w_scale, bias=None):
+    """EPI_I8 on exact int32 sums acc (fp64 [M, n]): the reference's order, bf16 between the two scales,
+    bf16(bf16(acc * x_scale[m]) * w_scale[n] + bias[n]) (x_scale f32 [M, 1], w_scale f32 [n], bias bf16 [n] or None);
+    fp64 of the fp32 value before the last rounding."""
+    assert float(acc.abs().max()) < 2.0**24, "premise: int32 sums must convert to fp32 exactly"
+    t = (acc.float() * x_scale).to(torch.bfloat16).float()
+    fp32_exact(t.double() * w_scale.double(), "int8: bf16(acc * x_scale) * w_scale")   # fma == mul then add
+    return (t * w_scale if bias is None else t * w_scale + bias.float()).double()
 
 
 def mxfp4_value(codes, scale_bytes):
@@ -684,12 +697,10 @@ def served(op, M, N, K, seed=0, group_size=32, n_out=None, x_seed=None):
             return wq.double(), wq
 
         def epi(acc, n0, n1):
-            assert float(acc.abs().max()) < 2.0**24, "premise: int32 sums must convert to fp32 exactly"
             if op == "int8_mm_i32":
+                assert float(acc.abs().max()) < 2.0**24, "premise: int32 sums must convert to fp32 exactly"
                 return acc
-            t = (acc.float() * sx).to(torch.bfloat16).float()   # the reference's order: bf16 between the two scales
-            fp32_exact(t.double() * sw[n0:n1].double(), "int8: bf16(acc * x_scale) * w_scale")
-            return (t * sw[n0:n1] + b[n0:n1].float()).double()
+            return int8_epilogue(acc, sx, sw[n0:n1], b[n0:n1])
         ref = _reference(op, xq.double(), N, blocks(N, make), epi, False)
         wq = torch.cat(parts, 0)
         if op == "int8_mm_i32":
