@@ -198,16 +198,15 @@ extern "C" int ao_int4_tilepacked_linear_strided(const uint16_t* x, int ldx, int
                                                  void* workspace, size_t workspace_bytes, int impl,
                                                  void* stream) {
   using namespace ao;
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int4 linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 1024 == 0, "int4 linear: K=%d must be a multiple of 1024 (format pads K)", K);
   AO_REQUIRE(N % 8 == 0, "int4 linear: N=%d must be a multiple of 8", N);
   AO_REQUIRE(N_out > 0 && N_out <= N, "int4 linear: N_out=%d out of range (N=%d)", N_out, N);
   AO_REQUIRE(group_size == 32 || group_size == 64 || group_size == 128 || group_size == 256,
              "int4 linear: group_size=%d not in {32,64,128,256}", group_size);
-  AO_REQUIRE(ldx >= K && ldx % 8 == 0, "int4 linear: ldx=%d must be >= K=%d and a multiple of 8", ldx, K);
+  tsg::Params p{};
+  if (int rc = tsg::dense_params(p, "int4 linear", "x", x, ldx, M, K, N, N_out, bias, y)) return rc;
   if (M == 0) return AO_OK;
-  AO_REQUIRE(x && qdata && scale_and_zero && y, "int4 linear: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "int4 linear: x must be 16-byte aligned");
+  AO_REQUIRE(qdata && scale_and_zero, "int4 linear: null pointer");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (impl == 2) {
     constexpr int MT = 8;
@@ -221,10 +220,7 @@ extern "C" int ao_int4_tilepacked_linear_strided(const uint16_t* x, int ldx, int
   }
   CUtensorMap tm_w, tm_sz;
   if (int rc = int4k::Int4Fmt::make_maps(qdata, scale_and_zero, N, K, group_size, &tm_w, &tm_sz)) return rc;
-  tsg::Params p{};
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.M = M; p.N = N; p.N_out = N_out; p.K = K; p.group_size = group_size;
+  p.group_size = group_size;
   return tsg::run<int4k::Int4Fmt>(p, tm_w, tm_sz, x, ldx, workspace, workspace_bytes, "int4 linear", st);
 }
 

@@ -727,35 +727,25 @@ __global__ void __launch_bounds__(256) dequant_act_kernel(const uint8_t* __restr
   dst[1] = reinterpret_cast<const uint4*>(o)[1];
 }
 
-// int8 / fp8 rowwise
-template <int KIND>
-static int rowwise(const uint8_t* xq, const float* x_scale, int M, int K, const uint8_t* wq, const float* w_scale, int N,
-                   const uint16_t* bias, uint16_t* y, int32_t* i32_out, void* ws, size_t ws_bytes, void* stream) {
-  using Fmt = SsFmt<KIND>;
-  CUtensorMap tm_w, tm_aux;
-  if (int rc = Fmt::make_maps(wq, N, K, &tm_w, &tm_aux)) return rc;
-  tsg::Params p{};
-  p.row_scale = x_scale;
-  p.w_scale = w_scale;
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.i32_out = i32_out;
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<Fmt>(p, tm_w, tm_aux, xq, K, ws, ws_bytes, "lowp linear", reinterpret_cast<cudaStream_t>(stream));
-}
-
 // mxfp8 / nvfp4: activation slabs dequantised into the workspace behind the partial slots, one GEMM per slab
 template <int KIND>
-static int block_scaled(const uint8_t* xq, const uint8_t* x_sf, const float* a_pts, int M, int K, const uint8_t* wq,
-                        const uint8_t* w_sf, const float* b_pts, int N, const uint16_t* bias, uint16_t* y, void* ws,
-                        size_t ws_bytes, void* stream) {
+static int block_scaled(const char* what, const uint8_t* xq, const uint8_t* x_sf, const float* a_pts, int M, int K,
+                        const uint8_t* wq, const uint8_t* w_sf, const float* b_pts, int N, const uint16_t* bias,
+                        uint16_t* y, void* ws, size_t ws_bytes, void* stream) {
   using Fmt = std::conditional_t<KIND == KIND_NVF4, nvf4w::Nvfp4Fmt,
                                  std::conditional_t<KIND == KIND_MXF4, Mxfp4Fmt, Mxfp8Fmt>>;
+  tsg::Params p{};
+  if (int rc = tsg::dense_params(p, what, "xq", xq, K, M, K, N, N, bias, y)) return rc;
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x_sf && wq && w_sf, "%s: null pointer", what);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int sf_per_row = KIND == KIND_NVF4 ? K / 16 : K / 32;
   const int sf_col_blocks = ceil_div(sf_per_row, 4);
   CUtensorMap tm_w, tm_sf;
   if (int rc = Fmt::make_maps(wq, w_sf, N, K, &tm_w, &tm_sf)) return rc;
+  p.out_scale = KIND == KIND_NVF4 ? b_pts : nullptr;
+  p.out_scale2 = KIND == KIND_NVF4 ? a_pts : nullptr;
+  p.aux_col_blocks = sf_col_blocks;
   // the partial slots take at most (SMs x 128 x 128) words; the slab starts on the next MiB (restated by
   // tests/test_exact_gemm_gpu.py::test_block_scaled_activation_slabs, which sizes workspaces to given slab heights)
   const size_t act_off = (streamk::WS_PARTIAL_OFF + (size_t)sm_count() * ROWS * 128 * 4 + (1u << 20) - 1) & ~(size_t)((1u << 20) - 1);
@@ -770,14 +760,10 @@ static int block_scaled(const uint8_t* xq, const uint8_t* x_sf, const float* a_p
     const long long threads = (long long)rows * (K / 16);
     AO_CUDA_CHECK(ao::launch(dequant_act_kernel<KIND>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st,
                              pdl_enabled(), xq, x_sf, m0, rows, K, sf_col_blocks, xb));
-    tsg::Params p{};
-    p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-    p.y = reinterpret_cast<__nv_bfloat16*>(y) + (size_t)m0 * N;
-    p.out_scale = KIND == KIND_NVF4 ? b_pts : nullptr;
-    p.out_scale2 = KIND == KIND_NVF4 ? a_pts : nullptr;
-    p.aux_col_blocks = sf_col_blocks;
-    p.M = rows; p.N = N; p.N_out = N; p.K = K;
-    if (int rc = tsg::run<Fmt>(p, tm_w, tm_sf, xb, K, ws, act_off, "lowp linear", st)) return rc;
+    tsg::Params ps = p;
+    ps.y = p.y + (size_t)m0 * N;
+    ps.M = rows;
+    if (int rc = tsg::run<Fmt>(ps, tm_w, tm_sf, xb, K, ws, act_off, what, st)) return rc;
   }
   return AO_OK;
 }
@@ -791,24 +777,29 @@ extern "C" int ao_int8_dyn_linear(const int8_t* xq, const float* x_scale, int M,
                                   const int8_t* wq, const float* w_scale, int N,
                                   const uint16_t* bias, uint16_t* y, void* workspace,
                                   size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int8 linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 16 == 0, "int8 linear: K=%d must be a multiple of 16 (TMA row pitch)", K);
   AO_REQUIRE(N % 8 == 0, "int8 linear: N=%d must be a multiple of 8 (reference: int8/kernels.py:48-58)", N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale && wq && w_scale && y, "int8 linear: null pointer");
-  return lowp::rowwise<lowp::KIND_I8>(reinterpret_cast<const uint8_t*>(xq), x_scale, M, K,
-                                      reinterpret_cast<const uint8_t*>(wq), w_scale, N, bias, y, nullptr, workspace,
-                                      workspace_bytes, stream);
+  using Fmt = lowp::SsFmt<lowp::KIND_I8>;
+  return tsg::run_dense<Fmt>("int8 linear", "xq", xq, K, M, K, N, N, bias, y, workspace, workspace_bytes, stream,
+                             [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(x_scale && wq && w_scale, "int8 linear: null pointer");
+    p.row_scale = x_scale;
+    p.w_scale = w_scale;
+    return Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), N, K, tm_w, tm_aux);
+  });
 }
 
 extern "C" int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, int N, int32_t* acc,
                               void* workspace, size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0 && K % 16 == 0, "int8 mm: bad sizes M=%d K=%d N=%d (K%%16==0)", M, K, N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && wq && acc, "int8 mm: null pointer");
-  return lowp::rowwise<lowp::KIND_I8>(reinterpret_cast<const uint8_t*>(xq), nullptr, M, K,
-                                      reinterpret_cast<const uint8_t*>(wq), nullptr, N, nullptr, nullptr, acc, workspace,
-                                      workspace_bytes, stream);
+  AO_REQUIRE(K % 16 == 0, "int8 mm: K=%d must be a multiple of 16 (TMA row pitch)", K);
+  using Fmt = lowp::SsFmt<lowp::KIND_I8>;
+  return tsg::run_dense<Fmt>("int8 mm", "xq", xq, K, M, K, N, N, nullptr, acc, workspace, workspace_bytes, stream,
+                             [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(wq, "int8 mm: null pointer");
+    p.i32_out = acc;   // the raw s32 sums instead of y
+    p.y = nullptr;
+    return Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), N, K, tm_w, tm_aux);
+  });
 }
 
 // F.linear(x, Int8Tensor without act_quant_kwargs), per-row or per-tensor scale (int8_tensor.py:336-359):
@@ -816,21 +807,14 @@ extern "C" int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, 
 extern "C" int ao_int8_weight_linear(const uint16_t* x, int ldx, int M, int K, const int8_t* wq, const float* w_scale,
                                      int N, const uint16_t* bias, uint16_t* y, void* workspace,
                                      size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "int8 weight linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 16 == 0, "int8 weight linear: K=%d must be a multiple of 16 (TMA row pitch)", K);
-  AO_REQUIRE(ldx >= K && ldx % 8 == 0, "int8 weight linear: ldx=%d must be >= K=%d and a multiple of 8", ldx, K);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(x && wq && w_scale && y, "int8 weight linear: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "int8 weight linear: x must be 16-byte aligned");
-  CUtensorMap tm_w, tm_aux;
-  if (int rc = lowp::Int8WoFmt::make_maps(reinterpret_cast<const uint8_t*>(wq), N, K, &tm_w, &tm_aux)) return rc;
-  tsg::Params p{};
-  p.w_scale = w_scale;
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<lowp::Int8WoFmt>(p, tm_w, tm_aux, x, ldx, workspace, workspace_bytes, "int8 weight linear",
-                                   reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::Int8WoFmt;
+  return tsg::run_dense<Fmt>("int8 weight linear", "x", x, ldx, M, K, N, N, bias, y, workspace, workspace_bytes, stream,
+                             [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(wq && w_scale, "int8 weight linear: null pointer");
+    p.w_scale = w_scale;
+    return Fmt::make_maps(reinterpret_cast<const uint8_t*>(wq), N, K, tm_w, tm_aux);
+  });
 }
 
 // F.linear(x, Float8Tensor without act_quant_kwargs), per-row or per-tensor scale (float8_tensor.py:459-469):
@@ -838,35 +822,31 @@ extern "C" int ao_int8_weight_linear(const uint16_t* x, int ldx, int M, int K, c
 extern "C" int ao_fp8_weight_linear(const uint16_t* x, int ldx, int M, int K, const uint8_t* wq, const float* w_scale,
                                     int N, const uint16_t* bias, uint16_t* y, void* workspace,
                                     size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 weight linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 16 == 0, "fp8 weight linear: K=%d must be a multiple of 16 (TMA row pitch)", K);
-  AO_REQUIRE(ldx >= K && ldx % 8 == 0, "fp8 weight linear: ldx=%d must be >= K=%d and a multiple of 8", ldx, K);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(x && wq && w_scale && y, "fp8 weight linear: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "fp8 weight linear: x must be 16-byte aligned");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(w_scale) & 15) == 0,
-             "fp8 weight linear: w_scale must be 16-byte aligned (it is loaded by TMA)");
-  CUtensorMap tm_w, tm_s;
-  if (int rc = lowp::Fp8WoFmt::make_maps(wq, w_scale, N, K, &tm_w, &tm_s)) return rc;
-  tsg::Params p{};
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<lowp::Fp8WoFmt>(p, tm_w, tm_s, x, ldx, workspace, workspace_bytes, "fp8 weight linear",
-                                  reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::Fp8WoFmt;
+  return tsg::run_dense<Fmt>("fp8 weight linear", "x", x, ldx, M, K, N, N, bias, y, workspace, workspace_bytes, stream,
+                             [&](tsg::Params&, CUtensorMap* tm_w, CUtensorMap* tm_s) {
+    AO_REQUIRE(wq && w_scale, "fp8 weight linear: null pointer");
+    AO_REQUIRE((reinterpret_cast<uintptr_t>(w_scale) & 15) == 0,
+               "fp8 weight linear: w_scale must be 16-byte aligned (it is loaded by TMA)");
+    return Fmt::make_maps(wq, w_scale, N, K, tm_w, tm_s);
+  });
 }
 
 extern "C" int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, int M, int K,
                                      const uint8_t* wq, const float* w_scale, int N,
                                      const uint16_t* bias, uint16_t* y, void* workspace,
                                      size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 16 == 0, "fp8 linear: K=%d must be a multiple of 16 (reference: quantization/utils.py:663-687)", K);
   AO_REQUIRE(N % 16 == 0, "fp8 linear: N=%d must be a multiple of 16 (reference: quantization/utils.py:663-687)", N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale && wq && w_scale && y, "fp8 linear: null pointer");
-  return lowp::rowwise<lowp::KIND_F8>(xq, x_scale, M, K, wq, w_scale, N, bias, y, nullptr, workspace, workspace_bytes,
-                                      stream);
+  using Fmt = lowp::SsFmt<lowp::KIND_F8>;
+  return tsg::run_dense<Fmt>("fp8 linear", "xq", xq, K, M, K, N, N, bias, y, workspace, workspace_bytes, stream,
+                             [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(x_scale && wq && w_scale, "fp8 linear: null pointer");
+    p.row_scale = x_scale;
+    p.w_scale = w_scale;
+    return Fmt::make_maps(wq, N, K, tm_w, tm_aux);
+  });
 }
 
 // F.linear(x, PrototypeFloat8Tensor) (prototype_float8_tensor.py:329-474) on the static quantizer's codes: the output of
@@ -877,24 +857,18 @@ extern "C" int ao_fp8_static_linear(const uint8_t* xq, const float* x_scale, int
                                     const float* w_scale, int w_scale_per_row, int N, const uint16_t* bias,
                                     const float* out_scale, int out_scale_per_row, uint16_t* y, void* workspace,
                                     size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 static linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 16 == 0, "fp8 static linear: K=%d must be a multiple of 16 (reference: quantization/utils.py:663-687)", K);
   AO_REQUIRE(N % 16 == 0, "fp8 static linear: N=%d must be a multiple of 16 (reference: quantization/utils.py:663-687)", N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale && wq && w_scale && y, "fp8 static linear: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(xq) & 15) == 0, "fp8 static linear: xq must be 16-byte aligned");
-  CUtensorMap tm_w, tm_aux;
-  if (int rc = lowp::F8StaticFmt::make_maps(wq, N, K, &tm_w, &tm_aux)) return rc;
-  tsg::Params p{};
-  p.row_scale = x_scale;
-  p.w_scale = w_scale;
-  p.out_scale = out_scale;
-  p.out_scale_per_row = (out_scale_per_row ? tsg::F8S_OUT_PER_TOKEN : 0) | (w_scale_per_row ? 0 : tsg::F8S_W_PER_TENSOR);
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<lowp::F8StaticFmt>(p, tm_w, tm_aux, xq, K, workspace, workspace_bytes, "fp8 static linear",
-                                     reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::F8StaticFmt;
+  return tsg::run_dense<Fmt>("fp8 static linear", "xq", xq, K, M, K, N, N, bias, y, workspace, workspace_bytes, stream,
+                             [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(x_scale && wq && w_scale, "fp8 static linear: null pointer");
+    p.row_scale = x_scale;
+    p.w_scale = w_scale;
+    p.out_scale = out_scale;
+    p.out_scale_per_row = (out_scale_per_row ? tsg::F8S_OUT_PER_TOKEN : 0) | (w_scale_per_row ? 0 : tsg::F8S_W_PER_TENSOR);
+    return Fmt::make_maps(wq, N, K, tm_w, tm_aux);
+  });
 }
 
 // F.linear(x, Float8Tensor with 128x128 weight blocks and 1x128 activation blocks) (float8_tensor.py:431-447):
@@ -903,23 +877,17 @@ extern "C" int ao_fp8_static_linear(const uint8_t* xq, const float* x_scale, int
 extern "C" int ao_fp8_blockwise_linear(const uint8_t* xq, const float* x_scale_t, int M, int K, const uint8_t* wq,
                                        const float* w_scale, int N, const uint16_t* bias, uint16_t* y, void* workspace,
                                        size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 blockwise linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 128 == 0, "fp8 blockwise linear: K=%d must be a multiple of 128 (one scale per 128 k)", K);
   AO_REQUIRE(N % 128 == 0, "fp8 blockwise linear: N=%d must be a multiple of 128 (one scale per 128 rows)", N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale_t && wq && w_scale && y, "fp8 blockwise linear: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(xq) & 15) == 0, "fp8 blockwise linear: xq must be 16-byte aligned");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x_scale_t) & 15) == 0,
-             "fp8 blockwise linear: x_scale must be 16-byte aligned (it is loaded by TMA)");
-  CUtensorMap tm_w, tm_xs;
-  if (int rc = lowp::BlockwiseF8Fmt::make_maps(wq, x_scale_t, M, N, K, &tm_w, &tm_xs)) return rc;
-  tsg::Params p{};
-  p.w_scale = w_scale;
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<lowp::BlockwiseF8Fmt>(p, tm_w, tm_xs, xq, K, workspace, workspace_bytes, "fp8 blockwise linear",
-                                        reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::BlockwiseF8Fmt;
+  return tsg::run_dense<Fmt>("fp8 blockwise linear", "xq", xq, K, M, K, N, N, bias, y, workspace, workspace_bytes,
+                             stream, [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_xs) {
+    AO_REQUIRE(x_scale_t && wq && w_scale, "fp8 blockwise linear: null pointer");
+    AO_REQUIRE((reinterpret_cast<uintptr_t>(x_scale_t) & 15) == 0,
+               "fp8 blockwise linear: x_scale must be 16-byte aligned (it is loaded by TMA)");
+    p.w_scale = w_scale;
+    return Fmt::make_maps(wq, x_scale_t, M, N, K, tm_w, tm_xs);
+  });
 }
 
 // F.linear(x, Float8Sparse2x4_2DData2DMetadataTensor) (float8_sparse_2x4_2d_data_2d_metadata_tensor.py): per-token
@@ -929,25 +897,19 @@ extern "C" int ao_fp8_blockwise_linear(const uint8_t* xq, const float* x_scale_t
 extern "C" int ao_fp8_sparse_linear(const uint8_t* xq, const float* x_scale, int M, int K, const uint8_t* wq,
                                     const uint8_t* w_meta, const float* w_scale, int N, const uint16_t* bias, uint16_t* y,
                                     void* workspace, size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "fp8 sparse linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 32 == 0, "fp8 sparse linear: K=%d must be a multiple of 32 (16-byte rows of compressed codes)", K);
   AO_REQUIRE(N % 16 == 0, "fp8 sparse linear: N=%d must be a multiple of 16", N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale && wq && w_meta && w_scale && y, "fp8 sparse linear: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(xq) & 15) == 0, "fp8 sparse linear: xq must be 16-byte aligned");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(wq) & 15) == 0, "fp8 sparse linear: wq must be 16-byte aligned");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(w_meta) & 15) == 0,
-             "fp8 sparse linear: w_meta must be 16-byte aligned (it is loaded by TMA)");
-  CUtensorMap tm_w, tm_m;
-  if (int rc = lowp::SparseF8Fmt::make_maps(wq, w_meta, N, K, &tm_w, &tm_m)) return rc;
-  tsg::Params p{};
-  p.row_scale = x_scale;
-  p.w_scale = w_scale;
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<lowp::SparseF8Fmt>(p, tm_w, tm_m, xq, K, workspace, workspace_bytes, "fp8 sparse linear",
-                                     reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = lowp::SparseF8Fmt;
+  return tsg::run_dense<Fmt>("fp8 sparse linear", "xq", xq, K, M, K, N, N, bias, y, workspace, workspace_bytes, stream,
+                             [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_m) {
+    AO_REQUIRE(x_scale && wq && w_meta && w_scale, "fp8 sparse linear: null pointer");
+    AO_REQUIRE((reinterpret_cast<uintptr_t>(wq) & 15) == 0, "fp8 sparse linear: wq must be 16-byte aligned");
+    AO_REQUIRE((reinterpret_cast<uintptr_t>(w_meta) & 15) == 0,
+               "fp8 sparse linear: w_meta must be 16-byte aligned (it is loaded by TMA)");
+    p.row_scale = x_scale;
+    p.w_scale = w_scale;
+    return Fmt::make_maps(wq, w_meta, N, K, tm_w, tm_m);
+  });
 }
 
 // torch._grouped_mm(x, W.transpose(-2, -1), offs) on rowwise e4m3 operands: expert e's rows [offs[e-1], offs[e]) of
@@ -1097,38 +1059,29 @@ extern "C" int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked
                                const uint8_t* wq, const uint8_t* w_scale_blocked, int N,
                                const uint16_t* bias, uint16_t* y, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "mxfp8 linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 32 == 0, "mxfp8 linear: K=%d must be a multiple of 32 (mx_tensor.py:244-246)", K);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale_blocked && wq && w_scale_blocked && y, "mxfp8 linear: null pointer");
-  return lowp::block_scaled<lowp::KIND_MXF8>(xq, x_scale_blocked, nullptr, M, K, wq, w_scale_blocked, nullptr, N, bias,
-                                             y, workspace, workspace_bytes, stream);
+  return lowp::block_scaled<lowp::KIND_MXF8>("mxfp8 linear", xq, x_scale_blocked, nullptr, M, K, wq, w_scale_blocked,
+                                             nullptr, N, bias, y, workspace, workspace_bytes, stream);
 }
 
 extern "C" int ao_mxfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,
                                const uint8_t* wq, const uint8_t* w_scale_blocked, int N,
                                const uint16_t* bias, uint16_t* y, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "mxfp4 linear: bad sizes M=%d K=%d N=%d", M, K, N);
   // K / 2 bytes per weight row: a multiple of 16, the TMA row pitch; a K tail of the last chunk is zero-filled
   AO_REQUIRE(K % 32 == 0, "mxfp4 linear: K=%d must be a multiple of 32 (mx_tensor.py:244-246)", K);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale_blocked && wq && w_scale_blocked && y, "mxfp4 linear: null pointer");
-  return lowp::block_scaled<lowp::KIND_MXF4>(xq, x_scale_blocked, nullptr, M, K, wq, w_scale_blocked, nullptr, N, bias,
-                                             y, workspace, workspace_bytes, stream);
+  return lowp::block_scaled<lowp::KIND_MXF4>("mxfp4 linear", xq, x_scale_blocked, nullptr, M, K, wq, w_scale_blocked,
+                                             nullptr, N, bias, y, workspace, workspace_bytes, stream);
 }
 
 extern "C" int ao_nvfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, const float* a_pts,
                                int M, int K, const uint8_t* wq, const uint8_t* w_scale_blocked,
                                const float* b_pts, int N, const uint16_t* bias, uint16_t* y,
                                void* workspace, size_t workspace_bytes, void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "nvfp4 linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 256 == 0, "nvfp4 linear: K=%d must be a multiple of 256", K);
   AO_REQUIRE(N % 16 == 0, "nvfp4 linear: N=%d must be a multiple of 16 (inference_workflow.py:248-251)", N);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(xq && x_scale_blocked && wq && w_scale_blocked && y, "nvfp4 linear: null pointer");
-  return lowp::block_scaled<lowp::KIND_NVF4>(xq, x_scale_blocked, a_pts, M, K, wq, w_scale_blocked, b_pts, N, bias, y,
-                                             workspace, workspace_bytes, stream);
+  return lowp::block_scaled<lowp::KIND_NVF4>("nvfp4 linear", xq, x_scale_blocked, a_pts, M, K, wq, w_scale_blocked,
+                                             b_pts, N, bias, y, workspace, workspace_bytes, stream);
 }
 
 // nvfp4 weights x bf16 activations = F.linear(x, NVFP4Tensor.dequantize()) (nvfp4_tensor.py:199-231, weight-only
@@ -1139,25 +1092,18 @@ extern "C" int ao_nvfp4_weight_linear_ex(const uint16_t* x, int ldx, const float
                                          const uint8_t* w_scale_blocked, const float* b_pts, int b_pts_per_row, int N,
                                          const uint16_t* bias, uint16_t* y, void* workspace, size_t workspace_bytes,
                                          void* stream) {
-  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "nvfp4 weight linear: bad sizes M=%d K=%d N=%d", M, K, N);
   AO_REQUIRE(K % 128 == 0, "nvfp4 weight linear: K=%d must be a multiple of 128", K);
   AO_REQUIRE(N % 16 == 0, "nvfp4 weight linear: N=%d must be a multiple of 16 (inference_workflow.py:248-251)", N);
-  AO_REQUIRE(ldx >= K && ldx % 8 == 0, "nvfp4 weight linear: ldx=%d must be >= K=%d and a multiple of 8", ldx, K);
-  if (M == 0) return AO_OK;
-  AO_REQUIRE(x && wq && w_scale_blocked && y, "nvfp4 weight linear: null pointer");
-  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "nvfp4 weight linear: x must be 16-byte aligned");
-  CUtensorMap tm_w, tm_sf;
-  if (int rc = nvf4w::Nvfp4Fmt::make_maps(wq, w_scale_blocked, N, K, &tm_w, &tm_sf)) return rc;
-  tsg::Params p{};
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  p.row_scale = x_scale;
-  p.out_scale = b_pts;
-  p.out_scale_per_row = b_pts_per_row;
-  p.y = reinterpret_cast<__nv_bfloat16*>(y);
-  p.aux_col_blocks = ceil_div(K / 16, 4);
-  p.M = M; p.N = N; p.N_out = N; p.K = K;
-  return tsg::run<nvf4w::Nvfp4Fmt>(p, tm_w, tm_sf, x, ldx, workspace, workspace_bytes, "nvfp4 weight linear",
-                                   reinterpret_cast<cudaStream_t>(stream));
+  using Fmt = nvf4w::Nvfp4Fmt;
+  return tsg::run_dense<Fmt>("nvfp4 weight linear", "x", x, ldx, M, K, N, N, bias, y, workspace, workspace_bytes,
+                             stream, [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_sf) {
+    AO_REQUIRE(wq && w_scale_blocked, "nvfp4 weight linear: null pointer");
+    p.row_scale = x_scale;
+    p.out_scale = b_pts;
+    p.out_scale_per_row = b_pts_per_row;
+    p.aux_col_blocks = ceil_div(K / 16, 4);
+    return Fmt::make_maps(wq, w_scale_blocked, N, K, tm_w, tm_sf);
+  });
 }
 
 extern "C" int ao_nvfp4_weight_linear(const uint16_t* x, const float* x_scale, int M, int K, const uint8_t* wq,

@@ -50,6 +50,46 @@ void check_cuda(const Tensor& t, const char* name) {
 const uint16_t* bf16_ptr(const Tensor& t) { return reinterpret_cast<const uint16_t*>(t.data_ptr()); }
 uint16_t* bf16_ptr_mut(Tensor& t) { return reinterpret_cast<uint16_t*>(t.data_ptr()); }
 
+// t, or a copy of it when it does not start on 16 bytes (TMA boxes and the kernels' vector loads need that start)
+Tensor aligned16(const Tensor& t) { return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0 ? t : t.clone(); }
+
+const uint16_t* opt_bias(const c10::optional<Tensor>& bias, int64_t n, Tensor& keep) {
+  if (bias.has_value() && bias->defined()) {
+    keep = bias->to(at::kBFloat16).contiguous();
+    TORCH_CHECK(keep.numel() == n, "ao_b200: bias must have N elements");
+    return bf16_ptr(keep);
+  }
+  return nullptr;
+}
+
+// bf16 activations may be row-strided (a column slice of a wider buffer); returns the row pitch in elements
+int64_t check_rows(const Tensor& x, const char* name) {
+  TORCH_CHECK(x.is_cuda(), "ao_b200: ", name, " must be a CUDA tensor");
+  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2, "ao_b200: ", name, " must be bf16 [M, K]");
+  TORCH_CHECK(x.size(1) <= 1 || x.stride(1) == 1, "ao_b200: ", name, " must have unit inner stride");
+  TORCH_CHECK(x.size(0) <= 1 || (x.stride(0) >= x.size(1) && x.stride(0) % 8 == 0), "ao_b200: the row pitch of ", name,
+              " must be >= K and a multiple of 8 elements");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "ao_b200: ", name, " must be 16-byte aligned");
+  return x.size(0) > 1 ? x.stride(0) : x.size(1);
+}
+
+// A dense linear as every such op runs it once it has checked its own operands and allocated y [M, n_out] through its
+// Meta kernel.  The activation x [M, K] has passed one of two rules: bf16 rows check_rows (strided rows keep their
+// pitch, a start off 16 bytes is rejected); quantized codes check_cuda (contiguous), and codes that do not start on 16
+// bytes are copied here.  launch(x, ldx, bias, y, ws, ws_bytes) makes the op's C call; without rows there is none.
+template <class Launch>
+Tensor dense_linear(const Tensor& x, const c10::optional<Tensor>& bias, Tensor y, Launch launch) {
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor keep;
+  const uint16_t* b = opt_bias(bias, y.size(1), keep);
+  if (x.size(0) == 0) return y;
+  const Tensor xc = aligned16(x);
+  const int64_t ldx = xc.size(0) > 1 ? xc.stride(0) : xc.size(1);
+  Tensor ws = workspace_for(x);
+  launch(xc.data_ptr(), (int)ldx, b, y.data_ptr(), ws.data_ptr(), (size_t)ws.numel());
+  return y;
+}
+
 // torch._grouped_mm(x, W.transpose(-2, -1), offs), 2-D x 3-D, as every grouped op runs it once it has checked its own
 // operands: x [M, K] on the GPU, w the experts' weights [E, ...], offs int32 [E] on x's device (cumulative row ends,
 // never read on the host) -> y [M, n_out] bf16.  The kernels read dense rows from a 16-byte aligned start, so an x
@@ -65,8 +105,7 @@ Tensor grouped_mm(const Tensor& x, const char* name, const Tensor& w, const Tens
   c10::cuda::CUDAGuard guard(x.device());
   Tensor y = at::empty({x.size(0), n_out}, x.options().dtype(at::kBFloat16));
   if (x.size(0) == 0) return y;
-  Tensor xc = x.contiguous();
-  if (reinterpret_cast<uintptr_t>(xc.data_ptr()) % 16 != 0) xc = xc.clone();
+  const Tensor xc = aligned16(x.contiguous());
   Tensor ws = workspace_for(x);
   launch(xc.data_ptr(), bf16_ptr_mut(y), ws.data_ptr(), (size_t)ws.numel());
   return y;
@@ -129,40 +168,28 @@ std::tuple<Tensor, Tensor, Tensor> int4_hqq_quantize_meta(const Tensor& w, int64
 }
 
 // x [M, K] bf16 -> y [M, n_out] bf16  (aten._weight_int4pack_mm + bias + out-feature slice)
+Tensor int4_tilepacked_linear_meta(const Tensor& x, const Tensor& qdata, int64_t, const Tensor&,
+                                   const c10::optional<Tensor>&, int64_t n_out, int64_t) {
+  if (n_out <= 0) n_out = qdata.size(0) * 8;
+  return at::empty({x.size(0), n_out}, x.options());
+}
 Tensor int4_tilepacked_linear(const Tensor& x, const Tensor& qdata, int64_t group_size,
                               const Tensor& scale_and_zero, const c10::optional<Tensor>& bias,
                               int64_t n_out, int64_t impl) {
-  TORCH_CHECK(x.is_cuda(), "ao_b200: x must be a CUDA tensor");
+  check_rows(x, "x");
   check_cuda(qdata, "qdata");
   check_cuda(scale_and_zero, "scale_and_zero");
-  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2, "ao_b200: x must be bf16 [M, K]");
-  // rows may be strided (a column slice of a wider buffer): the TMA descriptor carries the pitch
-  TORCH_CHECK(x.size(1) <= 1 || x.stride(1) == 1, "ao_b200: x must have unit inner stride");
-  TORCH_CHECK(x.size(0) <= 1 || (x.stride(0) >= x.size(1) && x.stride(0) % 8 == 0),
-              "ao_b200: the row pitch of x must be >= K and a multiple of 8 elements");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "ao_b200: x must be 16-byte aligned");
   TORCH_CHECK(qdata.scalar_type() == at::kInt && qdata.dim() == 4 && qdata.size(2) == 32 && qdata.size(3) == 4, "ao_b200: qdata must be int32 [N/8, K/128, 32, 4] (inner_k_tiles=8)");
   TORCH_CHECK(scale_and_zero.scalar_type() == at::kBFloat16 && scale_and_zero.dim() == 3 && scale_and_zero.size(2) == 2, "ao_b200: scale_and_zero must be bf16 [K/g, N, 2]");
-  c10::cuda::CUDAGuard guard(x.device());
   const int64_t M = x.size(0), K = x.size(1);
   const int64_t N = qdata.size(0) * 8;
   TORCH_CHECK(qdata.size(1) * 128 == K, "ao_b200: x has K=", K, " but qdata encodes K=", qdata.size(1) * 128);
   TORCH_CHECK(scale_and_zero.size(0) * group_size == K && scale_and_zero.size(1) == N, "ao_b200: scale_and_zero shape does not match (K/g, N)");
-  if (n_out <= 0) n_out = N;
   TORCH_CHECK(n_out <= N, "ao_b200: n_out > N");
-  const uint16_t* bias_p = nullptr;
-  Tensor bias_c;
-  if (bias.has_value() && bias->defined()) {
-    bias_c = bias->to(at::kBFloat16).contiguous();
-    TORCH_CHECK(bias_c.numel() == n_out, "ao_b200: bias must have n_out elements");
-    bias_p = bf16_ptr(bias_c);
-  }
-  Tensor y = at::empty({M, n_out}, x.options());
-  if (M == 0) return y;
-  Tensor ws = workspace_for(x);
-  const int64_t ldx = M > 1 ? x.stride(0) : K;
-  AO_CALL(ao_int4_tilepacked_linear_strided(bf16_ptr(x), (int)ldx, (int)M, (int)K, qdata.data_ptr<int32_t>(), bf16_ptr(scale_and_zero), (int)group_size, (int)N, bias_p, bf16_ptr_mut(y), (int)n_out, ws.data_ptr(), (size_t)ws.numel(), (int)impl, cur_stream()));
-  return y;
+  Tensor y = int4_tilepacked_linear_meta(x, qdata, group_size, scale_and_zero, bias, n_out, impl);
+  return dense_linear(x, bias, y, [&](const void* xp, int ldx, const uint16_t* b, void* yp, void* ws, size_t ws_bytes) {
+    AO_CALL(ao_int4_tilepacked_linear_strided(static_cast<const uint16_t*>(xp), ldx, (int)M, (int)K, qdata.data_ptr<int32_t>(), bf16_ptr(scale_and_zero), (int)group_size, (int)N, b, static_cast<uint16_t*>(yp), (int)y.size(1), ws, ws_bytes, (int)impl, cur_stream()));
+  });
 }
 
 // torch._grouped_mm on 3-D int4 expert weights (2-D x 3-D): x bf16 [M, K], qdata int32 [E, N/8, K/128, 32, 4],
@@ -195,11 +222,6 @@ Tensor int4_unpack_tile4d_meta(const Tensor& qdata) {
 }
 Tensor int4_dequant_tile4d_meta(const Tensor& qdata, const Tensor& sz, int64_t) {
   return at::empty({qdata.size(0) * 8, qdata.size(1) * 128}, sz.options());
-}
-Tensor int4_tilepacked_linear_meta(const Tensor& x, const Tensor& qdata, int64_t, const Tensor&,
-                                   const c10::optional<Tensor>&, int64_t n_out, int64_t) {
-  if (n_out <= 0) n_out = qdata.size(0) * 8;
-  return at::empty({x.size(0), n_out}, x.options());
 }
 Tensor int4_tilepacked_grouped_mm_meta(const Tensor& x, const Tensor& qdata, int64_t, const Tensor&, const Tensor&,
                                        int64_t n_out) {

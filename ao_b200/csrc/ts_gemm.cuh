@@ -844,6 +844,35 @@ inline int run(Params& p, const CUtensorMap& tm_w, const CUtensorMap& tm_aux, co
   return launch_gemm<Fmt, Fmt::MAX_N_MMA>(p, tm_w, tm_aux, x, ldx, ws, ws_bytes, what, stream);
 }
 
+// The checks every dense linear shares, made once the caller has checked its format's K, N and group rules: x [M][ldx]
+// (byte codes pass ldx = K) into the output y [M][N_out].  Returns at M == 0 before any pointer is looked at; then x
+// and y must be set and x (named x_name in the message) start on 16 bytes, and p gets bias, y, M, N, N_out and K.
+inline int dense_params(Params& p, const char* what, const char* x_name, const void* x, int ldx, int M, int K, int N,
+                        int N_out, const uint16_t* bias, void* y) {
+  AO_REQUIRE(M >= 0 && K > 0 && N > 0, "%s: bad sizes M=%d K=%d N=%d", what, M, K, N);
+  AO_REQUIRE(ldx >= K && ldx % 8 == 0, "%s: ldx=%d must be >= K=%d and a multiple of 8", what, ldx, K);
+  if (M == 0) return AO_OK;
+  AO_REQUIRE(x && y, "%s: null pointer", what);
+  AO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "%s: %s must be 16-byte aligned", what, x_name);
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.M = M; p.N = N; p.N_out = N_out; p.K = K;
+  return AO_OK;
+}
+
+// Y = X * W^T for one dense linear: dense_params, then `setup(p, &tm_w, &tm_aux)` checks the format's own pointers,
+// sets its Params fields and builds its two maps, and the GEMM runs on x.
+template <class Fmt, class Setup>
+inline int run_dense(const char* what, const char* x_name, const void* x, int ldx, int M, int K, int N, int N_out,
+                     const uint16_t* bias, void* y, void* ws, size_t ws_bytes, void* stream, Setup setup) {
+  Params p{};
+  if (int rc = dense_params(p, what, x_name, x, ldx, M, K, N, N_out, bias, y)) return rc;
+  if (M == 0) return AO_OK;
+  CUtensorMap tm_w, tm_aux;
+  if (int rc = setup(p, &tm_w, &tm_aux)) return rc;
+  return run<Fmt>(p, tm_w, tm_aux, x, ldx, ws, ws_bytes, what, reinterpret_cast<cudaStream_t>(stream));
+}
+
 // torch._grouped_mm(x, W.transpose(-2, -1), offs), 2-D x 3-D, for every format: expert e's rows [offs[e-1], offs[e])
 // of x [M][K] (dense rows) against rows e*N .. e*N+N-1 of the weight map, into y [M][N_out] under Grouped<Fmt>.  The
 // caller has checked its format's K and N rules.  This checks what every grouped launch needs, returns at M == 0

@@ -146,7 +146,8 @@ int ao_int8_quantize_static(const uint16_t* x, int ldx, int M, int K, const void
                             int qmax, int8_t* q, float* x_scale, int8_t* x_zero_point, void* stream);
 /* Replaces _int_scaled_matmul + the epilogue (int8/kernels.py:114-144,
  * int8_tensor.py:305-359): y = bf16(bf16(acc_i32 * x_scale[m]) * w_scale[n] + bias[n]).
- * xq int8 [M,K], wq int8 [N,K] (K-major, i.e. the stored qdata), scales f32.         */
+ * xq int8 [M,K] (16-byte aligned), wq int8 [N,K] (K-major, i.e. the stored qdata), scales f32.  K % 16 == 0,
+ * N % 8 == 0. */
 int ao_int8_dyn_linear(const int8_t* xq, const float* x_scale, int M, int K,
                        const int8_t* wq, const float* w_scale, int N,
                        const uint16_t* bias, uint16_t* y, void* workspace,
@@ -198,7 +199,7 @@ int ao_int8_weight_grouped_mm(const uint16_t* x, int M, int K, const int8_t* wq,
 int ao_int8_dyn_grouped_mm(const int8_t* xq, const float* x_scale, int M, int K, const int8_t* wq,
                            const float* w_scale, int E, int N, const int32_t* offs, uint16_t* y, void* workspace,
                            size_t workspace_bytes, void* stream);
-/* int32 accumulator only (aten._int_mm equivalent; int8/kernels.py:18-76). */
+/* int32 accumulator only (aten._int_mm equivalent; int8/kernels.py:18-76).  xq 16-byte aligned, K % 16 == 0. */
 int ao_int8_mm_i32(const int8_t* xq, int M, int K, const int8_t* wq, int N, int32_t* acc,
                    void* workspace, size_t workspace_bytes, void* stream);
 
@@ -210,7 +211,8 @@ int ao_fp8_quantize_rowwise(const uint16_t* x, int M, int K, uint8_t* q, float* 
                             void* stream);
 /* Replaces torch._scaled_mm(a, b, scale_a, scale_b, bias, out_dtype=bf16)
  * (float8/inference.py:86-123 <- float8_tensor.py:449-457).
- * y = bf16( (Xq Wq^T)[m,n] * x_scale[m] * w_scale[n] + bias[n] ), f32 accumulate.     */
+ * y = bf16( (Xq Wq^T)[m,n] * x_scale[m] * w_scale[n] + bias[n] ), f32 accumulate.
+ * xq 16-byte aligned, K % 16 == 0, N % 16 == 0.                                       */
 int ao_fp8_rowwise_linear(const uint8_t* xq, const float* x_scale, int M, int K,
                           const uint8_t* wq, const float* w_scale, int N,
                           const uint16_t* bias, uint16_t* y, void* workspace,
@@ -310,7 +312,8 @@ int ao_fp8_blockwise_grouped_mm(const uint8_t* xq, const float* x_scale_t, int M
 int ao_mxfp8_quantize(const uint16_t* x, int M, int K, uint8_t* q, uint8_t* scale_e8m0,
                       int swizzled, void* stream);
 /* Replaces torch._scaled_mm(e4m3, e4m3, e8m0 blocked, e8m0 blocked, bias, bf16)
- * (mx_tensor.py:803-810).  Both scale tensors are in the blocked layout.              */
+ * (mx_tensor.py:803-810).  Both scale tensors are in the blocked layout.  xq 16-byte aligned,
+ * K % 32 == 0.                                                                        */
 int ao_mxfp8_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,
                     const uint8_t* wq, const uint8_t* w_scale_blocked, int N,
                     const uint16_t* bias, uint16_t* y, void* workspace,
@@ -326,7 +329,7 @@ int ao_mxfp4_quantize(const uint16_t* x, int M, int K, uint8_t* q, uint8_t* scal
                       int swizzled, void* stream);
 /* y = bf16( sum_k xhat[m,k] * what[n,k] (fp32) + bias ), xhat / what = each operand's code x 2^(e8-127), the
  * MXTensor.dequantize() of both (exact in bf16 for every scale byte: the products of the block-scaled fp4 MMA).
- * xq uint8 [M,K/2], wq uint8 [N,K/2], both scale tensors in the blocked layout with zero padding.  K % 32 == 0
+ * xq uint8 [M,K/2] (16-byte aligned), wq uint8 [N,K/2], both scale tensors in the blocked layout with zero padding.  K % 32 == 0
  * (a K tail of the last 128-k chunk is zero-filled), any N.                                                  */
 int ao_mxfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, int K,
                     const uint8_t* wq, const uint8_t* w_scale_blocked, int N,
@@ -340,7 +343,8 @@ int ao_mxfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, int M, in
 int ao_nvfp4_quantize(const uint16_t* x, int M, int K, const float* per_tensor_scale,
                       uint8_t* q, uint8_t* scale_e4m3, int swizzled, void* stream);
 /* Replaces torch._scaled_mm(fp4x2, fp4x2, e4m3 blocked scales) * (a_pts*b_pts) + bias
- * (nvfp4_tensor.py:487-578).  a_pts / b_pts: device f32 scalars or NULL (=1).          */
+ * (nvfp4_tensor.py:487-578).  a_pts / b_pts: device f32 scalars or NULL (=1).  xq 16-byte aligned,
+ * K % 256 == 0, N % 16 == 0.                                                          */
 int ao_nvfp4_linear(const uint8_t* xq, const uint8_t* x_scale_blocked, const float* a_pts,
                     int M, int K, const uint8_t* wq, const uint8_t* w_scale_blocked,
                     const float* b_pts, int N, const uint16_t* bias, uint16_t* y,

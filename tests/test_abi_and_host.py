@@ -45,6 +45,43 @@ def test_c_abi_argument_validation_without_gpu():
     assert lib.ao_int4_tilepacked_linear(None, 0, 1024, None, None, 32, 128, None, None, 128, None, ctypes.c_size_t(0), 0, None) == 0
 
 
+# Every dense linear's C entry point as fn(x, M, p): x the activation, M the rows, p every other pointer.  K = 4096 and
+# N = 256 pass every format's K and N rules.
+_K, _N = 4096, 256
+_WS = ctypes.c_size_t(1 << 20)
+_DENSE = {
+    "ao_int8_dyn_linear": ("xq", lambda x, M, p: (x, p, M, _K, p, p, _N, p, p, p, _WS, None)),
+    "ao_int8_mm_i32": ("xq", lambda x, M, p: (x, M, _K, p, _N, p, p, _WS, None)),
+    "ao_int8_weight_linear": ("x", lambda x, M, p: (x, _K, M, _K, p, p, _N, p, p, p, _WS, None)),
+    "ao_fp8_weight_linear": ("x", lambda x, M, p: (x, _K, M, _K, p, p, _N, p, p, p, _WS, None)),
+    "ao_fp8_rowwise_linear": ("xq", lambda x, M, p: (x, p, M, _K, p, p, _N, p, p, p, _WS, None)),
+    "ao_fp8_static_linear": ("xq", lambda x, M, p: (x, p, M, _K, p, p, 1, _N, p, p, 0, p, p, _WS, None)),
+    "ao_fp8_blockwise_linear": ("xq", lambda x, M, p: (x, p, M, _K, p, p, _N, p, p, p, _WS, None)),
+    "ao_fp8_sparse_linear": ("xq", lambda x, M, p: (x, p, M, _K, p, p, p, _N, p, p, p, _WS, None)),
+    "ao_mxfp8_linear": ("xq", lambda x, M, p: (x, p, M, _K, p, p, _N, p, p, p, _WS, None)),
+    "ao_mxfp4_linear": ("xq", lambda x, M, p: (x, p, M, _K, p, p, _N, p, p, p, _WS, None)),
+    "ao_nvfp4_linear": ("xq", lambda x, M, p: (x, p, p, M, _K, p, p, p, _N, p, p, p, _WS, None)),
+    "ao_nvfp4_weight_linear_ex": ("x", lambda x, M, p: (x, _K, p, M, _K, p, p, p, 0, _N, p, p, p, _WS, None)),
+    "ao_int4_tilepacked_linear_strided": ("x", lambda x, M, p: (x, _K, M, _K, p, p, 32, _N, p, p, _N, p, _WS, 0, None)),
+}
+
+
+@pytest.mark.parametrize("name", sorted(_DENSE))
+def test_dense_entry_points_check_the_activation_before_any_cuda_call(name):
+    """Every dense linear rejects an activation that does not start on 16 bytes with a message (the kernels read it by
+    TMA or by 16-byte vector loads) and returns 0 at M == 0 without looking at a pointer.  No GPU: a CUDA call would
+    fail with a different error."""
+    lib = ctypes.CDLL(os.path.join(ROOT, "ao_b200", "lib", "libao_b200.so"))
+    lib.ao_b200_last_error.restype = ctypes.c_char_p
+    x_name, args = _DENSE[name]
+    fn = getattr(lib, name)
+    one = ctypes.c_void_p(4096)
+    assert fn(*args(ctypes.c_void_p(4104), 4, one)) == -1
+    assert f"{x_name} must be 16-byte aligned".encode() in lib.ao_b200_last_error(), lib.ao_b200_last_error()
+    assert fn(*args(None, 4, one)) == -1 and b"null pointer" in lib.ao_b200_last_error()
+    assert fn(*args(None, 0, None)) == 0
+
+
 def test_pdl_fence_on_the_null_stream():
     """ao_b200_pdl_fence(NULL) launches its empty kernel on the legacy default stream; without a device it reports the
     failed launch instead of crashing.  torch.ops.ao_b200.pdl_fence is its registration."""
