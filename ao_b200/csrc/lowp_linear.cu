@@ -13,6 +13,7 @@
 //                         and, per expert, the same on select()ed int8 expert weights
 //   e4m3 weight x bf16    (bf16 wgmma, weights dequantised per element)  replaces torch.matmul on the dequantised weight
 //                         and, per expert, torch._grouped_mm on the dequantised expert weights
+//   nf4 weight x bf16     (bf16 wgmma, weights dequantised per element)  replaces F.linear on get_original_weight()
 // Reference call sites: int8/kernels.py:18-76,114-144 + int8_tensor.py:305-359;
 // float8/inference.py:86-123; mx_formats/mx_tensor.py:759-843; nvfp4_tensor.py:487-578.
 //
@@ -495,6 +496,12 @@ struct Mxfp4Fmt {
     uint32_t c[2][4];
     uint32_t s[2][2];
   };
+  // Raw::c[h][j] of row r from the 64-byte-swizzled stage (the byte selector sel of thread t, see load)
+  __device__ static __forceinline__ uint32_t lds_codes(uint32_t w_smem, int r, int j, uint32_t sel) {
+    const uint32_t off = (uint32_t)r * 64u + j * 16;
+    const uint4 v = tsg::lds128(w_smem + (off ^ (((off >> 7) & 3) << 4)));   // undo the TMA 64B swizzle
+    return __byte_perm(__byte_perm(v.x, v.y, sel), __byte_perm(v.z, v.w, sel), 0x5410);
+  }
   __device__ static __forceinline__ void load(const tsg::Params&, uint32_t w_smem, uint32_t aux_smem, int row_lo, int lane,
                                               Raw& raw) {
     const uint32_t t = lane & 3;
@@ -510,11 +517,7 @@ struct Mxfp4Fmt {
         raw.s[h][i] = *reinterpret_cast<const uint32_t*>(&s2);
       }
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint32_t off = (uint32_t)r * 64u + j * 16;
-        const uint4 v = tsg::lds128(w_smem + (off ^ (((off >> 7) & 3) << 4)));   // undo the TMA 64B swizzle
-        raw.c[h][j] = __byte_perm(__byte_perm(v.x, v.y, sel), __byte_perm(v.z, v.w, sel), 0x5410);
-      }
+      for (int j = 0; j < 4; ++j) raw.c[h][j] = lds_codes(w_smem, r, j, sel);
     }
   }
   __device__ static __forceinline__ uint32_t deq(uint32_t byte, __nv_bfloat162 s2) {
@@ -678,6 +681,168 @@ struct Fp8WoFmt {
   }
 };
 
+// NF4 weights x bf16 activations (NF4Tensor, QLoRA; reference nf4_tensor.py get_original_weight and LinearNF4): the
+// stored codes [N*K/2] viewed as [N, K/2] bytes (even k in the high nibble) in the stage and map of Mxfp4Fmt, and per
+// flat block b = (n*K + k) / block_size the double-quantized scaler
+//   s[b] = bf16(bf16(qs[b] / f[b / sbs]) + mean),  w~[n,k] = bf16(nf4[code] * s[b])
+// with qs int8, f, mean and the 16-entry table nf4 bf16 tensors of the weight.  The scalers are decoded in the GEMM, by
+// the aux fillers of ts_gemm.cuh (AUX_FILL): one chunk's scaler bytes are 2 per row at block_size 64, under TMA's
+// 16-byte box minimum, and their row pitch K / block_size is a multiple of 16 bytes only when K % 1024 == 0.  A filler
+// warp reads them with ordinary loads (each block once), divides as torch does (IEEE division, then a separate add) and
+// writes one bf16 scaler per (row, k16 step) into the stage's aux slot, with the table behind them.
+// Conversion: the four codes of a thread's 16-bit code word select their table entries with byte permutes, the low and
+// the high bytes of the bf16 values separately (entries 0..7 and 8..15, then bit 3 of the code picks one), and one bf16x2
+// multiply by the step's scaler rounds each element once, as torch's bf16 multiply does.  Every bf16 x w~ product is exact
+// in fp32, and the epilogue (EPI_BF16) rounds the sum to bf16 and adds the bias in bf16, as F.linear and `+ bias` do.
+// Params: the fields its EPI_BF16 epilogue never reads carry the NF4 tensors, so Params (and the code of every other
+// kernel) stays as it is: row_scale = quantized_scalers (int8), out_scale = quantization_factor (bf16), out_scale2 =
+// scaler_mean (bf16), w_scale = nf4 (bf16), group_size = block_size, aux_col_blocks = scaler_block_size.
+// Shapes: block_size % 16 == 0 (a k16 step lies in one block), K % block_size == 0 (no block spans two rows; then every
+// row has its block boundaries at the same k), K % 32 == 0 (the TMA row pitch of the codes), any N.
+struct Nf4Fmt {
+  static constexpr bool SS = false;
+  // one CTA per SM: the aux fillers hold a chunk's loads in registers (ts_gemm.cuh, AuxFill)
+  static constexpr bool DECODE_2CTA = false;
+  static constexpr bool PROMOTE = false;
+  static constexpr bool AUX_FILL = true;
+  static constexpr int X_ELEM_BYTES = 2;
+  static constexpr int W_BYTES = ROWS * KCHUNK / 2;   // 128 rows x 64 bytes, 64-byte swizzle
+  // the scalers [128 rows][8 k16 steps] bf16, then the table as byte planes: words 0..3 the low bytes of entries 0..15,
+  // words 4..7 their high bytes
+  static constexpr int LUT_OFF = ROWS * 16;
+  static constexpr int AUX_BYTES = LUT_OFF + 32;
+  static constexpr int EPI = tsg::EPI_BF16;
+  static constexpr int ACC_EXP2 = 0;
+  static constexpr int MAX_N_MMA = 128;
+  // no aux map: the weight map stands in for it (the aux slot is written by the fillers)
+  static int make_maps(const uint8_t* qdata, int N, int K, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    const uint64_t dims[2] = {(uint64_t)K / 2, (uint64_t)N};
+    const uint64_t str[1] = {(uint64_t)K / 2};
+    const uint32_t box[2] = {64, 128};
+    if (int rc = make_tmap(tm_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, qdata, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B))
+      return rc;
+    *tm_aux = *tm_w;
+    return AO_OK;
+  }
+  __device__ static __forceinline__ uint32_t w_tx_bytes(const tsg::Params&) { return W_BYTES; }
+  __device__ static __forceinline__ void issue_w(const CUtensorMap* tm_w, const CUtensorMap*, const tsg::Params&,
+                                                 uint8_t* w_dst, uint8_t*, uint64_t* bar, int n_tile, int kc,
+                                                 uint64_t policy) {
+    tma_load_2d(w_dst, tm_w, bar, kc * 64, n_tile * ROWS, policy);
+  }
+  // the reference's dequantize_scalers: an int8 / bf16 division rounded to bf16, then a bf16 add of the mean
+  __device__ static __forceinline__ uint32_t scaler_bits(int8_t q, __nv_bfloat16 f, float mean) {
+    const float d = __bfloat162float(__float2bfloat16_rn(__fdiv_rn((float)q, __bfloat162float(f))));
+    return __bfloat16_as_ushort(__float2bfloat16_rn(__fadd_rn(d, mean)));
+  }
+  // one warp: the aux slot of chunk kc of tile n_tile; lane l writes rows l, l + 32, l + 64, l + 96
+  __device__ static __forceinline__ void fill_aux(const tsg::Params& p, uint8_t* aux, int n_tile, int kc, int lane) {
+    const int bs = p.group_size, k0 = kc * KCHUNK;
+    const uint32_t per_row = (uint32_t)(p.K / bs), o0 = (uint32_t)(k0 / bs), sbs = (uint32_t)p.aux_col_blocks;
+    // step kk lies in block o0 + ob[kk] of its row and starts a block (fresh) at kk == 0 and where k0 + 16kk is a
+    // multiple of bs.  Steps past K get the scaler 0: their codes are TMA zero fill (code 0 = -1), and a 0 keeps them
+    // out of the sums even in a row whose scalers are inf or NaN
+    int ob[8];
+    bool fresh[8], in_k[8];
+    {
+      int o = 0, pos = k0 - (int)o0 * bs;
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        if (kk > 0 && (pos += 16) == bs) {
+          pos = 0;
+          ++o;
+        }
+        ob[kk] = o;
+        fresh[kk] = kk == 0 || pos == 0;
+        in_k[kk] = k0 + 16 * kk < p.K;
+      }
+    }
+    // every load of the chunk first (each block once), then the arithmetic
+    int8_t q[4][8];
+    __nv_bfloat16 f[4][8];
+#pragma unroll
+    for (int rr = 0; rr < 4; ++rr) {
+      const int n = n_tile * ROWS + lane + 32 * rr;
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        q[rr][kk] = 0;
+        f[rr][kk] = __ushort_as_bfloat16(0x3F80);
+        if (fresh[kk] && in_k[kk] && n < p.N) {
+          const uint32_t b = (uint32_t)n * per_row + o0 + ob[kk];
+          q[rr][kk] = reinterpret_cast<const int8_t*>(p.row_scale)[b];
+          f[rr][kk] = reinterpret_cast<const __nv_bfloat16*>(p.out_scale)[b / sbs];
+        }
+      }
+    }
+    const float mean = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(p.out_scale2));
+#pragma unroll
+    for (int rr = 0; rr < 4; ++rr) {
+      const int r = lane + 32 * rr;
+      const bool row_ok = n_tile * ROWS + r < p.N;
+      uint32_t w[4] = {0u, 0u, 0u, 0u}, s = 0u;
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        if (fresh[kk]) s = in_k[kk] && row_ok ? scaler_bits(q[rr][kk], f[rr][kk], mean) : 0u;
+        w[kk >> 1] |= s << (16 * (kk & 1));
+      }
+      *reinterpret_cast<uint4*>(aux + r * 16) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    if (lane < 8) {
+      const uint16_t* e = reinterpret_cast<const uint16_t*>(p.w_scale) + 4 * (lane & 3);
+      const uint32_t lo = e[0] | (uint32_t)e[1] << 16, hi = e[2] | (uint32_t)e[3] << 16;
+      *reinterpret_cast<uint32_t*>(aux + LUT_OFF + 4 * lane) = __byte_perm(lo, hi, lane < 4 ? 0x6420 : 0x7531);
+    }
+  }
+  // c: the code words of Mxfp4Fmt::Raw (the same bytes; here the even k is the high nibble); s[h][i]: the bf16 scalers
+  // of row h's steps 2i, 2i + 1; lut: the table's byte planes
+  struct Raw {
+    uint32_t c[2][4];
+    uint32_t s[2][4];
+    uint32_t lut[8];
+  };
+  __device__ static __forceinline__ void load(const tsg::Params&, uint32_t w_smem, uint32_t aux_smem, int row_lo, int lane,
+                                              Raw& raw) {
+    const uint32_t t = lane & 3;
+    const uint32_t sel = t | (t + 4) << 4 | t << 8 | (t + 4) << 12;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row_lo + 8 * h;
+      const uint4 sv = tsg::lds128(aux_smem + (uint32_t)r * 16u);
+      raw.s[h][0] = sv.x;
+      raw.s[h][1] = sv.y;
+      raw.s[h][2] = sv.z;
+      raw.s[h][3] = sv.w;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) raw.c[h][j] = Mxfp4Fmt::lds_codes(w_smem, r, j, sel);
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const uint4 l = tsg::lds128(aux_smem + LUT_OFF + 16 * i);
+      raw.lut[4 * i] = l.x;
+      raw.lut[4 * i + 1] = l.y;
+      raw.lut[4 * i + 2] = l.z;
+      raw.lut[4 * i + 3] = l.w;
+    }
+  }
+  __device__ static __forceinline__ void frag(const tsg::Params&, const Raw& raw, int kk, uint32_t (&a)[4]) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t s_bits = __byte_perm(raw.s[h][kk >> 1], 0u, (kk & 1) ? 0x3232u : 0x1010u);
+      const __nv_bfloat162 s2 = *reinterpret_cast<const __nv_bfloat162*>(&s_bits);
+      // nibbles 0..3: the odd and the even k of the pair 16kk + 2t, then of the pair 8 further
+      const uint32_t w = raw.c[h][kk >> 1] >> (16 * (kk & 1));
+      const uint32_t sel7 = w & 0x7777u, pick = ((w >> 1) & 0x4444u) | 0x3210u;
+      const uint32_t lo = __byte_perm(__byte_perm(raw.lut[0], raw.lut[1], sel7), __byte_perm(raw.lut[2], raw.lut[3], sel7), pick);
+      const uint32_t hi = __byte_perm(__byte_perm(raw.lut[4], raw.lut[5], sel7), __byte_perm(raw.lut[6], raw.lut[7], sel7), pick);
+      const uint32_t v0 = __byte_perm(lo, hi, 0x4051), v1 = __byte_perm(lo, hi, 0x6273);
+      const __nv_bfloat162 d0 = __hmul2(*reinterpret_cast<const __nv_bfloat162*>(&v0), s2);
+      const __nv_bfloat162 d1 = __hmul2(*reinterpret_cast<const __nv_bfloat162*>(&v1), s2);
+      a[h] = *reinterpret_cast<const uint32_t*>(&d0);
+      a[h + 2] = *reinterpret_cast<const uint32_t*>(&d1);
+    }
+  }
+};
+
 // Activation pre-pass of the block-scaled kinds: rows [m0, m0 + rows) of the quantised activations -> bf16 [rows][K],
 // every element times its block scale (exact in bf16).  One thread per 16 elements.
 template <int KIND>
@@ -830,6 +995,36 @@ extern "C" int ao_fp8_weight_linear(const uint16_t* x, int ldx, int M, int K, co
     AO_REQUIRE((reinterpret_cast<uintptr_t>(w_scale) & 15) == 0,
                "fp8 weight linear: w_scale must be 16-byte aligned (it is loaded by TMA)");
     return Fmt::make_maps(wq, w_scale, N, K, tm_w, tm_s);
+  });
+}
+
+// F.linear(x, NF4Tensor) (nf4_tensor.py LinearNF4 and the F.linear override): y = bf16(bf16(sum_k x[m,k] * w~[n,k]) +
+// bias[n]), w~ = the reference's get_original_weight(); one launch, the scalers decoded in the kernel (Nf4Fmt)
+extern "C" int ao_nf4_linear(const uint16_t* x, int ldx, int M, int K, const uint8_t* quantized_data,
+                             const int8_t* quantized_scalers, const uint16_t* quantization_factor,
+                             const uint16_t* scaler_mean, const uint16_t* nf4, int block_size, int scaler_block_size,
+                             int N, const uint16_t* bias, uint16_t* y, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+  AO_REQUIRE(block_size > 0 && block_size % 16 == 0, "nf4 linear: block_size=%d must be a positive multiple of 16",
+             block_size);
+  AO_REQUIRE(K % block_size == 0, "nf4 linear: K=%d must be a multiple of block_size=%d", K, block_size);
+  AO_REQUIRE(K % 32 == 0, "nf4 linear: K=%d must be a multiple of 32 (TMA row pitch of the codes)", K);
+  const long long n_blocks = N > 0 ? (long long)N * (K / block_size) : 0;
+  AO_REQUIRE(n_blocks <= 0x7FFFFFFF, "nf4 linear: N*K/block_size=%lld scalers exceed the int32 range", n_blocks);
+  AO_REQUIRE(scaler_block_size > 0 && n_blocks % scaler_block_size == 0,
+             "nf4 linear: scaler_block_size=%d must divide the %lld scalers", scaler_block_size, n_blocks);
+  using Fmt = lowp::Nf4Fmt;
+  return tsg::run_dense<Fmt>("nf4 linear", "x", x, ldx, M, K, N, N, bias, y, workspace, workspace_bytes, stream,
+                             [&](tsg::Params& p, CUtensorMap* tm_w, CUtensorMap* tm_aux) {
+    AO_REQUIRE(quantized_data && quantized_scalers && quantization_factor && scaler_mean && nf4,
+               "nf4 linear: null pointer");
+    p.row_scale = reinterpret_cast<const float*>(quantized_scalers);   // the fields of Nf4Fmt (see there)
+    p.out_scale = reinterpret_cast<const float*>(quantization_factor);
+    p.out_scale2 = reinterpret_cast<const float*>(scaler_mean);
+    p.w_scale = reinterpret_cast<const float*>(nf4);
+    p.group_size = block_size;
+    p.aux_col_blocks = scaler_block_size;
+    return Fmt::make_maps(quantized_data, N, K, tm_w, tm_aux);
   });
 }
 

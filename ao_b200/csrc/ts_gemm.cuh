@@ -4,7 +4,7 @@
 //
 // Swap-AB: 128 weight rows of a tile are the wgmma M dimension (two consumer warpgroups of 64 rows each), the tokens
 // are the wgmma N dimension (N_MMA = 16..128).  A format policy (Fmt) decides how the weights reach the tensor core:
-//   * register-A (Fmt::SS == false): int4 tinygemm, nvfp4, mxfp8, mxfp4, int8 and fp8 weight-only.  Each consumer thread loads the packed
+//   * register-A (Fmt::SS == false): int4 tinygemm, nvfp4, mxfp8, mxfp4, int8, fp8 and nf4 weight-only.  Each consumer thread loads the packed
 //     weights of its two fragment rows straight from the TMA-filled stage and dequantises them into the bf16 A
 //     fragment of wgmma.m64nNk16 (4 x bf16x2 per k16 step); the activations (bf16) are the shared-memory B operand
 //   * shared-memory A (Fmt::SS == true): int8 x int8 -> s32 and e4m3 x e4m3 -> f32 (wgmma k32), both operands are
@@ -102,6 +102,20 @@ struct WXpose {
 template <class F>
 struct WXpose<F, std::void_t<decltype(F::W_XPOSE_BYTES)>> {
   static constexpr int BYTES = F::W_XPOSE_BYTES;
+};
+
+// Fmt::AUX_FILL (optional, default false): a register-A format whose aux slot is not loaded by TMA but written by
+// warps 1..3 of the producer warpgroup, which the other formats leave idle.  Unit i belongs to warp 1 + i % 3: it waits
+// for the stage as the producer does, runs Fmt::fill_aux(p, aux smem, n_tile, kc, lane) on all 32 lanes and arrives on
+// the stage's wfull, which then expects two arrivals (the producer's with the weight bytes, and this one).  Three warps
+// keep three stages' global loads in flight, and the weight TMAs never wait for them
+template <class F, class = void>
+struct AuxFill {
+  static constexpr bool value = false;
+};
+template <class F>
+struct AuxFill<F, std::void_t<decltype(F::AUX_FILL)>> {
+  static constexpr bool value = F::AUX_FILL;
 };
 
 template <class Fmt, int N_MMA>
@@ -245,6 +259,8 @@ struct Cfg {
   // the owner's gather stages up to STAGES contributors' partials in the ring (see the producer) when one fits a stage;
   // not for PROMOTE (e4m3 x e4m3): its bs=32 decode stack measured 5 % slower with it (DESIGN §4)
   static constexpr bool STAGE_PARTIALS = !Fmt::PROMOTE && N_MMA * ROWS * 4 <= STAGE_BYTES;
+  // the aux fillers keep a stage's loads in registers: they run at the kernel's register count, not PRODUCER_REGS
+  static_assert(!AuxFill<Fmt>::value || CTAS == 1, "AUX_FILL formats run one CTA per SM");
 };
 
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
@@ -349,7 +365,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < S; ++i) {
-      mbar_init(&wfull[i], 1);
+      mbar_init(&wfull[i], AuxFill<Fmt>::value ? 2 : 1);
       mbar_init(&xfull[i], 1);
       mbar_init(&sempty[i], CONSUMER_WARPS);
     }
@@ -368,6 +384,19 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
 
   if (wgi == 0) {
     if constexpr (C::CTAS > 1) setmaxnreg_dec<PRODUCER_REGS>();   // all four warps, before three of them leave
+    if constexpr (AuxFill<Fmt>::value) {
+      if (warp != 0) {
+        // the aux fillers (see AuxFill): their stores, then the warp barrier, then one arrival on the stage
+        for (int i = warp - 1; i < nunits; i += 3) {
+          const int s = i % S;
+          if (i >= S) mbar_wait(&sempty[s], ((i / S) & 1) ^ 1);
+          Fmt::fill_aux(p, stage(s) + Fmt::W_BYTES, tile_of(i) % p.n_tiles, kc_of(i), lane);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&wfull[s]);
+        }
+        goto done;
+      }
+    }
     if (warp != 0) goto done;
     // ------------------------------------------------------------ TMA producer
     const uint64_t pol_w = policy_evict_first();
@@ -441,6 +470,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           fence_proxy_async_global();   // the contributor's st.cg stores, acquired above, before the bulk reads
           mbar_expect_tx(&wfull[s], cols * ROWS * 4);
           bulk_load(stage(s), p.ws_partial + (size_t)(b + 1 + lane) * (N_MMA * ROWS), cols * ROWS * 4, &wfull[s]);
+          if constexpr (AuxFill<Fmt>::value) mbar_arrive(&wfull[s]);   // the arrival no filler makes for this stage
         }
         __syncwarp();
       }

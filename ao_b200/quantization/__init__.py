@@ -4,7 +4,8 @@ from .quant_primitives import MappingType  # noqa: F401
 from .quantize_.common import KernelPreference  # noqa: F401
 from .quantize_.workflows import (  # noqa: F401
     Float8PackingFormat, Float8Sparse2x4_2DData2DMetadataTensor, Float8Tensor, Int4ChooseQParamsAlgorithm,
-    Int4PackingFormat, Int4TilePackedTo4dTensor, Int8Tensor, QuantizeTensorToFloat8Kwargs, QuantizeTensorToInt8Kwargs)
+    Int4PackingFormat, Int4TilePackedTo4dTensor, Int8Tensor, NF4Tensor, QuantizeTensorToFloat8Kwargs,
+    QuantizeTensorToInt8Kwargs, to_nf4)
 from .quant_api import (  # noqa: F401
     Float8DynamicActivationFloat8WeightConfig, Float8WeightOnlyConfig, FqnToConfig, Int4WeightOnlyConfig,
     Int8DynamicActivationInt8WeightConfig, Int8StaticActivationInt8WeightConfig, Int8WeightOnlyConfig, ModuleFqnToConfig,

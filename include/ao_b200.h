@@ -167,6 +167,19 @@ int ao_int8_weight_linear(const uint16_t* x, int ldx, int M, int K, const int8_t
 int ao_fp8_weight_linear(const uint16_t* x, int ldx, int M, int K, const uint8_t* wq, const float* w_scale,
                          int N, const uint16_t* bias, uint16_t* y, void* workspace,
                          size_t workspace_bytes, void* stream);
+/* NF4 (QLoRA) weight-only: bf16 activations on the stored NF4Tensor of a bf16 weight [N, K].  Replaces
+ * F.linear(x, W.get_original_weight()) + bias (nf4_tensor.py) with the same roundings: per flat block
+ * b = (n*K + k) / block_size the scaler s[b] = bf16(bf16(quantized_scalers[b] / quantization_factor[b / scaler_block_size])
+ * + scaler_mean), each weight w~ = bf16(nf4[code] * s[b]), y = bf16(bf16(sum_k x[m,k] * w~[n,k]) + bias[n]); no add
+ * without a bias.  x bf16 [M][ldx] (ldx >= K, ldx % 8 == 0, 16-byte aligned); quantized_data uint8 [N*K/2] (codes of
+ * the row-major weight, even element in the high nibble, 16-byte aligned); quantized_scalers int8 [N*K/block_size];
+ * quantization_factor bf16 [N*K/(block_size*scaler_block_size)]; scaler_mean bf16 (one value); nf4 bf16 [16].
+ * block_size % 16 == 0, K % block_size == 0, K % 32 == 0, N*K/block_size a multiple of scaler_block_size and at most
+ * 2^31 - 1; any N. */
+int ao_nf4_linear(const uint16_t* x, int ldx, int M, int K, const uint8_t* quantized_data,
+                  const int8_t* quantized_scalers, const uint16_t* quantization_factor, const uint16_t* scaler_mean,
+                  const uint16_t* nf4, int block_size, int scaler_block_size, int N, const uint16_t* bias, uint16_t* y,
+                  void* workspace, size_t workspace_bytes, void* stream);
 /* torch._grouped_mm(x, W.transpose(-2, -1), offs) for a 3-D weight-only Float8Tensor expert weight W [E, N, K],
  * 2-D x 3-D form (float8_tensor.py:1085-1122, weight-only branch: torch._grouped_mm on W.dequantize()): for
  * offs[e-1] <= m < offs[e] (offs[-1] = 0)
