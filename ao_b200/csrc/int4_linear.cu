@@ -121,11 +121,10 @@ struct Int4Fmt {
     const int wd = kk >> 1, e0 = 2 * (kk & 1);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const uint32_t sz = raw.sz[h][wd];
-      const uint32_t s_bits = __byte_perm(sz, sz, 0x1010);
-      const uint32_t z_bits = __byte_perm(sz, sz, 0x3232);
-      const __nv_bfloat162 s2 = *reinterpret_cast<const __nv_bfloat162*>(&s_bits);
-      const __nv_bfloat162 z2 = *reinterpret_cast<const __nv_bfloat162*>(&z_bits);
+      const __nv_bfloat162 sz2 = *reinterpret_cast<const __nv_bfloat162*>(&raw.sz[h][wd]);
+      // s and z broadcast to both halves: ptxas folds the broadcasts into HFMA2 operand selectors (.H0_H0 / .H1_H1),
+      // where byte permutes cost two instructions per word
+      const __nv_bfloat162 s2 = __low2bfloat162(sz2), z2 = __high2bfloat162(sz2);
       const uint32_t word = wd == 0 ? raw.v[h].x : wd == 1 ? raw.v[h].y : wd == 2 ? raw.v[h].z : raw.v[h].w;
 #pragma unroll
       for (int e = 0; e < 2; ++e) {

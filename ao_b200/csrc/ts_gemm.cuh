@@ -683,6 +683,9 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       }
     };
 
+    // the ring's shared-memory address, converted once: converting a stage's generic pointer in the chunk loop costs
+    // a dozen uniform instructions per chunk
+    const uint32_t ring_s = smem_u32(smem);
     int i = 0;
     for (int seg = 0; seg < walk.nseg; ++seg) {
       const int cnt = walk.seg_count(seg);
@@ -698,8 +701,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         const uint32_t scale_d = c > 0;   // the first wgmma of a segment overwrites the accumulator
         const int s = i % S;
         const uint32_t ph = (i / S) & 1;
-        uint8_t* st = stage(s);
-        const uint32_t w_s = smem_u32(st), aux_s = w_s + Fmt::W_BYTES, x_s = aux_s + C::AUX_SLOT;
+        const uint32_t w_s = ring_s + s * C::STAGE_BYTES, aux_s = w_s + Fmt::W_BYTES, x_s = aux_s + C::AUX_SLOT;
         mbar_wait(&wfull[s], ph);
         if constexpr (Fmt::PROMOTE) {
           // e4m3: a chain of wgmmas accumulates in the tensor core's reduced-precision adder; each chunk's four k32
@@ -769,6 +771,7 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           // two halves: the wgmmas of k16 steps 0..3 run while steps 4..7 are dequantised (same wgmmas, same order)
 #pragma unroll
           for (int kk = 0; kk < 4; ++kk) Fmt::frag(p, raw, kk, a[kk]);
+          const uint64_t x_desc = wgmma_desc_k_sw128(x_s);
           mbar_wait(&xfull[s], ph);
           wgmma_fence_operand(acc);
 #pragma unroll
@@ -783,8 +786,10 @@ ts_gemm_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
             wgmma_fence();   // orders the fragment registers just written before the wgmmas that read them
 #pragma unroll
             for (int kk = 4 * half; kk < 4 * half + 4; ++kk) {
-              // k16 step kk of the bf16 B tile: atom kk / 4 (64 k each), 32 bytes per step inside the 128-byte row
-              const uint64_t bd = wgmma_desc_k_sw128(x_s + (kk >> 2) * (N_MMA * 128) + (kk & 3) * 32);
+              // k16 step kk of the bf16 B tile: atom kk / 4 (64 k each), 32 bytes per step inside the 128-byte row.
+              // The step's byte offset goes straight into the start-address field (16-byte units) of the chunk's
+              // descriptor: shared addresses stay below 2^18 bytes, so the 14-bit field never carries
+              const uint64_t bd = x_desc + (uint32_t)(((kk >> 2) * (N_MMA * 128) + (kk & 3) * 32) >> 4);
               MMA::ra_bf16(acc, a[kk], bd, kk == 0 ? scale_d : 1u);
             }
           }
